@@ -117,7 +117,9 @@ RX_API int rx_set_particles(rx_engine *h, const double *sigma, const double *eps
                      const uint8_t *alchemical_mask);
 RX_API int rx_set_states(rx_engine *h, const rx_state_params *states /* [n_states] */);
 /* RX_SYSTEM_MOLECULE: the particles and the force field at once (instead of rx_set_particles).
- * Replaces: the System built by AmberPrmtopFile.createSystem for AlanineDipeptideVacuum, testsystems.py:3375-3388. */
+ * Replaces: the System built by AmberPrmtopFile.createSystem for AlanineDipeptideVacuum, testsystems.py:3375-3388.
+ * RX_ERR_UNSUPPORTED (and no molecule set) when the term tables need more shared memory than a block of the device can
+ * have (each torsion term takes 236 bytes of the 227 KB of an H100 block: decane with three terms per torsion needs 95 KB); a refused call leaves the engine without a molecule. */
 RX_API int rx_set_molecule(rx_engine *h, const rx_molecule *molecule);
 /* LangevinSplittingDynamicsMove parameters (mcmc.py:1280-1291) / LangevinIntegrator (integrators.py:1071-1158):
  * timestep (ps), collision_rate (1/ps), n_steps, splitting with the spaces removed, e.g. "VRORV".        */

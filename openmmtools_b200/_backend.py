@@ -171,6 +171,8 @@ def build_engine(thermodynamic_states, n_replicas, device=0, rank=0, world_size=
                      softcore_c=sys0.softcore_c)
         eng.set_particles(sys0.sigma, sys0.epsilon, sys0.masses, sys0.alchemical_mask())
     elif sys0.kind == MOLECULE:
+        if N > 32:
+            raise NotImplementedError('molecules above 32 atoms are not provided (one lane per atom): %d atoms' % N)
         eng = Engine(_lib.RX_SYSTEM_MOLECULE, n_replicas, M, N, device=device, rank=rank, world_size=world_size)
         eng.set_molecule(sys0)
     else:

@@ -710,6 +710,16 @@ int rxi_convert_out(rx_engine *h, const float4 *src, int first_local, int count,
 
 #include "rx_molecule.cuh"
 
+// A block may take 48 KB of shared memory, static and dynamic together, unless the kernel has opted in to more (up to
+// cudaDevAttrMaxSharedMemoryPerBlockOptin, which rxi_set_molecule checks).  The molecule's tables grow with its terms.
+static int mol_smem_optin(rx_engine *h, const void *kern, int dyn) {
+    cudaFuncAttributes fa;
+    RX_CHECK_CUDA(h, cudaFuncGetAttributes(&fa, kern));
+    if (fa.sharedSizeBytes + (size_t)dyn > 48 * 1024)
+        RX_CHECK_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
+    return RX_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------
 static int fill_dyn(rx_engine *h, DynParams &p) {
     const rx_config &c = h->cfg;
@@ -768,6 +778,8 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         const MolDev *md = (const MolDev *)h->mol_dev;
         const bool no_star = getenv("RX_MOL_NO_STAR") != nullptr;   // cross-check: the general cluster path for every molecule
         auto kern = (md->max_cluster <= 3 && !no_star) ? k_propagate_mol<true> : k_propagate_mol<false>;
+        const int rco = mol_smem_optin(h, (const void *)kern, md->dyn_shared_bytes);
+        if (rco) return rco;
         kern<<<h->kloc, 32 * MOL_WARPS, md->dyn_shared_bytes, h->stream>>>(*md, p, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
                                                                            (double *)h->d_vel, h->k0, mkey, (uint32_t)iteration, reassign, h->d_pot,
                                                                            h->d_kin, h->d_nan, d_only);
@@ -993,6 +1005,8 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
     if (h->kloc == 0) return RX_OK;
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
         const MolDev *m = (const MolDev *)h->mol_dev;
+        const int rco = mol_smem_optin(h, (const void *)k_minimize_mol, m->shared_bytes);
+        if (rco) return rco;
         k_minimize_mol<<<h->kloc, 32, m->shared_bytes, h->stream>>>(*m, (double *)h->d_pos, h->k0, tolerance,
                                                                    max_iterations > 0 ? max_iterations : 100000, d_rms, d_iters);
         RX_CHECK_CUDA(h, cudaGetLastError());
@@ -1037,6 +1051,8 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     if (h->kloc == 0) return RX_OK;
     const rx_config &c = h->cfg;
     if (c.system_kind == RX_SYSTEM_MOLECULE) {
+        const int rco = mol_smem_optin(h, (const void *)k_energy_mol, ((const MolDev *)h->mol_dev)->shared_bytes);
+        if (rco) return rco;
         k_energy_mol<<<h->kloc, 32, ((const MolDev *)h->mol_dev)->shared_bytes, h->stream>>>(*(const MolDev *)h->mol_dev, d_states, n_states, (const double *)h->d_pos, h->k0, d_out);
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
@@ -1086,8 +1102,8 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
     if (n > MOL_MAX_ATOMS) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_molecule: more than 32 atoms per molecule is not provided");
     if (!mol->mass || !mol->charge || !mol->sigma || !mol->epsilon) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: null per-atom arrays");
     auto atom_ok = [&](double v) { return v >= 0 && v < n && v == floor(v); };
-    for (void *d : h->mol_allocs) cudaFree(d);
-    h->mol_allocs.clear();
+    rxi_free_molecule(h);         // (a refused molecule leaves the engine without one, not with freed tables)
+    h->have_particles = false;
     std::vector<double> mass(mol->mass, mol->mass + n), charge(mol->charge, mol->charge + n), sigma(mol->sigma, mol->sigma + n),
         eps(mol->epsilon, mol->epsilon + n);
     for (int i = 0; i < n; i++)
@@ -1246,6 +1262,30 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
         m->terms_bytes = (int)off;
         m->n_tb = (int)tb.size(); m->n_ta = (int)tang.size(); m->n_tt = (int)tt.size(); m->n_tp = (int)tp.size(); m->n_slots = slot;
         m->dyn_shared_bytes = m->shared_bytes + (int)up(off) + (int)up(sizeof(float) * 3 * (size_t)(slot > 0 ? slot : 1));
+    }
+    // What no block can hold is refused here rather than at launch (which opts in above 48 KB: mol_smem_optin).  The slot
+    // indices of the term tables are shorts; tables that fit in shared memory have far fewer slots, checked all the same.
+    {
+        int dev = 0, optin = 0;
+        RX_CHECK_CUDA(h, cudaGetDevice(&dev));
+        RX_CHECK_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        const struct { const void *kern; int dyn; } use[] = {{(const void *)k_propagate_mol<true>, m->dyn_shared_bytes},
+                                                             {(const void *)k_propagate_mol<false>, m->dyn_shared_bytes},
+                                                             {(const void *)k_minimize_mol, m->shared_bytes},
+                                                             {(const void *)k_energy_mol, m->shared_bytes}};
+        size_t need = 0;
+        for (const auto &u : use) {
+            cudaFuncAttributes fa;
+            RX_CHECK_CUDA(h, cudaFuncGetAttributes(&fa, u.kern));
+            need = std::max(need, fa.sharedSizeBytes + (size_t)u.dyn);
+        }
+        const int slots = m->n_slots;
+        if (need > (size_t)optin || slots > 32767) {
+            rxi_free_molecule(h);
+            RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_molecule: the term tables need " + std::to_string(need) +
+                                               " bytes of shared memory per block, more than the device's " + std::to_string(optin) +
+                                               " (too many bonded terms)");
+        }
     }
     int rc = 0;
     if ((rc = mol_upload(h, mass, &m->mass)) || (rc = mol_upload(h, charge, &m->charge)) || (rc = mol_upload(h, sigma, &m->sigma)) ||

@@ -404,8 +404,10 @@ __device__ __forceinline__ void mol_shake_cluster(const MolDev &m, int c, const 
     }
 }
 
-// RATTLE on one cluster: the velocity components along its constraints are removed.
-__device__ __forceinline__ void mol_rattle_cluster(const MolDev &m, int c, const MolCluster &k, const double (*X)[3], double (*V)[3]) {
+// RATTLE on one cluster: the velocity components along its constraints are removed.  unit: unit weights instead of 1/m
+// (the minimiser's projection; clusters of <= MOL_MAXC constraints carry their weights in k).
+__device__ __forceinline__ void mol_rattle_cluster(const MolDev &m, int c, const MolCluster &k, const double (*X)[3], double (*V)[3],
+                                                   bool unit = false) {
     switch (k.nc) {
         case 1: mol_rattle_n<1>(k, X, V); return;
         case 2: mol_rattle_n<2>(k, X, V); return;
@@ -422,7 +424,7 @@ __device__ __forceinline__ void mol_rattle_cluster(const MolDev &m, int c, const
             const double rv = mol_dot(r, dv), r2 = mol_dot(r, r);
             if (fabs(rv) > m.tol * r2) {
                 done = false;
-                const double wi = 1.0 / m.mass[s.i], wj = 1.0 / m.mass[s.j];
+                const double wi = unit ? 1.0 : 1.0 / m.mass[s.i], wj = unit ? 1.0 : 1.0 / m.mass[s.j];
                 const double g = rv / ((wi + wj) * r2);
                 for (int a = 0; a < 3; a++) { V[s.i][a] -= g * wi * r[a]; V[s.j][a] += g * wj * r[a]; }
             }
@@ -728,7 +730,8 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
 
 // MultiStateSampler.minimize (multistatesampler.py:611-647) for a molecule: FIRE descent on the constraint manifold.  The
 // force is projected onto the manifold (components along the constrained bonds removed: the RATTLE solve with unit
-// weights), the move is followed by SHAKE, the FIRE velocity is kept tangent.  Converged when the RMS of the projected force
+// weights, unit-weight sweeps for clusters of more than MOL_MAXC constraints), the move is followed by SHAKE, the FIRE
+// velocity is kept tangent.  Converged when the RMS of the projected force
 // falls below tol_rms (kJ/mol/nm); f64 throughout.  (OpenMM's L-BFGS is not reproduced, as for the other systems.)
 __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restrict__ pos, int k0, double tol_rms, int max_iter,
                                                      double *__restrict__ rms_out, int *__restrict__ iters_out) {
@@ -767,7 +770,7 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
         if (active) mol_atom<false, double>(ms, X, a, f);
         if (active) for (int c = 0; c < 3; c++) F[a][c] = f[c];
         __syncwarp();
-        if (a < m.n_clusters && ku.nc <= MOL_MAXC) mol_rattle_cluster(m, a, ku, X, F);   // projected force
+        if (a < m.n_clusters) mol_rattle_cluster(m, a, ku, X, F, true);   // projected force
         __syncwarp();
         if (active) for (int c = 0; c < 3; c++) f[c] = F[a][c];
         const double FF = mol_warp_sum(active ? f[0] * f[0] + f[1] * f[1] + f[2] * f[2] : 0.0);
@@ -795,7 +798,7 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
         __syncwarp();
         if (a < m.n_clusters) mol_shake_cluster(m, a, kc, XO, X);
         __syncwarp();
-        if (a < m.n_clusters && ku.nc <= MOL_MAXC) mol_rattle_cluster(m, a, ku, X, V);   // velocity stays tangent
+        if (a < m.n_clusters) mol_rattle_cluster(m, a, ku, X, V, true);   // velocity stays tangent
         __syncwarp();
     }
     if (a == 0) { rms_out[k] = rms; iters_out[k] = it; }

@@ -220,13 +220,17 @@ def emulate_kernel(m, stars, x0, v0, noise, kT, dt, gamma, n_steps, remove_cm):
     return X, V
 
 
-@pytest.mark.parametrize('which', ['alanine dipeptide', 'water dimer'])
+@pytest.mark.parametrize('which', ['alanine dipeptide', 'water dimer', 'decane shuffled', 'ten waters'])
 def test_whole_step_sequence_matches_the_oracle(which):
     import ctypes as C
     from oracle import oracle
-    from helpers import device_noise
+    from helpers import device_noise, alkane, waters
     if which == 'water dimer':
         s, x0 = water_dimer()
+    elif which == 'decane shuffled':      # clusters of 2 and 3 constraints, i > j, clusters interleaved in the list
+        s, x0 = alkane(10, terms_per_torsion=3, shuffle=5)
+    elif which == 'ten waters':
+        s, x0 = waters(10, shuffle=3)
     else:
         a = testsystems.AlanineDipeptideVacuum()
         s, x0 = a.system, np.ascontiguousarray(a.positions.value_in_unit(unit.nanometer), np.float64)
