@@ -165,7 +165,9 @@ RX_API int rx_get_replica_states(rx_engine *h, int64_t *states /*[K]*/);
 /* Replaces MultiStateSampler._propagate_replicas (multistatesampler.py:1287-1337) ->
  * BaseIntegratorMove.apply (mcmc.py:668-776) -> integrator.step(n_steps) (mcmc.py:719).
  * Noise is Philox4x32-10 keyed by (seed; iteration, global replica, atom, step), so trajectories do not
- * depend on the number of GPUs.  nan_flags[K] (may be NULL) gets 1 for replicas whose state went NaN.    */
+ * depend on the number of GPUs.  nan_flags[K] (may be NULL) gets 1 for replicas whose state went NaN.
+ * Replicas of up to 4096 atoms (RX_SYSTEM_LJ_ALCH; above 1024 a replica spans a cluster of 2, 4 or 8 thread blocks) or
+ * 1024 atoms (RX_SYSTEM_HARMONIC); larger ones return RX_ERR_UNSUPPORTED here and in rx_minimize.        */
 RX_API int rx_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int32_t reassign_velocities,
                  int32_t *nan_flags);
 /* Replaces the restart loop of BaseIntegratorMove.apply (mcmc.py:706-759, n_restart_attempts): after rx_propagate
@@ -248,6 +250,33 @@ RX_API int rx_get_mix_stats(rx_engine *h, int64_t out[6]);
 /* Diagnostic: y[t] = the device's correctly rounded exp(x[t]) (host arrays) -- the function behind the one decision the
  * mixing kernels do not take in the log domain, `rand() < exp(log_p)` of replicaexchange.py:340 inside the 1e-9 guard band. */
 RX_API int rx_selftest_exp(rx_engine *h, const double *x, double *y, int32_t n);
+
+/* Diagnostic: the launch rx_propagate would make for a RX_SYSTEM_LJ_ALCH or RX_SYSTEM_HARMONIC engine, computed on the host
+ * without any device call (so it can be checked without a GPU).  The device enters through n_sm and smem_optin
+ * (cudaDevAttrMultiProcessorCount, cudaDevAttrMaxSharedMemoryPerBlockOptin); the environment overrides rx_propagate reads
+ * (RX_CLUSTER, RX_SKIN, RX_SKIN_IN, RX_NO_VERLET, RX_NO_SORT) enter through the query.  Returns RX_ERR_UNSUPPORTED for
+ * sizes rx_propagate refuses (more than 4096 LJ atoms or 1024 harmonic atoms per replica); the message is then
+ * rx_last_error(NULL). */
+typedef struct {
+    int32_t system_kind, n_atoms;
+    int32_t kloc;              /* replicas owned by the engine */
+    int32_t per_state;         /* 1: per-state moves (rx_set_state_integrator) are set */
+    int32_t n_sm, smem_optin;  /* multiprocessors; opt-in shared memory per block (bytes) */
+    double box[3], r_cutoff;
+    double skin_out, skin_in;  /* neighbour-list skins (nm); < 0: the defaults 0.40 / 0.05 */
+    int32_t cluster;           /* blocks per replica requested (RX_CLUSTER), 0: the planner's choice */
+    int32_t no_list, no_sort;  /* all-pairs forces only (RX_NO_VERLET); atoms kept on their threads (RX_NO_SORT) */
+} rx_propagate_query;
+typedef struct {
+    int32_t cluster;           /* thread blocks per replica (a thread-block cluster of 1, 2, 4 or 8) */
+    int32_t threads;           /* threads per block, one atom each */
+    int32_t list_capacity;     /* neighbour-list entries per atom, 0: all-pairs forces */
+    int32_t sort_atoms;        /* 1: atoms are re-dealt to threads by neighbour count at every list build */
+    int32_t compact;           /* 1: the layout of more than 1024 atoms (position buffers strided by N, 8-byte parameters) */
+    int32_t reserved;
+    int64_t smem_bytes;        /* dynamic shared memory per block */
+} rx_propagate_plan;
+RX_API int rx_plan_propagate(const rx_propagate_query *query, rx_propagate_plan *plan);
 
 /* ---- multi-GPU ------------------------------------------------------------------------------------ */
 /* NCCL is loaded with dlopen(nccl_library_path).  Rank 0 creates an id (rx_comm_unique_id), the host code

@@ -335,6 +335,23 @@ class Engine:
         return dict(rounds=int(out[0]), exact_exp=int(out[1]), passes=int(out[2]), words=int(out[3]),
                     walker_ms=out[4] / 1e3, prepare_wait_ms=out[5] / 1e3)
 
+    @staticmethod
+    def plan_propagate(system_kind, n_atoms, kloc, n_sm, smem_optin, box=(1.0, 1.0, 1.0), r_cutoff=0.0,
+                       per_state=False, skin_out=-1.0, skin_in=-1.0, cluster=0, no_list=False, no_sort=False):
+        """The launch rx_propagate would make (blocks per replica, threads, list capacity, ...) for a device with `n_sm`
+        multiprocessors and `smem_optin` bytes of opt-in shared memory per block; host arithmetic, no device needed.
+        Arguments after r_cutoff mirror the RX_SKIN, RX_SKIN_IN, RX_CLUSTER, RX_NO_VERLET and RX_NO_SORT overrides."""
+        lib = _lib.load()
+        q = _lib.RxPropagateQuery(int(system_kind), int(n_atoms), int(kloc), int(bool(per_state)), int(n_sm),
+                                  int(smem_optin), (C.c_double * 3)(*[float(b) for b in box]), float(r_cutoff),
+                                  float(skin_out), float(skin_in), int(cluster), int(bool(no_list)), int(bool(no_sort)))
+        out = _lib.RxPropagatePlan()
+        rc = lib.rx_plan_propagate(C.byref(q), C.byref(out))
+        if rc != 0:
+            raise EngineError(rc, lib.rx_last_error(None).decode())
+        return dict(cluster=out.cluster, threads=out.threads, list_capacity=out.list_capacity,
+                    sort_atoms=bool(out.sort_atoms), compact=bool(out.compact), smem_bytes=int(out.smem_bytes))
+
     # -- multi-GPU
     @staticmethod
     def comm_unique_id(nccl_path=None):

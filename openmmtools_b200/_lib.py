@@ -21,7 +21,7 @@ SYMBOLS = [
     'rx_get_replica_energies', 'rx_pin_host_memory', 'rx_unpin_host_memory', 'rx_randomize_velocities', 'rx_minimize', 'rx_set_replica_states', 'rx_get_replica_states',
     'rx_propagate', 'rx_propagate_retry', 'rx_compute_energies', 'rx_compute_energies_at', 'rx_set_energies', 'rx_get_energies', 'rx_mix_seed',
     'rx_mix_skip', 'rx_mix_swap_all', 'rx_mix_swap_neighbors', 'rx_get_mix_counts', 'rx_mix_stream_position',
-    'rx_run_iterations', 'rx_sams_set', 'rx_sams_step', 'rx_sams_get', 'rx_sams_run_iterations', 'rx_get_phase_times', 'rx_timer_mark', 'rx_timer_elapsed', 'rx_get_mix_stats', 'rx_selftest_exp', 'rx_comm_unique_id', 'rx_comm_init',
+    'rx_run_iterations', 'rx_sams_set', 'rx_sams_step', 'rx_sams_get', 'rx_sams_run_iterations', 'rx_get_phase_times', 'rx_timer_mark', 'rx_timer_elapsed', 'rx_get_mix_stats', 'rx_selftest_exp', 'rx_plan_propagate', 'rx_comm_unique_id', 'rx_comm_init',
 ]
 
 
@@ -42,6 +42,18 @@ class RxStateParams(C.Structure):
 class RxSamsConfig(C.Structure):
     _fields_ = [('gamma0', C.c_double), ('flatness_threshold', C.c_double), ('weight_update_method', C.c_int32),
                 ('two_stage', C.c_int32), ('flatness_criteria', C.c_int32), ('stage', C.c_int32), ('t0', C.c_int64)]
+
+
+class RxPropagateQuery(C.Structure):
+    _fields_ = [('system_kind', C.c_int32), ('n_atoms', C.c_int32), ('kloc', C.c_int32), ('per_state', C.c_int32),
+                ('n_sm', C.c_int32), ('smem_optin', C.c_int32), ('box', C.c_double * 3), ('r_cutoff', C.c_double),
+                ('skin_out', C.c_double), ('skin_in', C.c_double), ('cluster', C.c_int32), ('no_list', C.c_int32),
+                ('no_sort', C.c_int32)]
+
+
+class RxPropagatePlan(C.Structure):
+    _fields_ = [('cluster', C.c_int32), ('threads', C.c_int32), ('list_capacity', C.c_int32), ('sort_atoms', C.c_int32),
+                ('compact', C.c_int32), ('reserved', C.c_int32), ('smem_bytes', C.c_int64)]
 
 
 class RxMolecule(C.Structure):
@@ -108,6 +120,7 @@ def load():
     lib.rx_timer_elapsed.argtypes = [vp, C.POINTER(dbl)]
     lib.rx_get_mix_stats.argtypes = [vp, vp]
     lib.rx_selftest_exp.argtypes = [vp, vp, vp, C.c_int32]
+    lib.rx_plan_propagate.argtypes = [C.POINTER(RxPropagateQuery), C.POINTER(RxPropagatePlan)]
     lib.rx_comm_unique_id.argtypes = [C.c_char_p, vp]
     lib.rx_comm_init.argtypes = [vp, C.c_char_p, vp]
     if lib.rx_abi_version() != RX_ABI_VERSION:

@@ -51,6 +51,7 @@ extern "C" int rx_create(const rx_config *cfg, rx_engine **out) {
     h = new rx_engine();
     h->cfg = *cfg;
     CREATE_CUDA(cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, cfg->device));
+    CREATE_CUDA(cudaDeviceGetAttribute(&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, cfg->device));
     const int K = cfg->n_replicas, M = cfg->n_states, N = cfg->n_atoms, W = cfg->world_size, R = cfg->rank;
     h->k0 = (int)(((long long)R * K) / W);
     h->kloc = (int)(((long long)(R + 1) * K) / W) - h->k0;
@@ -732,6 +733,10 @@ extern "C" int rx_selftest_exp(rx_engine *h, const double *x, double *y, int32_t
     if (n > 0 && (!x || !y)) RX_FAIL(h, RX_ERR_INVALID, "rx_selftest_exp: null array");
     RX_CHECK_CUDA(h, cudaSetDevice(h->cfg.device));
     return rxi_selftest_exp(h, x, y, n);
+}
+extern "C" int rx_plan_propagate(const rx_propagate_query *q, rx_propagate_plan *out) {
+    if (!q || !out) { g_rx_create_error = "rx_plan_propagate: null argument"; return RX_ERR_INVALID; }
+    return rxi_plan_propagate(q, out, g_rx_create_error);
 }
 
 extern "C" int rx_get_mix_stats(rx_engine *h, int64_t out[6]) {

@@ -131,7 +131,8 @@ __device__ __forceinline__ float4 lds_f4(unsigned a) {
     asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
     return v;
 }
-#define RX_MAX_ATOMS 1024
+#define RX_MAX_ATOMS 1024      // atoms per block (one per thread); the shared-memory stride of the layout up to that size
+#define RX_MAX_ATOMS_LJ 4096   // atoms per replica of the LJ kernels (k_propagate over a cluster of up to 8 blocks)
 __device__ __forceinline__ float2 lds_f2(unsigned a) {
     float2 v;
     asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
@@ -161,8 +162,9 @@ struct PairCtx {
     PairLam lam;
 };
 
-// One candidate pair with atom j (position records at pos_base, parameter records par_off bytes further).
-template <bool C6, bool SW, bool ENERGY>
+// One candidate pair with atom j (position records at pos_base; parameter records par_off bytes further, or with P8
+// 8-byte parameter records (sqrt_eps, alch) starting at the shared address par_off).
+template <bool C6, bool SW, bool ENERGY, bool P8 = false>
 __device__ __forceinline__ void pair_term(const DynParams &p, const PairCtx &c, unsigned pos_base, int par_off, unsigned j,
                                           float &ax, float &ay, float &az, float &en) {
     const unsigned aj = pos_base + 16u * j;
@@ -171,7 +173,7 @@ __device__ __forceinline__ void pair_term(const DynParams &p, const PairCtx &c, 
                 dz = min_image_f(c.z - pj.z, c.Lz, c.iLz);
     const float r2 = dx * dx + dy * dy + dz * dz;
     if (r2 < c.rc2) {
-        const float2 qj = lds_f2(aj + (unsigned)par_off);
+        const float2 qj = lds_f2(P8 ? (unsigned)par_off + 8u * j : aj + (unsigned)par_off);
         const bool alch_j = qj.y != 0.f;
         const bool soft = (c.alch_i != alch_j) || (c.alch_i && alch_j && p.annihilate);
         float e;
@@ -182,7 +184,7 @@ __device__ __forceinline__ void pair_term(const DynParams &p, const PairCtx &c, 
 }
 
 // Force on one atom from the inner part of its neighbour list or, in the fallback, from all other atoms.
-template <bool C6, bool SW, bool ENERGY>
+template <bool C6, bool SW, bool ENERGY, bool P8 = false>
 __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, unsigned pos_base, int par_off,
                                           unsigned nb_t, int N, int ncol, int a, bool use_list, int n_inner,
                                           float &fx, float &fy, float &fz, float &en) {
@@ -191,17 +193,17 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
         const unsigned stride = 2u * (unsigned)ncol;
         unsigned q = nb_t;
         for (int n = 0; n < n_inner; n++, q += stride)
-            pair_term<C6, SW, ENERGY>(p, c, pos_base, par_off, lds_u16(q), ax, ay, az, e);
+            pair_term<C6, SW, ENERGY, P8>(p, c, pos_base, par_off, lds_u16(q), ax, ay, az, e);
     } else {
         for (int j = 0; j < N; j++)
-            if (j != a) pair_term<C6, SW, ENERGY>(p, c, pos_base, par_off, (unsigned)j, ax, ay, az, e);
+            if (j != a) pair_term<C6, SW, ENERGY, P8>(p, c, pos_base, par_off, (unsigned)j, ax, ay, az, e);
     }
     fx = ax; fy = ay; fz = az; en = e;
 }
 
 #define RX_SORT_BINS 128
 
-// One CTA per owned replica, one atom per thread (N <= 1024).
+// One CTA (or thread-block cluster) per owned replica, one atom per thread (N <= 1024 per block, N <= 4096 per replica).
 //
 // Neighbour search is a dual list held in shared memory, one column per thread:
 //   outer list  every j with r < cutoff + skin_out when it was built (an all-pairs pass);
@@ -218,14 +220,17 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
 //
 // Positions are double buffered: a force evaluation writes the moved positions into the buffer the previous
 // evaluation did not read, and the displacement vote (__syncthreads_or) is the only barrier of the step.
-// A replica may be split over a cluster of CL thread blocks (CL = 1, 2 or 4; chosen when there are fewer replicas than SMs):
+// A replica may be split over a cluster of CL thread blocks (CL = 1, 2 or 4 up to 1024 atoms, chosen when there are fewer
+// replicas than SMs; CL = 2, 4 or 8 above, where one block cannot hold the atoms):
 // block q of the cluster owns the atoms [q Nq, (q+1) Nq), every block keeps ALL positions in its own shared memory -- a block
 // writes the new positions of its atoms into every block's buffer through distributed shared memory -- and the step's only
 // barrier becomes a cluster barrier.  The displacement votes are cluster wide, so the lists are rebuilt at the same steps and
 // with the same contents as in one block: trajectories do not depend on CL (each atom sums its own list in list order, noise
 // is keyed by atom id).
 // PS: per-state moves (the integrator parameters come from `moves[state]` instead of `p`).
-template <bool C6, bool SW, int CL, bool PS = false>
+// COMPACT: the layout above 1024 atoms (DESIGN 4.2): position buffers strided by N instead of RX_MAX_ATOMS and 8-byte
+// parameter records (sqrt_eps, alch) -- sigma rides in the position's w -- so that 4096 atoms leave room for a list.
+template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false>
 __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *__restrict__ atom,
                                                     const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                     float4 *__restrict__ pos, float4 *__restrict__ vel, int k0,
@@ -236,12 +241,16 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     extern __shared__ float4 s_dyn[];
     // (the whole cluster takes this exit together: `only` is indexed by replica)
     if (only && !only[k0 + blockIdx.x / CL]) return;   // a retry launch propagates the replicas that failed, nothing else
-    float4 *s_par = s_dyn + RX_MAX_ATOMS;  // [RX_MAX_ATOMS] (sqrt_eps, alch, -, -); s_dyn[0..] / s_dyn[2*MAX..]: positions
-    float4 *s_ref = s_dyn + 3 * RX_MAX_ATOMS;                  // [nthr] the thread's position at the last outer build
+    // s_dyn[0..] / s_dyn[pos1..]: the two position buffers (pos1 = 2*MAX, or N when COMPACT)
+    const int pos1 = COMPACT ? p.N : 2 * RX_MAX_ATOMS;
+    float4 *s_par = s_dyn + RX_MAX_ATOMS;  // [RX_MAX_ATOMS] (sqrt_eps, alch, -, -)
+    float2 *s_par8 = (float2 *)(s_dyn + 2 * p.N);                     // COMPACT: [N] (sqrt_eps, alch)
+    float4 *s_ref = COMPACT ? s_dyn + (2 * p.N + (p.N + 1) / 2)      // [nthr] the thread's position at the last outer build
+                            : s_dyn + 3 * RX_MAX_ATOMS;
     unsigned short *s_nb = (unsigned short *)(s_ref + blockDim.x);  // [maxnb][nthr] lists, slot-major (conflict free)
     __shared__ double s_red[32];
     __shared__ int s_vote[2];            // cluster-wide votes (alternating words)
-    __shared__ double s_part[3 * 4];     // per-block partial sums, gathered in block 0 of the cluster
+    __shared__ double s_part[3 * (CL > 4 ? CL : 4)];   // per-block partial sums, gathered in block 0 of the cluster
     const int r = blockIdx.x / CL, q = blockIdx.x % CL, k = k0 + r, t = threadIdx.x, nthr = blockDim.x;
     const int Nq = (p.N + CL - 1) / CL, a_base = q * Nq;
     const int n_own = min(Nq, p.N - a_base);
@@ -289,7 +298,8 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     }
     for (int j = t; j < p.N; j += nthr) {   // parameter records of ALL atoms (the pair loop reads those of its partners)
         const float4 a4 = atom[j];
-        s_par[j] = make_float4(a4.y, a4.w != 0.f ? 1.f : 0.f, 0.f, 0.f);
+        if (COMPACT) s_par8[j] = make_float2(a4.y, a4.w != 0.f ? 1.f : 0.f);
+        else s_par[j] = make_float4(a4.y, a4.w != 0.f ? 1.f : 0.f, 0.f, 0.f);
     }
     if (CL > 1) cg::this_cluster().sync();   // every block of the cluster is resident and has cleared its vote words
     float fx = 0, fy = 0, fz = 0;
@@ -301,7 +311,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     bool have_list = false;        // an outer list exists
     int n_all = 0, n_inner = 0;
     float xi = x, yi = y, zi = z;  // position at the last partition
-    int cur = 1;                   // position buffer of the latest force evaluation (0: s_dyn, 1: s_dyn + 2*MAX)
+    int cur = 1;                   // position buffer of the latest force evaluation (0: s_dyn, 1: s_dyn + pos1)
     const unsigned dyn_base = (unsigned)__cvta_generic_to_shared(s_dyn);
     const unsigned nb_t = (unsigned)__cvta_generic_to_shared(s_nb + t);
     const unsigned stride = 2u * (unsigned)nthr;
@@ -410,7 +420,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     // Publish the current positions and make the neighbour list valid for them: one barrier unless a list is rebuilt.
     auto publish = [&]() {
         cur ^= 1;
-        float4 *s_pos = s_dyn + (cur ? 2 * RX_MAX_ATOMS : 0);
+        float4 *s_pos = s_dyn + (cur ? pos1 : 0);
         if (active) {
             const float4 me = make_float4(x, y, z, sig_i);
             if (CL == 1) s_pos[a] = me;
@@ -433,10 +443,11 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         if (!f_valid) publish();
         if (active) {
             pc.x = x; pc.y = y; pc.z = z; pc.sig_i = sig_i; pc.se_i = se_i; pc.alch_i = alch_i;
-            const unsigned pos_base = dyn_base + (cur ? 2u * 16u * RX_MAX_ATOMS : 0u);
-            const int par_off = cur ? -16 * RX_MAX_ATOMS : 16 * RX_MAX_ATOMS;
-            if (want_energy) lj_forces<C6, SW, true>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
-            else lj_forces<C6, SW, false>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
+            const unsigned pos_base = dyn_base + (cur ? 16u * (unsigned)pos1 : 0u);
+            // (COMPACT: the address of the 8-byte records; otherwise the offset from either buffer to the 16-byte records)
+            const int par_off = COMPACT ? (int)(dyn_base + 32u * (unsigned)N) : (cur ? -16 * RX_MAX_ATOMS : 16 * RX_MAX_ATOMS);
+            if (want_energy) lj_forces<C6, SW, true, COMPACT>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
+            else lj_forces<C6, SW, false, COMPACT>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
         } else {
             fx = fy = fz = 0.f; e_out = 0.f;
         }
@@ -711,8 +722,9 @@ int rxi_convert_out(rx_engine *h, const float4 *src, int first_local, int count,
 #include "rx_molecule.cuh"
 
 // A block may take 48 KB of shared memory, static and dynamic together, unless the kernel has opted in to more (up to
-// cudaDevAttrMaxSharedMemoryPerBlockOptin, which rxi_set_molecule checks).  The molecule's tables grow with its terms.
-static int mol_smem_optin(rx_engine *h, const void *kern, int dyn) {
+// cudaDevAttrMaxSharedMemoryPerBlockOptin, which rxi_set_molecule checks).  The molecule's tables grow with its terms, the
+// energy kernel's coordinates with the atoms (48 KB of them at 2048 atoms, over the limit with its static arrays).
+static int smem_opt_in(rx_engine *h, const void *kern, int dyn) {
     cudaFuncAttributes fa;
     RX_CHECK_CUDA(h, cudaFuncGetAttributes(&fa, kern));
     if (fa.sharedSizeBytes + (size_t)dyn > 48 * 1024)
@@ -767,6 +779,115 @@ int rxi_upload_state_moves(rx_engine *h) {
     return RX_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Launch plan of k_propagate: host arithmetic only (rx_plan_propagate exports it, so that it can be checked without a GPU).
+// ---------------------------------------------------------------------------------------------------
+#define RX_PROP_STATIC_SMEM 1024   // bound on k_propagate's static shared memory (s_red, s_vote, s_part: under 0.5 KB)
+#define RX_MIN_LIST_CAP 48         // list entries per atom every cluster chosen above 1024 atoms holds (DESIGN 4.2)
+
+// Dual neighbour list: outer skin 0.40 nm (at 300 K and 10/ps friction the all-pairs build usually lasts a whole 500-step
+// launch), inner skin 0.05 nm (a re-partition of the column about every 25 steps; both tuned on the 512-atom fluid, see
+// profiles/prop_r1_v6.summary.txt).  The outer radius is clipped to half the shortest box edge.
+struct ListGeom { bool on; double rl, skin_in, eff_out; };
+static ListGeom list_geometry(const rx_propagate_query *q) {
+    ListGeom g = {false, 0.0, 0.0, 0.0};
+    if (q->system_kind != RX_SYSTEM_LJ_ALCH || q->n_atoms < 64 || q->no_list) return g;
+    const double skin_out = q->skin_out >= 0 ? q->skin_out : 0.40;
+    double skin_in = q->skin_in >= 0 ? q->skin_in : 0.05;
+    double rl = q->r_cutoff + skin_out;
+    for (int d = 0; d < 3; d++) if (rl > 0.5 * q->box[d]) rl = 0.5 * q->box[d];
+    const double eff_out = rl - q->r_cutoff;
+    if (skin_in > eff_out / 3.0) skin_in = eff_out / 3.0;
+    g.on = eff_out > 0.03; g.rl = rl; g.skin_in = skin_in; g.eff_out = eff_out;
+    return g;
+}
+
+// Threads, list capacity, sort flag and dynamic shared memory of N atoms over `cl` blocks.  The list capacity comes from
+// the shared-memory budget: up to 1024 atoms two CTAs per SM up to 512 threads (112 KB each), 200 KB above; the compact
+// layout takes the device's opt-in limit.  Denser systems fall back to all-pairs in the kernel.  False: the atoms alone
+// do not fit in the compact budget.
+static bool plan_at(int N, int cl, bool compact, const ListGeom &g, size_t compact_budget, bool no_sort, rx_propagate_plan *o) {
+    memset(o, 0, sizeof(*o));
+    const int n_per = (N + cl - 1) / cl;
+    const int threads = ((n_per + 31) / 32) * 32;
+    // shared memory: two position buffers + the parameter records + per-thread reference positions + the list area
+    // (compact: 16 + 16 + 8 bytes per atom, rounded up to 16 bytes; otherwise 3 x 16 bytes x RX_MAX_ATOMS)
+    const size_t atoms_bytes = (compact ? ((size_t)40 * N + 15) / 16 * 16 : (size_t)3 * RX_MAX_ATOMS * sizeof(float4)) +
+                               (size_t)threads * sizeof(float4);
+    size_t area = (size_t)threads * sizeof(double2);  // the list area doubles as scratch for the final reductions
+    if (g.on) {
+        const size_t budget = compact ? compact_budget : (size_t)(threads > 512 ? 200 : 112) * 1024;
+        int cap = budget > atoms_bytes ? (int)((budget - atoms_bytes) / ((size_t)threads * sizeof(unsigned short))) : 0;
+        if (cap > 128) cap = 128;
+        if (cap >= 8) {
+            o->list_capacity = cap;
+            const size_t list_bytes = (((size_t)cap * threads * sizeof(unsigned short)) + 15) / 16 * 16;
+            // scratch of the atom re-assignment: velocities, order, per-warp bin counts, bin bases
+            const size_t sort_bytes = (size_t)threads * (sizeof(float4) + 2) + (size_t)(threads / 32 + 1) * RX_SORT_BINS * 2;
+            o->sort_atoms = (list_bytes >= sort_bytes && !no_sort) ? 1 : 0;
+            if (list_bytes > area) area = list_bytes;
+        }
+    }
+    o->cluster = cl;
+    o->threads = threads;
+    o->compact = compact ? 1 : 0;
+    o->smem_bytes = (int64_t)(atoms_bytes + area);
+    return !compact || atoms_bytes + area <= compact_budget;
+}
+
+int rxi_plan_propagate(const rx_propagate_query *q, rx_propagate_plan *o, std::string &err) {
+    memset(o, 0, sizeof(*o));
+    const int N = q->n_atoms;
+    const bool lj = q->system_kind == RX_SYSTEM_LJ_ALCH;
+    if (!lj && q->system_kind != RX_SYSTEM_HARMONIC) { err = "rx_plan_propagate: LJ and harmonic systems only"; return RX_ERR_INVALID; }
+    if (N < 1 || q->kloc < 0 || q->n_sm < 1) { err = "rx_plan_propagate: need n_atoms >= 1, kloc >= 0, n_sm >= 1"; return RX_ERR_INVALID; }
+    if (!lj && N > RX_MAX_ATOMS) {
+        err = "rx_propagate: more than 1024 atoms per replica of a harmonic system is not supported";
+        return RX_ERR_UNSUPPORTED;
+    }
+    if (N > RX_MAX_ATOMS_LJ) {
+        err = "rx_propagate: more than 4096 atoms per replica is not supported (every block of a replica's cluster holds "
+              "all of its positions in shared memory)";
+        return RX_ERR_UNSUPPORTED;
+    }
+    const ListGeom g = list_geometry(q);
+    if (N <= RX_MAX_ATOMS) {
+        // Blocks per replica (a thread-block cluster; RX_CLUSTER = 1 | 2 | 4 overrides).  A block of 128 threads leaves ONE
+        // warp per scheduler, which runs the step's
+        // ~1100 dependent instructions no faster than four warps sharing a scheduler do: the split only pays for the few
+        // replicas that would otherwise leave three quarters of the GPU idle, so that is the only case it is chosen for.
+        int cl = 1;
+        if (lj && N >= 256) {
+            if (q->kloc * 4 <= q->n_sm) cl = 4;
+            if (q->cluster == 1 || q->cluster == 2 || q->cluster == 4) cl = q->cluster;
+        }
+        if (q->per_state) cl = 1;
+        plan_at(N, cl, false, g, 0, q->no_sort, o);
+        return RX_OK;
+    }
+    // Above 1024 atoms a replica needs CL >= N/1024 blocks.  The smallest CL of 2, 4, 8 whose blocks hold the atoms and a
+    // list of at least RX_MIN_LIST_CAP entries; widened to 4 or 8 when the replicas leave SMs idle (kloc CL <= #SMs).
+    // RX_CLUSTER = 2 | 4 | 8 overrides when that CL can hold the atoms and such a list.
+    const size_t budget = q->smem_optin > RX_PROP_STATIC_SMEM ? (size_t)q->smem_optin - RX_PROP_STATIC_SMEM : 0;
+    rx_propagate_plan tmp;
+    auto feasible = [&](int cl) {
+        return cl * RX_MAX_ATOMS >= N && plan_at(N, cl, true, g, budget, q->no_sort, &tmp) &&
+               (!g.on || tmp.list_capacity >= RX_MIN_LIST_CAP);
+    };
+    int cl = 0;
+    for (int c = 2; c <= 8 && !cl; c *= 2) if (feasible(c)) cl = c;
+    if (!cl) {
+        err = "rx_propagate: " + std::to_string(N) + " atoms per replica do not fit in a cluster of up to 8 blocks with " +
+              std::to_string(q->smem_optin) + " bytes of shared memory each";
+        return RX_ERR_UNSUPPORTED;
+    }
+    for (int c = 8; c > cl; c /= 2)
+        if ((long long)q->kloc * c <= q->n_sm && feasible(c)) { cl = c; break; }
+    if ((q->cluster == 2 || q->cluster == 4 || q->cluster == 8) && feasible(q->cluster)) cl = q->cluster;
+    plan_at(N, cl, true, g, budget, q->no_sort, o);
+    return RX_OK;
+}
+
 int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign, int *launches, const int *d_only) {
     if (h->kloc == 0) return RX_OK;
     DynParams p;
@@ -778,7 +899,7 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         const MolDev *md = (const MolDev *)h->mol_dev;
         const bool no_star = getenv("RX_MOL_NO_STAR") != nullptr;   // cross-check: the general cluster path for every molecule
         auto kern = (md->max_cluster <= 3 && !no_star) ? k_propagate_mol<true> : k_propagate_mol<false>;
-        const int rco = mol_smem_optin(h, (const void *)kern, md->dyn_shared_bytes);
+        const int rco = smem_opt_in(h, (const void *)kern, md->dyn_shared_bytes);
         if (rco) return rco;
         kern<<<h->kloc, 32 * MOL_WARPS, md->dyn_shared_bytes, h->stream>>>(*md, p, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
                                                                            (double *)h->d_vel, h->k0, mkey, (uint32_t)iteration, reassign, h->d_pot,
@@ -787,58 +908,35 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         (*launches)++;
         return RX_OK;
     }
-    if (N > 1024) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_propagate: more than 1024 atoms per replica is not supported yet");
-    // Blocks per replica (a thread-block cluster; RX_CLUSTER = 1 | 2 | 4 overrides).  A block of 128 threads leaves ONE
-    // warp per scheduler, which runs the step's
-    // ~1100 dependent instructions no faster than four warps sharing a scheduler do: the split only pays for the few
-    // replicas that would otherwise leave three quarters of the GPU idle, so that is the only case it is chosen for.
-    int cl = 1;
-    if (h->cfg.system_kind == RX_SYSTEM_LJ_ALCH && N >= 256) {
-        if (h->kloc * 4 <= h->n_sm) cl = 4;
-        if (const char *e = getenv("RX_CLUSTER")) { const int v = atoi(e); if (v == 1 || v == 2 || v == 4) cl = v; }
-    }
     const bool per_state = !h->state_moves.empty();
     if (per_state) {
-        cl = 1;
         int rcm = rxi_upload_state_moves(h);
         if (rcm) return rcm;
     }
-    const int n_per = (N + cl - 1) / cl;
-    const int threads = ((n_per + 31) / 32) * 32;
-    // shared memory: two position buffers + the parameter records + per-thread reference positions + the list area
-    const size_t atoms_bytes = (size_t)3 * RX_MAX_ATOMS * sizeof(float4) + (size_t)threads * sizeof(float4);
-    size_t area = (size_t)threads * sizeof(double2);  // the list area doubles as scratch for the final reductions
-    if (h->cfg.system_kind == RX_SYSTEM_LJ_ALCH && N >= 64 && !getenv("RX_NO_VERLET")) {
-        // Dual neighbour list: outer skin 0.40 nm (at 300 K and 10/ps friction the all-pairs build usually lasts a
-        // whole 500-step launch), inner skin 0.05 nm (a re-partition of the column about every 25 steps; both tuned
-        // on the 512-atom fluid, see profiles/prop_r1_v6.summary.txt).  Capacity from the
-        // shared-memory budget (two CTAs per SM up to 512 atoms); denser systems fall back to all-pairs in the kernel.
-        const char *so = getenv("RX_SKIN"), *si = getenv("RX_SKIN_IN");
-        const double skin_out = so ? atof(so) : 0.40;
-        double skin_in = si ? atof(si) : 0.05;
-        double rl = h->cfg.r_cutoff + skin_out;
-        for (int d = 0; d < 3; d++) if (rl > 0.5 * h->cfg.box[d]) rl = 0.5 * h->cfg.box[d];
-        const double eff_out = rl - h->cfg.r_cutoff;
-        if (skin_in > eff_out / 3.0) skin_in = eff_out / 3.0;
-        if (eff_out > 0.03) {
-            const size_t budget = (threads > 512 ? 200 : 112) * 1024;
-            int cap = (int)((budget - atoms_bytes) / ((size_t)threads * sizeof(unsigned short)));
-            if (cap > 128) cap = 128;
-            if (cap >= 8) {
-                p.maxnb = cap;
-                p.rl2 = (float)(rl * rl);
-                p.rin2 = (float)((h->cfg.r_cutoff + skin_in) * (h->cfg.r_cutoff + skin_in));
-                p.half_in2 = (float)(0.25 * skin_in * skin_in);
-                p.half_out2 = (float)(0.25 * (eff_out - skin_in) * (eff_out - skin_in));
-                const size_t list_bytes = (((size_t)cap * threads * sizeof(unsigned short)) + 15) / 16 * 16;
-                // scratch of the atom re-assignment: velocities, order, per-warp bin counts, bin bases
-                const size_t sort_bytes = (size_t)threads * (sizeof(float4) + 2) + (size_t)(threads / 32 + 1) * RX_SORT_BINS * 2;
-                p.sort_atoms = (list_bytes >= sort_bytes && !getenv("RX_NO_SORT")) ? 1 : 0;
-                if (list_bytes > area) area = list_bytes;
-            }
-        }
+    rx_propagate_query q;
+    memset(&q, 0, sizeof(q));
+    q.system_kind = h->cfg.system_kind; q.n_atoms = N; q.kloc = h->kloc; q.per_state = per_state ? 1 : 0;
+    q.n_sm = h->n_sm; q.smem_optin = h->smem_optin;
+    for (int d = 0; d < 3; d++) q.box[d] = h->cfg.box[d];
+    q.r_cutoff = h->cfg.r_cutoff;
+    const char *so = getenv("RX_SKIN"), *si = getenv("RX_SKIN_IN");
+    q.skin_out = so ? atof(so) : -1.0; q.skin_in = si ? atof(si) : -1.0;
+    if (const char *e = getenv("RX_CLUSTER")) q.cluster = atoi(e);
+    q.no_list = getenv("RX_NO_VERLET") != nullptr; q.no_sort = getenv("RX_NO_SORT") != nullptr;
+    rx_propagate_plan plan;
+    const int rcp = rxi_plan_propagate(&q, &plan, h->err);
+    if (rcp) return rcp;
+    const int cl = plan.cluster, threads = plan.threads;
+    if (plan.list_capacity > 0) {
+        const ListGeom g = list_geometry(&q);
+        p.maxnb = plan.list_capacity;
+        p.sort_atoms = plan.sort_atoms;
+        p.rl2 = (float)(g.rl * g.rl);
+        p.rin2 = (float)((h->cfg.r_cutoff + g.skin_in) * (h->cfg.r_cutoff + g.skin_in));
+        p.half_in2 = (float)(0.25 * g.skin_in * g.skin_in);
+        p.half_out2 = (float)(0.25 * (g.eff_out - g.skin_in) * (g.eff_out - g.skin_in));
     }
-    const size_t smem = atoms_bytes + area;
+    const size_t smem = (size_t)plan.smem_bytes;
     const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(iteration >> 32));
     cudaLaunchConfig_t lc = {};
     lc.gridDim = dim3((unsigned)(h->kloc * cl));
@@ -851,22 +949,30 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
     lc.attrs = at;
     lc.numAttrs = 1;
     const uint32_t it32 = (uint32_t)iteration;
-#define RX_LAUNCH_PROPAGATE(C6, SW, CL, PS)                                                                               \
+#define RX_LAUNCH_PROPAGATE(C6, SW, CL, PS, CP)                                                                           \
     do {                                                                                                                   \
         if (smem > 48 * 1024)                                                                                              \
-            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_propagate<C6, SW, CL, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        RX_CHECK_CUDA(h, cudaLaunchKernelEx(&lc, k_propagate<C6, SW, CL, PS>, p, (const float4 *)h->d_atom, (const StateDev *)h->d_states, \
+            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_propagate<C6, SW, CL, PS, CP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        RX_CHECK_CUDA(h, cudaLaunchKernelEx(&lc, k_propagate<C6, SW, CL, PS, CP>, p, (const float4 *)h->d_atom, (const StateDev *)h->d_states, \
                                             (const int *)h->d_perm, h->d_pos, h->d_vel, h->k0, key, it32, reassign, h->d_pot, \
                                             h->d_kin, h->d_nan, d_only, (const MoveDev *)h->d_moves));                    \
     } while (0)
+// above 1024 atoms: the compact layout over 2, 4 or 8 blocks, per-state moves or not
+#define RX_LAUNCH_PROPAGATE_COMPACT(C6, SW, PS)                                                                           \
+    do {                                                                                                                   \
+        if (cl == 8) RX_LAUNCH_PROPAGATE(C6, SW, 8, PS, true); else if (cl == 4) RX_LAUNCH_PROPAGATE(C6, SW, 4, PS, true); \
+        else RX_LAUNCH_PROPAGATE(C6, SW, 2, PS, true);                                                                     \
+    } while (0)
 #define RX_LAUNCH_PROPAGATE_CL(C6, SW)                                                                                    \
     do {                                                                                                                   \
-        if (per_state) RX_LAUNCH_PROPAGATE(C6, SW, 1, true);                                                               \
-        else if (cl == 4) RX_LAUNCH_PROPAGATE(C6, SW, 4, false); else if (cl == 2) RX_LAUNCH_PROPAGATE(C6, SW, 2, false); \
-        else RX_LAUNCH_PROPAGATE(C6, SW, 1, false);                                                                        \
+        if (plan.compact) { if (per_state) RX_LAUNCH_PROPAGATE_COMPACT(C6, SW, true); else RX_LAUNCH_PROPAGATE_COMPACT(C6, SW, false); } \
+        else if (per_state) RX_LAUNCH_PROPAGATE(C6, SW, 1, true, false);                                                   \
+        else if (cl == 4) RX_LAUNCH_PROPAGATE(C6, SW, 4, false, false); else if (cl == 2) RX_LAUNCH_PROPAGATE(C6, SW, 2, false, false); \
+        else RX_LAUNCH_PROPAGATE(C6, SW, 1, false, false);                                                                 \
     } while (0)
     if (p.c_is_6) { if (p.use_switch) RX_LAUNCH_PROPAGATE_CL(true, true); else RX_LAUNCH_PROPAGATE_CL(true, false); }
     else { if (p.use_switch) RX_LAUNCH_PROPAGATE_CL(false, true); else RX_LAUNCH_PROPAGATE_CL(false, false); }
+#undef RX_LAUNCH_PROPAGATE_COMPACT
 #undef RX_LAUNCH_PROPAGATE_CL
 #undef RX_LAUNCH_PROPAGATE
     RX_CHECK_CUDA(h, cudaGetLastError());
@@ -924,31 +1030,39 @@ int rxi_restore_failed(rx_engine *h) {
 // (integrators.py FIREMinimizationIntegrator).  FIRE as published (Bitzek et al., PRL 97, 170201 (2006)):
 // semi-implicit Euler dynamics with the velocity steered towards the force, the time step grown while the power
 // F.v stays positive and the motion stopped when it turns negative; plus a cap on the displacement per step so the
-// overlapping starts of the reference's test systems cannot blow up.  One CTA per replica, one atom per thread,
-// all-pairs forces (this is a set-up step, not the hot path).  Velocities are left untouched.
+// overlapping starts of the reference's test systems cannot blow up.  One CTA per replica, all-pairs forces (this is a
+// set-up step, not the hot path).  Velocities are left untouched.
+// APT atoms per thread: thread t owns atoms t, t + nthr, ... (APT = 1 up to 1024 atoms, 4 above); its terms of the block
+// sums are added in that order, so the result does not depend on scheduling.  Shared memory: [stride] positions, then
+// [stride] parameter records, stride = RX_MAX_ATOMS (APT = 1) or N.
 // ---------------------------------------------------------------------------------------------------
-template <bool C6, bool SW>
+template <bool C6, bool SW, int APT>
 __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__restrict__ atom,
                                                    const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                    float4 *__restrict__ pos, int k0, float tol_rms, int max_iter,
                                                    double *__restrict__ rms_out, int *__restrict__ iters_out) {
     extern __shared__ float4 s_dyn[];
-    float4 *s_pos = s_dyn, *s_par = s_dyn + RX_MAX_ATOMS;
+    const int stride = APT == 1 ? RX_MAX_ATOMS : p.N;
+    float4 *s_pos = s_dyn, *s_par = s_dyn + stride;
     __shared__ float s_part[32][3];
     __shared__ float s_sum[3];
-    const int r = blockIdx.x, k = k0 + r, t = threadIdx.x, nw = blockDim.x >> 5;
-    const bool active = t < p.N;
+    const int r = blockIdx.x, k = k0 + r, t = threadIdx.x, nthr = blockDim.x, nw = nthr >> 5;
     const StateDev st = states[perm[k]];
-    const float4 a4 = active ? atom[t] : make_float4(1.f, 0.f, 1.f, 0.f);
-    const float sig_i = a4.x, se_i = a4.y, inv_m = a4.z;
-    const bool alch_i = a4.w != 0.f;
-    const float4 x4 = active ? pos[(size_t)r * p.N + t] : make_float4(0, 0, 0, 0);
-    float x = x4.x, y = x4.y, z = x4.z, vx = 0.f, vy = 0.f, vz = 0.f;
-    if (active) { s_pos[t] = make_float4(x, y, z, sig_i); s_par[t] = make_float4(se_i, alch_i ? 1.f : 0.f, 0.f, 0.f); }
+    float vx[APT], vy[APT], vz[APT];
+#pragma unroll
+    for (int u = 0; u < APT; u++) {
+        const int a = t + u * nthr;
+        vx[u] = vy[u] = vz[u] = 0.f;
+        if (a < p.N) {
+            const float4 a4 = atom[a], x4 = pos[(size_t)r * p.N + a];
+            s_pos[a] = make_float4(x4.x, x4.y, x4.z, a4.x);
+            s_par[a] = make_float4(a4.y, a4.w != 0.f ? 1.f : 0.f, 0.f, 0.f);
+        }
+    }
     __syncthreads();
     PairCtx pc;
     pc.Lx = p.Lx; pc.Ly = p.Ly; pc.Lz = p.Lz; pc.iLx = p.iLx; pc.iLy = p.iLy; pc.iLz = p.iLz; pc.rc2 = p.rc2;
-    pc.sig_i = sig_i; pc.se_i = se_i; pc.alch_i = alch_i; pc.lam = {(float)st.la, (float)st.ob};
+    pc.lam = {(float)st.la, (float)st.ob};
     const unsigned pos_base = (unsigned)__cvta_generic_to_shared(s_dyn);
     const float hx0 = (float)st.ho_x0[0], hx1 = (float)st.ho_x0[1], hx2 = (float)st.ho_x0[2], hK = (float)st.ho_K;
     const float dt0 = 0.001f, dt_max = 0.010f, alpha0 = 0.1f, max_move = 0.01f;  // ps, ps, -, nm per step
@@ -956,15 +1070,27 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
     int n_pos = 0, it = 0;
     float rms = 0.f;
     for (;;) {
-        float fx = 0.f, fy = 0.f, fz = 0.f, e = 0.f;
-        if (p.kind == RX_SYSTEM_HARMONIC) { fx = -hK * (x - hx0); fy = -hK * (y - hx1); fz = -hK * (z - hx2); }
-        else if (active) {
-            pc.x = x; pc.y = y; pc.z = z;
-            lj_forces<C6, SW, false>(p, pc, pos_base, 16 * RX_MAX_ATOMS, 0u, p.N, p.N, t, false, 0, fx, fy, fz, e);
+        float fx[APT], fy[APT], fz[APT], q0 = 0.f, q1 = 0.f, q2 = 0.f;
+#pragma unroll
+        for (int u = 0; u < APT; u++) {
+            const int a = t + u * nthr;
+            const bool active = a < p.N;
+            const float4 xa = active ? s_pos[a] : make_float4(0, 0, 0, 0);
+            float gx = 0.f, gy = 0.f, gz = 0.f, e = 0.f;
+            if (p.kind == RX_SYSTEM_HARMONIC) { gx = -hK * (xa.x - hx0); gy = -hK * (xa.y - hx1); gz = -hK * (xa.z - hx2); }
+            else if (active) {
+                const float4 a4 = atom[a];
+                pc.x = xa.x; pc.y = xa.y; pc.z = xa.z; pc.sig_i = a4.x; pc.se_i = a4.y; pc.alch_i = a4.w != 0.f;
+                lj_forces<C6, SW, false>(p, pc, pos_base, 16 * stride, 0u, p.N, p.N, a, false, 0, gx, gy, gz, e);
+            }
+            if (!active) { gx = gy = gz = 0.f; }
+            fx[u] = gx; fy[u] = gy; fz[u] = gz;
+            // this thread's terms of F.F, F.v, v.v in atom order
+            const float f2 = gx * gx + gy * gy + gz * gz, fv = gx * vx[u] + gy * vy[u] + gz * vz[u],
+                        v2 = vx[u] * vx[u] + vy[u] * vy[u] + vz[u] * vz[u];
+            if (u == 0) { q0 = f2; q1 = fv; q2 = v2; } else { q0 += f2; q1 += fv; q2 += v2; }
         }
-        if (!active) { fx = fy = fz = 0.f; }
         // block sums of F.F, F.v, v.v (fixed order: deterministic)
-        float q0 = fx * fx + fy * fy + fz * fz, q1 = fx * vx + fy * vy + fz * vz, q2 = vx * vx + vy * vy + vz * vz;
         for (int o = 16; o > 0; o >>= 1) {
             q0 += __shfl_down_sync(0xffffffffu, q0, o); q1 += __shfl_down_sync(0xffffffffu, q1, o); q2 += __shfl_down_sync(0xffffffffu, q2, o);
         }
@@ -976,28 +1102,46 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
         rms = sqrtf(FF / (3.0f * (float)p.N));
         if (!(rms > tol_rms) || it >= max_iter) break;  // converged, out of iterations, or NaN
         it++;
+        const float alpha_v = alpha;
+        const float mix = P > 0.f ? alpha * sqrtf(VV / fmaxf(FF, 1e-30f)) : 0.f;
         if (P > 0.f) {
-            const float mix = alpha * sqrtf(VV / fmaxf(FF, 1e-30f));
-            vx = (1.f - alpha) * vx + mix * fx; vy = (1.f - alpha) * vy + mix * fy; vz = (1.f - alpha) * vz + mix * fz;
             if (++n_pos > 5) { dt = fminf(dt * 1.1f, dt_max); alpha *= 0.99f; }
         } else {
-            vx = vy = vz = 0.f; dt *= 0.5f; alpha = alpha0; n_pos = 0;
+            dt *= 0.5f; alpha = alpha0; n_pos = 0;
         }
-        vx += dt * fx * inv_m; vy += dt * fy * inv_m; vz += dt * fz * inv_m;
-        float mx = dt * vx, my = dt * vy, mz = dt * vz;
-        const float m2 = mx * mx + my * my + mz * mz;
-        if (m2 > max_move * max_move) {  // displacement cap: rescale this atom's velocity
-            const float sc = max_move * rsqrtf(m2);
-            vx *= sc; vy *= sc; vz *= sc; mx *= sc; my *= sc; mz *= sc;
+#pragma unroll
+        for (int u = 0; u < APT; u++) {
+            const int a = t + u * nthr;
+            const bool active = a < p.N;
+            float wx = vx[u], wy = vy[u], wz = vz[u];
+            if (P > 0.f) {
+                wx = (1.f - alpha_v) * wx + mix * fx[u]; wy = (1.f - alpha_v) * wy + mix * fy[u]; wz = (1.f - alpha_v) * wz + mix * fz[u];
+            } else {
+                wx = wy = wz = 0.f;
+            }
+            const float inv_m = active ? atom[a].z : 1.f;
+            wx += dt * fx[u] * inv_m; wy += dt * fy[u] * inv_m; wz += dt * fz[u] * inv_m;
+            float mx = dt * wx, my = dt * wy, mz = dt * wz;
+            const float m2 = mx * mx + my * my + mz * mz;
+            if (m2 > max_move * max_move) {  // displacement cap: rescale this atom's velocity
+                const float sc = max_move * rsqrtf(m2);
+                wx *= sc; wy *= sc; wz *= sc; mx *= sc; my *= sc; mz *= sc;
+            }
+            vx[u] = wx; vy[u] = wy; vz[u] = wz;
+            if (active) { const float4 xa = s_pos[a]; s_pos[a] = make_float4(xa.x + mx, xa.y + my, xa.z + mz, xa.w); }
         }
-        x += mx; y += my; z += mz;
-        if (active) s_pos[t] = make_float4(x, y, z, sig_i);
         __syncthreads();
     }
     if (t == 0) { rms_out[k] = (double)rms; iters_out[k] = it; }
-    if (active) {
-        if (p.kind != RX_SYSTEM_HARMONIC) { x -= p.Lx * floorf(x * p.iLx); y -= p.Ly * floorf(y * p.iLy); z -= p.Lz * floorf(z * p.iLz); }
-        pos[(size_t)r * p.N + t] = make_float4(x, y, z, 0.f);
+#pragma unroll
+    for (int u = 0; u < APT; u++) {
+        const int a = t + u * nthr;
+        if (a < p.N) {
+            const float4 xa = s_pos[a];
+            float x = xa.x, y = xa.y, z = xa.z;
+            if (p.kind != RX_SYSTEM_HARMONIC) { x -= p.Lx * floorf(x * p.iLx); y -= p.Ly * floorf(y * p.iLy); z -= p.Lz * floorf(z * p.iLz); }
+            pos[(size_t)r * p.N + a] = make_float4(x, y, z, 0.f);
+        }
     }
 }
 
@@ -1005,7 +1149,7 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
     if (h->kloc == 0) return RX_OK;
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
         const MolDev *m = (const MolDev *)h->mol_dev;
-        const int rco = mol_smem_optin(h, (const void *)k_minimize_mol, m->shared_bytes);
+        const int rco = smem_opt_in(h, (const void *)k_minimize_mol, m->shared_bytes);
         if (rco) return rco;
         k_minimize_mol<<<h->kloc, 32, m->shared_bytes, h->stream>>>(*m, (double *)h->d_pos, h->k0, tolerance,
                                                                    max_iterations > 0 ? max_iterations : 100000, d_rms, d_iters);
@@ -1015,12 +1159,25 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
     DynParams p;
     fill_dyn(h, p);
     const int N = h->cfg.n_atoms;
-    if (N > 1024) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_minimize: more than 1024 atoms per replica is not supported yet");
-    const int threads = ((N + 31) / 32) * 32;
-    const size_t smem = (size_t)2 * RX_MAX_ATOMS * sizeof(float4);
+    if (h->cfg.system_kind == RX_SYSTEM_HARMONIC && N > RX_MAX_ATOMS)
+        RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_minimize: more than 1024 atoms per replica of a harmonic system is not supported");
+    if (N > RX_MAX_ATOMS_LJ)
+        RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_minimize: more than 4096 atoms per replica is not supported");
+    // up to 1024 atoms one atom per thread; above, four per thread with 32 bytes of shared memory per atom (opted in)
+    const bool wide = N > RX_MAX_ATOMS;
+    const int threads = wide ? ((N + 4 * 32 - 1) / (4 * 32)) * 32 : ((N + 31) / 32) * 32;
+    const size_t smem = (size_t)2 * (wide ? N : RX_MAX_ATOMS) * sizeof(float4);
 #define RX_LAUNCH_MINIMIZE(C6, SW)                                                                                         \
-    k_minimize<C6, SW><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0,       \
-                                                              (float)tolerance, max_iterations, d_rms, d_iters)
+    do {                                                                                                                   \
+        if (wide) {                                                                                                        \
+            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_minimize<C6, SW, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            k_minimize<C6, SW, 4><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
+                                                                         (float)tolerance, max_iterations, d_rms, d_iters); \
+        } else {                                                                                                           \
+            k_minimize<C6, SW, 1><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
+                                                                         (float)tolerance, max_iterations, d_rms, d_iters); \
+        }                                                                                                                  \
+    } while (0)
     if (p.c_is_6) { if (p.use_switch) RX_LAUNCH_MINIMIZE(true, true); else RX_LAUNCH_MINIMIZE(true, false); }
     else { if (p.use_switch) RX_LAUNCH_MINIMIZE(false, true); else RX_LAUNCH_MINIMIZE(false, false); }
 #undef RX_LAUNCH_MINIMIZE
@@ -1051,7 +1208,7 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     if (h->kloc == 0) return RX_OK;
     const rx_config &c = h->cfg;
     if (c.system_kind == RX_SYSTEM_MOLECULE) {
-        const int rco = mol_smem_optin(h, (const void *)k_energy_mol, ((const MolDev *)h->mol_dev)->shared_bytes);
+        const int rco = smem_opt_in(h, (const void *)k_energy_mol, ((const MolDev *)h->mol_dev)->shared_bytes);
         if (rco) return rco;
         k_energy_mol<<<h->kloc, 32, ((const MolDev *)h->mol_dev)->shared_bytes, h->stream>>>(*(const MolDev *)h->mol_dev, d_states, n_states, (const double *)h->d_pos, h->k0, d_out);
         RX_CHECK_CUDA(h, cudaGetLastError());
@@ -1068,7 +1225,8 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     p.c_is_6 = (c.softcore_c == 6.0); p.sc_c = c.softcore_c;
     p.pair_cap = h->pair_cap;
     const size_t smem = (size_t)3 * c.n_atoms * sizeof(double);
-    if (smem > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_energy_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int rco = smem_opt_in(h, (const void *)k_energy_rows, (int)smem);
+    if (rco) return rco;
     k_energy_rows<<<h->kloc, 512, smem, h->stream>>>(p, h->d_atom_d, h->d_alch_list, d_states, h->d_pos, h->k0,
                                                     (double2 *)h->d_pairs, d_out, h->d_err);
     RX_CHECK_CUDA(h, cudaGetLastError());
@@ -1263,7 +1421,7 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
         m->n_tb = (int)tb.size(); m->n_ta = (int)tang.size(); m->n_tt = (int)tt.size(); m->n_tp = (int)tp.size(); m->n_slots = slot;
         m->dyn_shared_bytes = m->shared_bytes + (int)up(off) + (int)up(sizeof(float) * 3 * (size_t)(slot > 0 ? slot : 1));
     }
-    // What no block can hold is refused here rather than at launch (which opts in above 48 KB: mol_smem_optin).  The slot
+    // What no block can hold is refused here rather than at launch (which opts in above 48 KB: smem_opt_in).  The slot
     // indices of the term tables are shorts; tables that fit in shared memory have far fewer slots, checked all the same.
     {
         int dev = 0, optin = 0;

@@ -60,6 +60,7 @@ struct rx_engine {
     rx_config cfg;
     int k0 = 0, kloc = 0;  // owned replicas [k0, k0+kloc)
     int n_sm = 0;          // multiprocessors of cfg.device
+    int smem_optin = 0;    // opt-in shared memory per block of cfg.device (bytes)
     cudaStream_t stream = nullptr, stream_rng = nullptr;
     cudaEvent_t ev[8] = {};
     cudaEvent_t ev_user[2] = {};
@@ -175,6 +176,7 @@ void rxi_sams_free(rx_engine *h);
 
 // ---- implemented in rx_dynamics.cu ----
 int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign, int *launches, const int *d_only = nullptr);
+int rxi_plan_propagate(const rx_propagate_query *q, rx_propagate_plan *out, std::string &err);   // host arithmetic only
 int rxi_upload_state_moves(rx_engine *h);
 int rxi_set_molecule(rx_engine *h, const rx_molecule *mol);
 void rxi_free_molecule(rx_engine *h);
