@@ -121,6 +121,25 @@ RX_API int rx_set_states(rx_engine *h, const rx_state_params *states /* [n_state
  * RX_ERR_UNSUPPORTED (and no molecule set) when the term tables need more shared memory than a block of the device can
  * have (each torsion term takes 236 bytes of the 227 KB of an H100 block: decane with three terms per torsion needs 95 KB); a refused call leaves the engine without a molecule. */
 RX_API int rx_set_molecule(rx_engine *h, const rx_molecule *molecule);
+/* OBC generalized Born implicit solvent for the molecule of the last rx_set_molecule (which returns the engine to vacuum):
+ * what AmberPrmtopFile.createSystem(implicitSolvent=OBC1|OBC2, nonbondedCutoff=None) adds, without salt.  For atom i
+ * (rt = radius - offset, sr = scale rt):
+ *   I_i = sum_{j != i} 1/2 [1/L - 1/U + 1/4 (r - sr_j^2/r)(1/U^2 - 1/L^2) + 1/2 ln(L/U)/r]   over pairs with r + sr_j > rt_i
+ *         (U = r + sr_j, L = max(rt_i, |r - sr_j|); every pair, excluded and 1-4 pairs included; no engulfment term),
+ *   B_i = 1 / (1/rt_i - tanh(alpha psi - beta psi^2 + gamma psi^3) / radius_i),  psi = I_i rt_i,
+ *   E   = sum_i [1/2 P q_i^2 / B_i + 4 pi sa_energy (radius_i + probe_radius)^2 (radius_i / B_i)^6]
+ *       + sum_{i<j} P q_i q_j / sqrt(r^2 + B_i B_j exp(-r^2 / (4 B_i B_j))),   P = -138.935456 (1/solute - 1/solvent dielectric).
+ * OBC1: alpha, beta, gamma = 0.8, 0, 2.909125; OBC2: 1.0, 0.8, 4.85; offset 0.009 nm; sa_energy 2.25936 kJ/mol/nm^2 (0: no
+ * non-polar term), probe_radius 0.14 nm.  RX_ERR_INVALID for a radius <= 0 or <= offset, a negative scale, or an engine
+ * without a molecule; RX_ERR_UNSUPPORTED when the tables no longer fit in a block (the propagation kernel adds
+ * 8 (4 n^2 + 3 n) bytes to the molecule's, 33 KB at 32 atoms); a refused call leaves the engine as it was. */
+typedef struct {
+    const double *radius, *scale;   /* [n_atoms]: nm, dimensionless */
+    double alpha, beta, gamma, offset;
+    double solute_dielectric, solvent_dielectric;
+    double sa_energy, probe_radius;   /* kJ/mol/nm^2, nm */
+} rx_gbsa;
+RX_API int rx_set_implicit_solvent(rx_engine *h, const rx_gbsa *gbsa);
 /* LangevinSplittingDynamicsMove parameters (mcmc.py:1280-1291) / LangevinIntegrator (integrators.py:1071-1158):
  * timestep (ps), collision_rate (1/ps), n_steps, splitting with the spaces removed, e.g. "VRORV".        */
 RX_API int rx_set_integrator(rx_engine *h, double timestep, double collision_rate, int32_t n_steps,

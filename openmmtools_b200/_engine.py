@@ -119,6 +119,17 @@ class Engine:
                                                            ('mass', 'charge', 'sigma', 'epsilon', 'bonds', 'angles', 'torsions',
                                                             'exclusions', 'exceptions', 'constraints')])
         self._check(self._lib.rx_set_molecule(self._h, C.byref(m)))
+        if getattr(system, 'gb_radius', None) is not None:
+            self.set_implicit_solvent(system.gb_radius, system.gb_scale, *system.gb_parameters)
+
+    def set_implicit_solvent(self, radius, scale, alpha, beta, gamma, offset, solute_dielectric, solvent_dielectric, sa_energy,
+                             probe_radius):
+        """OBC implicit solvent for the molecule of the last set_molecule (rx_set_implicit_solvent)."""
+        radius = np.ascontiguousarray(radius, np.float64)
+        scale = np.ascontiguousarray(scale, np.float64)
+        g = _lib.RxGbsa(radius.ctypes.data, scale.ctypes.data, alpha, beta, gamma, offset, solute_dielectric, solvent_dielectric,
+                        sa_energy, probe_radius)
+        self._check(self._lib.rx_set_implicit_solvent(self._h, C.byref(g)))
 
     def set_state_integrator(self, state, timestep, collision_rate, n_steps, splitting='V R O R V', reassign_velocities=False):
         """The move of one thermodynamic state where the states carry different moves (after set_integrator)."""

@@ -17,7 +17,7 @@ RX_STREAM_NUMBA, RX_STREAM_NUMPY = 0, 1
 # every symbol include/rx_b200.h declares
 SYMBOLS = [
     'rx_create', 'rx_destroy', 'rx_last_error', 'rx_abi_version', 'rx_set_particles', 'rx_set_states',
-    'rx_set_integrator', 'rx_set_state_integrator', 'rx_set_molecule', 'rx_set_positions', 'rx_set_velocities', 'rx_get_positions', 'rx_get_velocities',
+    'rx_set_integrator', 'rx_set_state_integrator', 'rx_set_molecule', 'rx_set_implicit_solvent', 'rx_set_positions', 'rx_set_velocities', 'rx_get_positions', 'rx_get_velocities',
     'rx_get_replica_energies', 'rx_pin_host_memory', 'rx_unpin_host_memory', 'rx_randomize_velocities', 'rx_minimize', 'rx_set_replica_states', 'rx_get_replica_states',
     'rx_propagate', 'rx_propagate_retry', 'rx_compute_energies', 'rx_compute_energies_at', 'rx_set_energies', 'rx_get_energies', 'rx_mix_seed',
     'rx_mix_skip', 'rx_mix_swap_all', 'rx_mix_swap_neighbors', 'rx_get_mix_counts', 'rx_mix_stream_position',
@@ -65,6 +65,12 @@ class RxMolecule(C.Structure):
                 ('exceptions', C.c_void_p), ('constraints', C.c_void_p)]
 
 
+class RxGbsa(C.Structure):
+    _fields_ = [('radius', C.c_void_p), ('scale', C.c_void_p), ('alpha', C.c_double), ('beta', C.c_double), ('gamma', C.c_double),
+                ('offset', C.c_double), ('solute_dielectric', C.c_double), ('solvent_dielectric', C.c_double),
+                ('sa_energy', C.c_double), ('probe_radius', C.c_double)]
+
+
 _lib = None
 
 
@@ -89,6 +95,7 @@ def load():
     lib.rx_set_integrator.argtypes = [vp, dbl, dbl, i32, C.c_char_p]
     lib.rx_set_state_integrator.argtypes = [vp, i32, dbl, dbl, i32, C.c_char_p, i32]
     lib.rx_set_molecule.argtypes = [vp, C.POINTER(RxMolecule)]
+    lib.rx_set_implicit_solvent.argtypes = [vp, C.POINTER(RxGbsa)]
     for name in ('rx_set_positions', 'rx_set_velocities', 'rx_get_positions', 'rx_get_velocities'):
         getattr(lib, name).argtypes = [vp, i32, i32, vp]
     lib.rx_get_replica_energies.argtypes = [vp, vp, vp]

@@ -13,7 +13,10 @@ and OpenMM's documented conventions, NOT taken from OpenMM's source (which is no
     rmin_ii = 2 R_i), Lorentz-Berthelot combination; 1-4 pairs: Coulomb / 1.2 (SCEE), LJ epsilon / 2 (SCNB) with the pair's
     own A, B; 1-2 and 1-3 pairs (EXCLUDED_ATOMS_LIST) excluded;
   * constraints=HBonds: every bond that involves a hydrogen becomes a distance constraint at r0 and its bond term is dropped;
-  * no cutoff: plain sums over all non-excluded pairs; Coulomb constant 138.935456 kJ nm / (mol e^2).
+  * no cutoff: plain sums over all non-excluded pairs; Coulomb constant 138.935456 kJ nm / (mol e^2);
+  * implicitSolvent=OBC1 / OBC2: the generalized Born model of GBSAOBCForce with the file's RADII (Angstrom -> nm) and
+    SCREEN factors (RADIUS_SET names the radius set), solute / solvent dielectric 1 / 78.5, the ACE non-polar term
+    (2.25936 kJ/mol/nm^2, probe radius 0.14 nm), no salt (see obc_parameters).
 """
 import numpy as np
 
@@ -125,7 +128,36 @@ def read_prmtop(path):
     full = sorted(excluded - set(pairs14))
     return dict(names=names, mass=mass, charge=charge, sigma=sigma, epsilon=epsilon, bonds=all_bonds,
                 angles=angles('ANGLES_INC_HYDROGEN') + angles('ANGLES_WITHOUT_HYDROGEN'), torsions=torsions,
-                exclusions=full, exceptions=exceptions)
+                exclusions=full, exceptions=exceptions,
+                radii=np.array(get('RADII')) * 0.1 if 'RADII' in sec else None,
+                screen=np.array(get('SCREEN')) if 'SCREEN' in sec else None,
+                radius_set=''.join(get('RADIUS_SET')).strip() if 'RADIUS_SET' in sec else None)
+
+
+# (alpha, beta, gamma) of the OBC models (Onufriev, Bashford, Case 2004: OBC1 = AMBER igb=2, OBC2 = igb=5)
+OBC_MODELS = {'OBC1': (0.8, 0.0, 2.909125), 'OBC2': (1.0, 0.8, 4.85)}
+
+
+def obc_parameters(implicitSolvent='OBC1', implicitSolventKappa=None, implicitSolventSaltConc=None, soluteDielectric=1.0,
+                   solventDielectric=78.5, gbsaModel='ACE', nonbondedCutoff=None, nonbondedMethod=None):
+    """system.System.gb_parameters for createSystem(implicitSolvent=...): (alpha, beta, gamma, offset, solute dielectric,
+    solvent dielectric, surface-area energy, probe radius).  Salt screening, cutoffs and the HCT / GBn / GBn2 models are
+    not provided: they raise NotImplementedError."""
+    name = getattr(implicitSolvent, '__name__', implicitSolvent)
+    if name not in OBC_MODELS:
+        raise NotImplementedError('implicitSolvent=%r is not provided: OBC1 and OBC2 only (HCT, GBn and GBn2 are not)' % (name,))
+    for v, what in ((implicitSolventKappa, 'implicitSolventKappa'), (implicitSolventSaltConc, 'implicitSolventSaltConc')):
+        if v is not None and float(getattr(v, '_value', v)) != 0.0:
+            raise NotImplementedError('%s: salt screening of the GB model is not provided' % what)
+    method = getattr(nonbondedMethod, '__name__', nonbondedMethod)
+    if nonbondedCutoff is not None or method not in (None, 'NoCutoff'):
+        raise NotImplementedError('implicit solvent molecules are all-pairs (nonbondedMethod=NoCutoff, nonbondedCutoff=None)')
+    model = getattr(gbsaModel, '__name__', gbsaModel)
+    if model not in ('ACE', None):
+        raise NotImplementedError("gbsaModel must be 'ACE' or None")
+    sa = 2.25936 if model == 'ACE' else 0.0
+    eps_in, eps_out = (float(getattr(v, '_value', v)) for v in (soluteDielectric, solventDielectric))
+    return OBC_MODELS[name] + (0.009, eps_in, eps_out, sa, 0.14)
 
 
 def read_inpcrd(path):

@@ -192,6 +192,14 @@ extern "C" int rx_set_molecule(rx_engine *h, const rx_molecule *molecule) {
     return rxi_set_molecule(h, molecule);
 }
 
+extern "C" int rx_set_implicit_solvent(rx_engine *h, const rx_gbsa *gbsa) {
+    ENTER(h);
+    if (h->cfg.system_kind != RX_SYSTEM_MOLECULE) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: the engine was not created with RX_SYSTEM_MOLECULE");
+    if (!gbsa) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: null");
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    return rxi_set_implicit_solvent(h, gbsa);
+}
+
 static int convert_states(rx_engine *h, const rx_state_params *s, int n, std::vector<StateDev> &out, const char *who) {
     out.resize(n);
     for (int l = 0; l < n; l++) {

@@ -897,13 +897,17 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         if (!h->state_moves.empty()) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_propagate: per-state moves are not provided for molecules");
         const uint2 mkey = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(iteration >> 32));
         const MolDev *md = (const MolDev *)h->mol_dev;
+        const MolGB *gb = (const MolGB *)h->mol_gb;
         const bool no_star = getenv("RX_MOL_NO_STAR") != nullptr;   // cross-check: the general cluster path for every molecule
-        auto kern = (md->max_cluster <= 3 && !no_star) ? k_propagate_mol<true> : k_propagate_mol<false>;
-        const int rco = smem_opt_in(h, (const void *)kern, md->dyn_shared_bytes);
+        const bool star = md->max_cluster <= 3 && !no_star;
+        auto kern = gb ? (star ? k_propagate_mol<true, true> : k_propagate_mol<false, true>)
+                       : (star ? k_propagate_mol<true, false> : k_propagate_mol<false, false>);
+        const int dyn = md->dyn_shared_bytes + (gb ? gb->prop_bytes : 0);
+        const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
-        kern<<<h->kloc, 32 * MOL_WARPS, md->dyn_shared_bytes, h->stream>>>(*md, p, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
-                                                                           (double *)h->d_vel, h->k0, mkey, (uint32_t)iteration, reassign, h->d_pot,
-                                                                           h->d_kin, h->d_nan, d_only);
+        kern<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
+                                                            (double *)h->d_vel, h->k0, mkey, (uint32_t)iteration, reassign, h->d_pot,
+                                                            h->d_kin, h->d_nan, d_only, gb ? *gb : MolGB{});
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
         return RX_OK;
@@ -1149,10 +1153,13 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
     if (h->kloc == 0) return RX_OK;
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
         const MolDev *m = (const MolDev *)h->mol_dev;
-        const int rco = smem_opt_in(h, (const void *)k_minimize_mol, m->shared_bytes);
+        const MolGB *gb = (const MolGB *)h->mol_gb;
+        auto kern = gb ? k_minimize_mol<true> : k_minimize_mol<false>;
+        const int dyn = m->shared_bytes + (gb ? MOL_GB_LANE_BYTES : 0);
+        const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
-        k_minimize_mol<<<h->kloc, 32, m->shared_bytes, h->stream>>>(*m, (double *)h->d_pos, h->k0, tolerance,
-                                                                   max_iterations > 0 ? max_iterations : 100000, d_rms, d_iters);
+        kern<<<h->kloc, 32, dyn, h->stream>>>(*m, (double *)h->d_pos, h->k0, tolerance, max_iterations > 0 ? max_iterations : 100000,
+                                              d_rms, d_iters, gb ? *gb : MolGB{});
         RX_CHECK_CUDA(h, cudaGetLastError());
         return RX_OK;
     }
@@ -1208,9 +1215,13 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     if (h->kloc == 0) return RX_OK;
     const rx_config &c = h->cfg;
     if (c.system_kind == RX_SYSTEM_MOLECULE) {
-        const int rco = smem_opt_in(h, (const void *)k_energy_mol, ((const MolDev *)h->mol_dev)->shared_bytes);
+        const MolDev *m = (const MolDev *)h->mol_dev;
+        const MolGB *gb = (const MolGB *)h->mol_gb;
+        auto kern = gb ? k_energy_mol<true> : k_energy_mol<false>;
+        const int dyn = m->shared_bytes + (gb ? MOL_GB_LANE_BYTES : 0);
+        const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
-        k_energy_mol<<<h->kloc, 32, ((const MolDev *)h->mol_dev)->shared_bytes, h->stream>>>(*(const MolDev *)h->mol_dev, d_states, n_states, (const double *)h->d_pos, h->k0, d_out);
+        kern<<<h->kloc, 32, dyn, h->stream>>>(*m, d_states, n_states, (const double *)h->d_pos, h->k0, d_out, gb ? *gb : MolGB{});
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
         return RX_OK;
@@ -1427,10 +1438,10 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
         int dev = 0, optin = 0;
         RX_CHECK_CUDA(h, cudaGetDevice(&dev));
         RX_CHECK_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        const struct { const void *kern; int dyn; } use[] = {{(const void *)k_propagate_mol<true>, m->dyn_shared_bytes},
-                                                             {(const void *)k_propagate_mol<false>, m->dyn_shared_bytes},
-                                                             {(const void *)k_minimize_mol, m->shared_bytes},
-                                                             {(const void *)k_energy_mol, m->shared_bytes}};
+        const struct { const void *kern; int dyn; } use[] = {{(const void *)k_propagate_mol<true, false>, m->dyn_shared_bytes},
+                                                             {(const void *)k_propagate_mol<false, false>, m->dyn_shared_bytes},
+                                                             {(const void *)k_minimize_mol<false>, m->shared_bytes},
+                                                             {(const void *)k_energy_mol<false>, m->shared_bytes}};
         size_t need = 0;
         for (const auto &u : use) {
             cudaFuncAttributes fa;
@@ -1461,4 +1472,64 @@ void rxi_free_molecule(rx_engine *h) {
     h->mol_allocs.clear();
     delete (MolDev *)h->mol_dev;
     h->mol_dev = nullptr;
+    rxi_free_implicit_solvent(h);
+}
+
+void rxi_free_implicit_solvent(rx_engine *h) {
+    if (h->mol_gb) cudaFree((void *)((MolGB *)h->mol_gb)->atom);
+    delete (MolGB *)h->mol_gb;
+    h->mol_gb = nullptr;
+}
+
+// OBC implicit solvent (rx_set_implicit_solvent): the per-atom table and the constants of MolGB.  A refused call leaves the
+// engine as it was.
+int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s) {
+    const MolDev *m = (const MolDev *)h->mol_dev;
+    if (!m) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: call rx_set_molecule first");
+    const int n = m->n;
+    if (!s->radius || !s->scale) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: null per-atom arrays");
+    if (!(s->offset >= 0) || !(s->solute_dielectric > 0) || !(s->solvent_dielectric > 0) || !(s->sa_energy >= 0) ||
+        !(s->probe_radius >= 0) || !isfinite(s->alpha) || !isfinite(s->beta) || !isfinite(s->gamma))
+        RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: need offset >= 0, dielectrics > 0, sa_energy >= 0, probe_radius >= 0");
+    std::vector<double> tab(4 * (size_t)n);
+    for (int i = 0; i < n; i++) {
+        const double rho = s->radius[i], sc = s->scale[i];
+        if (!(rho > 0) || !(rho > s->offset) || !(sc >= 0) || !isfinite(rho) || !isfinite(sc))
+            RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: need radius > offset, radius > 0 and scale >= 0 for every atom");
+        const double rt = rho - s->offset;
+        tab[4 * i] = rt; tab[4 * i + 1] = sc * rt; tab[4 * i + 2] = rho;
+        tab[4 * i + 3] = 4.0 * M_PI * s->sa_energy * (rho + s->probe_radius) * (rho + s->probe_radius);
+    }
+    MolGB g;
+    memset(&g, 0, sizeof(g));
+    g.alpha = s->alpha; g.beta = s->beta; g.gamma = s->gamma;
+    g.pre = -MOL_ONE_4PI_EPS0 * (1.0 / s->solute_dielectric - 1.0 / s->solvent_dielectric);
+    g.on = 1;
+    g.prop_bytes = (int)(sizeof(double) * (4 * (size_t)n * n + 3 * (size_t)n));
+    {
+        int dev = 0, optin = 0;
+        RX_CHECK_CUDA(h, cudaGetDevice(&dev));
+        RX_CHECK_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        const struct { const void *kern; int dyn; } use[] = {{(const void *)k_propagate_mol<true, true>, m->dyn_shared_bytes + g.prop_bytes},
+                                                             {(const void *)k_propagate_mol<false, true>, m->dyn_shared_bytes + g.prop_bytes},
+                                                             {(const void *)k_minimize_mol<true>, m->shared_bytes + MOL_GB_LANE_BYTES},
+                                                             {(const void *)k_energy_mol<true>, m->shared_bytes + MOL_GB_LANE_BYTES}};
+        size_t need = 0;
+        for (const auto &u : use) {
+            cudaFuncAttributes fa;
+            RX_CHECK_CUDA(h, cudaFuncGetAttributes(&fa, u.kern));
+            need = std::max(need, fa.sharedSizeBytes + (size_t)u.dyn);
+        }
+        if (need > (size_t)optin)
+            RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_implicit_solvent: the term and solvent tables need " + std::to_string(need) +
+                                               " bytes of shared memory per block, more than the device's " + std::to_string(optin));
+    }
+    void *d = nullptr;
+    RX_CHECK_CUDA(h, cudaMalloc(&d, sizeof(double) * tab.size()));
+    const cudaError_t e = cudaMemcpy(d, tab.data(), sizeof(double) * tab.size(), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { cudaFree(d); RX_CHECK_CUDA(h, e); }
+    rxi_free_implicit_solvent(h);
+    g.atom = (const double *)d;
+    h->mol_gb = new MolGB(g);
+    return RX_OK;
 }

@@ -97,6 +97,7 @@ struct rx_engine {
     char program[RX_MAX_PROGRAM] = {0};
     void *mol_dev = nullptr;                 // MolDev (host copy of the device table of a RX_SYSTEM_MOLECULE engine)
     std::vector<void *> mol_allocs;
+    void *mol_gb = nullptr;                  // MolGB (host copy; nullptr: vacuum) and its device table, rx_set_implicit_solvent
     std::vector<rx_state_move> state_moves;   // per-state moves (empty: one move for all states)
     bool state_moves_dirty = false;
     void *d_moves = nullptr;
@@ -180,6 +181,8 @@ int rxi_plan_propagate(const rx_propagate_query *q, rx_propagate_plan *out, std:
 int rxi_upload_state_moves(rx_engine *h);
 int rxi_set_molecule(rx_engine *h, const rx_molecule *mol);
 void rxi_free_molecule(rx_engine *h);
+int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s);
+void rxi_free_implicit_solvent(rx_engine *h);
 int rxi_snapshot_state(rx_engine *h);   // positions + velocities at the start of a propagation
 int rxi_restore_failed(rx_engine *h);   // replicas with a NaN flag go back to the snapshot; d_retry = the flags
 int rxi_compute_energy_rows(rx_engine *h, int *launches);  // fills d_u rows [k0, k0+kloc)

@@ -60,6 +60,107 @@ struct MolDev {
     int terms_bytes, n_tb, n_ta, n_tt, n_tp, n_slots, dyn_shared_bytes;
 };
 
+// OBC generalized Born implicit solvent (rx_set_implicit_solvent), passed to the kernels as a trailing argument so that the
+// vacuum instantiations (GB = false) keep their argument layout.  All in f64.  For atom i: rho_i the radius, rt_i = rho_i -
+// offset, sr_i = scale_i rt_i.
+//   I_i = sum_{j != i} I_ij,  I_ij = 1/2 [1/L - 1/U + 1/4 (r - sr_j^2/r)(1/U^2 - 1/L^2) + 1/2 ln(L/U) / r]  if r + sr_j > rt_i
+//         (U = r + sr_j, L = max(rt_i, |r - sr_j|); no engulfment term),
+//   B_i = 1 / (1/rt_i - tanh(alpha psi - beta psi^2 + gamma psi^3) / rho_i),  psi = I_i rt_i,
+//   E = sum_i [1/2 pre q_i^2 / B_i + ace_i (rho_i / B_i)^6] + sum_{i<j} pre q_i q_j / sqrt(r^2 + B_i B_j exp(-r^2 / (4 B_i B_j)))
+// with pre = -138.935456 (1/eps_solute - 1/eps_solvent) and ace_i = 4 pi sa_energy (rho_i + probe)^2.
+struct MolGB {
+    const double *atom;   // [n][4]: rt, sr, rho, ace
+    double alpha, beta, gamma, pre;
+    int on;               // (0: vacuum; the GB = true kernels are only launched with 1)
+    int prop_bytes;       // k_propagate_mol<., true>'s arrays behind MolDev::dyn_shared_bytes
+};
+#define MOL_GB_LANE_BYTES (2 * MOL_MAX_ATOMS * 8)   // k_energy_mol / k_minimize_mol: B_i and C_i behind MolDev::shared_bytes
+
+// I_ij at distance r of atom i (offset radius rt) descreened by j (scaled radius sr); *dIdr its derivative.
+__device__ __forceinline__ double gb_descreen(double r, double rt, double sr, double *dIdr) {
+    if (!(r + sr > rt)) { *dIdr = 0.0; return 0.0; }
+    const double U = r + sr, d = r - sr, ad = fabs(d);
+    const bool far = ad > rt;
+    const double L = far ? ad : rt, dL = far ? (d > 0.0 ? 1.0 : -1.0) : 0.0;
+    const double iL = 1.0 / L, iU = 1.0 / U, ir = 1.0 / r, iL2 = iL * iL, iU2 = iU * iU, q = sr * sr * ir, lg = log(L * iU);
+    *dIdr = 0.5 * (-dL * iL2 + iU2 + 0.25 * (1.0 + q * ir) * (iU2 - iL2) + 0.5 * (r - q) * (dL * iL2 * iL - iU2 * iU) +
+                   0.5 * ((dL * iL - iU) - lg * ir) * ir);
+    return 0.5 * (iL - iU + 0.25 * (r - q) * (iU2 - iL2) + 0.5 * lg * ir);
+}
+
+// Born radius from the descreening sum; *dBdI its derivative.
+__device__ __forceinline__ double gb_born(const MolGB &g, double I, double rt, double rho, double *dBdI) {
+    const double psi = I * rt, th = tanh(psi * (g.alpha + psi * (-g.beta + psi * g.gamma)));
+    const double B = 1.0 / (1.0 / rt - th / rho);
+    *dBdI = B * B * (1.0 - th * th) / rho * (g.alpha + psi * (-2.0 * g.beta + 3.0 * g.gamma * psi)) * rt;
+    return B;
+}
+
+// The pair term pqq / f (pqq = pre q_i q_j); *dr: dE/dr / r; *dbi, *dbj: dE/dB_i, dE/dB_j.
+__device__ __forceinline__ double gb_pair(double r2, double Bi, double Bj, double pqq, double *dr, double *dbi, double *dbj) {
+    const double D = Bi * Bj, ex = exp(-0.25 * r2 / D), f2 = r2 + D * ex, E = pqq / sqrt(f2), c = -0.5 * E / f2;
+    const double cb = c * ex * (1.0 + 0.25 * r2 / D);
+    *dr = c * (2.0 - 0.5 * ex); *dbi = cb * Bj; *dbj = cb * Bi;
+    return E;
+}
+
+// The self and ACE terms of atom a; *dB: their dE/dB.
+__device__ __forceinline__ double gb_self(const MolGB &g, double q, double B, double rho, double ace, double *dB) {
+    const double es = 0.5 * g.pre * q * q / B, t = rho / B, t3 = t * t * t, ea = ace * t3 * t3;
+    *dB = -(es + 6.0 * ea) / B;
+    return es + ea;
+}
+
+__device__ __forceinline__ double gb_dist(const double (*X)[3], int i, int j, double *d) {
+    d[0] = X[i][0] - X[j][0]; d[1] = X[i][1] - X[j][1]; d[2] = X[i][2] - X[j][2];
+    return sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+}
+
+// GB energy owned by lane a (its self and ACE terms, its pairs with larger partners) of one warp, one lane per atom, f64;
+// FORCES: f += the GB force on atom a.  Bs, Cs: double[MOL_MAX_ATOMS] in shared memory.  Every lane of the warp calls it.
+template <bool FORCES>
+__device__ double mol_gb_lane(const MolGB &g, const double (*X)[3], const double *q, int a, int n, double *Bs, double *Cs, double *f) {
+    const bool active = a < n;
+    double rt = 1.0, rho = 1.0, ace = 0.0, B = 1.0, dBdI = 0.0, e = 0.0, dEdB = 0.0, d[3], dI;
+    if (active) {
+        rt = g.atom[4 * a]; rho = g.atom[4 * a + 2]; ace = g.atom[4 * a + 3];
+        double I = 0.0;
+        for (int j = 0; j < n; j++) if (j != a) I += gb_descreen(gb_dist(X, a, j, d), rt, g.atom[4 * j + 1], &dI);
+        B = gb_born(g, I, rt, rho, &dBdI);
+        Bs[a] = B;
+    }
+    __syncwarp();
+    if (active) {
+        e = gb_self(g, q[a], B, rho, ace, &dEdB);
+        for (int j = 0; j < n; j++) {
+            if (j == a || (!FORCES && j < a)) continue;
+            const double r = gb_dist(X, a, j, d);
+            double dr, dbi, dbj;
+            const double ep = gb_pair(r * r, B, Bs[j], g.pre * q[a] * q[j], &dr, &dbi, &dbj);
+            if (j > a) e += ep;
+            if (FORCES) { dEdB += dbi; for (int c = 0; c < 3; c++) f[c] -= dr * d[c]; }
+        }
+        if (FORCES) Cs[a] = dEdB * dBdI;
+    }
+    if (FORCES) {
+        __syncwarp();
+        if (active) {
+            const double sa = g.atom[4 * a + 1];
+            for (int j = 0; j < n; j++) {
+                if (j == a) continue;
+                const double r = gb_dist(X, a, j, d);
+                double dIa, dIj;
+                gb_descreen(r, rt, g.atom[4 * j + 1], &dIa);
+                gb_descreen(r, g.atom[4 * j], sa, &dIj);
+                const double s = (Cs[a] * dIa + Cs[j] * dIj) / r;
+                for (int c = 0; c < 3; c++) f[c] -= s * d[c];
+            }
+        }
+        __syncwarp();
+    }
+    return e;
+}
+
 __device__ __forceinline__ void mol_cross(const double *a, const double *b, double *c) {
     c[0] = a[1] * b[2] - a[2] * b[1]; c[1] = a[2] * b[0] - a[0] * b[2]; c[2] = a[0] * b[1] - a[1] * b[0];
 }
@@ -615,18 +716,85 @@ __device__ __forceinline__ double mol_warp_sum(double v) {   // fixed tree: bit-
     return v;
 }
 
+// k_propagate_mol's GB force, pair-parallel over the block, in the arrays of MolGB::prop_bytes: n x n matrices I_ij, dI_ij/dr,
+// the pair's dE/dr / r (symmetric) and dE_pair/dB_i, then B_i, dB_i/dI_i and C_i = dE/dB_i dB_i/dI_i.  Every entry is written by
+// one thread and every atom adds up its row in index order: no atomics, the same bits whatever the thread count.
+struct MolGBArrays {
+    double *I, *D, *P, *EB, *B, *dB, *C;
+    __device__ MolGBArrays(double *s, int n) : I(s), D(s + n * n), P(s + 2 * n * n), EB(s + 3 * n * n), B(s + 4 * n * n), dB(B + n), C(dB + n) {}
+};
+
+// phase 1 (before the barrier that ends the term evaluation): the descreening integrals of the ordered pairs
+__device__ __forceinline__ void mol_gb_integrals(const MolGB &g, const double (*X)[3], int n, const MolGBArrays &s) {
+    for (int t = threadIdx.x; t < n * n; t += blockDim.x) {
+        const int i = t / n, j = t - i * n;
+        double d[3], dI = 0.0, I = 0.0;
+        if (i != j) I = gb_descreen(gb_dist(X, i, j, d), g.atom[4 * i], g.atom[4 * j + 1], &dI);
+        s.I[t] = I; s.D[t] = dI;
+    }
+}
+
+// phases 2 and 3 (after it; every thread of the block): Born radii, the pair terms, the chain-rule factors C_i
+__device__ __forceinline__ void mol_gb_radii_pairs(const MolGB &g, const double (*X)[3], const double *q, int n, const MolGBArrays &s) {
+    const int a = threadIdx.x;
+    if (a < n) {
+        double I = 0.0;
+        for (int j = 0; j < n; j++) I += s.I[a * n + j];
+        s.B[a] = gb_born(g, I, g.atom[4 * a], g.atom[4 * a + 2], &s.dB[a]);
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < n * n; t += blockDim.x) {
+        const int i = t / n, j = t - i * n;
+        if (j <= i) continue;
+        double d[3], dr, dbi, dbj;
+        const double r = gb_dist(X, i, j, d);
+        gb_pair(r * r, s.B[i], s.B[j], g.pre * q[i] * q[j], &dr, &dbi, &dbj);
+        s.P[t] = s.P[j * n + i] = dr; s.EB[t] = dbi; s.EB[j * n + i] = dbj;
+    }
+    __syncthreads();
+    if (a < n) {
+        double dEdB;
+        gb_self(g, q[a], s.B[a], g.atom[4 * a + 2], g.atom[4 * a + 3], &dEdB);
+        for (int j = 0; j < n; j++) if (j != a) dEdB += s.EB[a * n + j];
+        s.C[a] = dEdB * s.dB[a];
+    }
+    __syncwarp();
+}
+
+// U of a molecule in implicit solvent (every lane of a warp; the same bits in k_propagate_mol and k_energy_mol)
+__device__ __forceinline__ double mol_energy_gb(const MolDev &m, const MolGB &g, const MolShared &ms, const double (*X)[3], double *Bs,
+                                                double *Cs) {
+    const int a = threadIdx.x;
+    const double e_gb = mol_gb_lane<false>(g, X, ms.charge, a, m.n, Bs, Cs, nullptr);
+    return mol_warp_sum(a < m.n ? mol_atom<true, double>(ms, X, a, nullptr) + e_gb : 0.0);
+}
+
+// the GB force on atom a (warp 0, after mol_gb_radii_pairs)
+__device__ __forceinline__ void mol_gb_force(const double (*X)[3], int a, int n, const MolGBArrays &s, double *f) {
+    for (int j = 0; j < n; j++) {
+        if (j == a) continue;
+        double d[3];
+        const double r = gb_dist(X, a, j, d);
+        const double c = s.P[a * n + j] + (s.C[a] * s.D[a * n + j] + s.C[j] * s.D[j * n + a]) / r;
+        for (int q = 0; q < 3; q++) f[q] -= c * d[q];
+    }
+}
+
 // One block of MOL_WARPS warps per owned replica.  Warp 0 integrates (one lane per atom, one lane per constraint cluster);
 // all warps evaluate the force terms (each term once, by whichever thread its index falls to, into its fixed slots: the
 // per-atom sums in slot order do not depend on the number of threads -- the same bits as with one warp), between two block
 // barriers per force evaluation.  Every warp runs the same control flow (steps, program, lazy force flag); warps 1.. only take
 // part in the force evaluations.  pos / vel: double[kloc][n][3].
 #define MOL_WARPS 4
-template <bool STAR>   // STAR: every constraint cluster has at most three constraints (MolDev::max_cluster): the MolStar path
+// STAR: every constraint cluster has at most three constraints (MolDev::max_cluster): the MolStar path.
+// GB: OBC implicit solvent (g), three phases per force evaluation: the descreening integrals with the other terms, then
+// (a block barrier) Born radii, (barrier) pair terms, (barrier) chain-rule factors, then each atom's sum.
+template <bool STAR, bool GB>
 __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynParams p, const StateDev *__restrict__ states,
                                                       const int *__restrict__ perm, double *__restrict__ pos,
                                                       double *__restrict__ vel, int k0, uint2 key, uint32_t iteration,
                                                       int reassign, double *__restrict__ pot, double *__restrict__ kin,
-                                                      int *__restrict__ nan_flag, const int *__restrict__ only) {
+                                                      int *__restrict__ nan_flag, const int *__restrict__ only, MolGB g) {
     __shared__ double X[MOL_MAX_ATOMS][3], XO[MOL_MAX_ATOMS][3], V[MOL_MAX_ATOMS][3];
     extern __shared__ unsigned long long mol_tab[];
     const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
@@ -637,6 +805,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
     unsigned char *tb = (unsigned char *)mol_tab + m.shared_bytes;
     for (int q = threadIdx.x * 8; q < m.terms_bytes; q += 32 * MOL_WARPS * 8) *(unsigned long long *)(tb + q) = *(const unsigned long long *)((const unsigned char *)m.terms + q);
     float (*FS)[3] = (float (*)[3])(tb + ((m.terms_bytes + 15) & ~15));
+    const MolGBArrays gs((double *)((unsigned char *)mol_tab + m.dyn_shared_bytes), n);
     __syncthreads();
     const int *g_off = (const int *)(tb + ((const MolTerms *)tb)->o_goff);
     const bool active = a < n;
@@ -678,11 +847,14 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
                 if (!f_valid) {
                     __syncthreads();   // warp 0's positions are in shared memory
                     mol_forces_terms(m, tb, X, FS);
+                    if (GB) mol_gb_integrals(g, X, n, gs);
                     __syncthreads();   // every term's contributions are in their slots
+                    if (GB) mol_gb_radii_pairs(g, X, ms.charge, n, gs);
                     if (active) {   // this atom's slots, in slot order
                         float fx = 0.f, fy = 0.f, fz = 0.f;
                         for (int q = g_off[a]; q < g_off[a + 1]; q++) { fx += FS[q][0]; fy += FS[q][1]; fz += FS[q][2]; }
                         f[0] = fx; f[1] = fy; f[2] = fz;
+                        if (GB) mol_gb_force(X, a, n, gs, f);
                     }
                     __syncwarp();
                     f_valid = true;
@@ -718,7 +890,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
             }
         }
     }
-    const double U = mol_warp_sum(active ? mol_atom<true, double>(ms, X, a, nullptr) : 0.0);
+    const double U = GB ? mol_energy_gb(m, g, ms, X, gs.B, gs.C) : mol_warp_sum(active ? mol_atom<true, double>(ms, X, a, nullptr) : 0.0);
     const double KE = mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
     const bool bad = active && !(isfinite(X[a][0]) && isfinite(X[a][1]) && isfinite(X[a][2]) && isfinite(V[a][0]) &&
                                  isfinite(V[a][1]) && isfinite(V[a][2]));
@@ -733,8 +905,10 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
 // weights, unit-weight sweeps for clusters of more than MOL_MAXC constraints), the move is followed by SHAKE, the FIRE
 // velocity is kept tangent.  Converged when the RMS of the projected force
 // falls below tol_rms (kJ/mol/nm); f64 throughout.  (OpenMM's L-BFGS is not reproduced, as for the other systems.)
+// GB: the OBC force of g added to each atom's (mol_gb_lane, f64).
+template <bool GB>
 __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restrict__ pos, int k0, double tol_rms, int max_iter,
-                                                     double *__restrict__ rms_out, int *__restrict__ iters_out) {
+                                                     double *__restrict__ rms_out, int *__restrict__ iters_out, MolGB g) {
     __shared__ double X[MOL_MAX_ATOMS][3], XO[MOL_MAX_ATOMS][3], V[MOL_MAX_ATOMS][3], F[MOL_MAX_ATOMS][3];
     extern __shared__ unsigned long long mol_tab[];
     const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
@@ -768,6 +942,10 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
     for (;; it++) {
         double f[3] = {0, 0, 0};
         if (active) mol_atom<false, double>(ms, X, a, f);
+        if (GB) {
+            double *gbs = (double *)((unsigned char *)mol_tab + m.shared_bytes);
+            mol_gb_lane<true>(g, X, ms.charge, a, n, gbs, gbs + MOL_MAX_ATOMS, f);
+        }
         if (active) for (int c = 0; c < 3; c++) F[a][c] = f[c];
         __syncwarp();
         if (a < m.n_clusters) mol_rattle_cluster(m, a, ku, X, F, true);   // projected force
@@ -807,8 +985,10 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
 
 // u[k][l] = beta_l (U(x_k) + offset_l): the states of a molecule differ in temperature only (parallel tempering,
 // paralleltempering.py:175-237: one potential evaluation per replica, scaled by beta_l).
+// GB: with the OBC energy of g (mol_energy_gb).
+template <bool GB>
 __global__ void __launch_bounds__(32) k_energy_mol(MolDev m, const StateDev *__restrict__ states, int n_states,
-                                                   const double *__restrict__ pos, int k0, double *__restrict__ u_out) {
+                                                   const double *__restrict__ pos, int k0, double *__restrict__ u_out, MolGB g) {
     __shared__ double X[MOL_MAX_ATOMS][3];
     extern __shared__ unsigned long long mol_tab[];
     const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
@@ -817,7 +997,9 @@ __global__ void __launch_bounds__(32) k_energy_mol(MolDev m, const StateDev *__r
     mol_stage(m, (unsigned char *)mol_tab, ms);
     if (active) for (int c = 0; c < 3; c++) X[a][c] = pos[((size_t)r * n + a) * 3 + c];
     __syncwarp();
-    const double U = mol_warp_sum(active ? mol_atom<true, double>(ms, X, a, nullptr) : 0.0);
+    double *gbs = (double *)((unsigned char *)mol_tab + m.shared_bytes);
+    const double U = GB ? mol_energy_gb(m, g, ms, X, gbs, gbs + MOL_MAX_ATOMS)
+                        : mol_warp_sum(active ? mol_atom<true, double>(ms, X, a, nullptr) : 0.0);
     for (int l = a; l < n_states; l += 32) u_out[(size_t)k * n_states + l] = states[l].beta * (U + states[l].offset);
 }
 

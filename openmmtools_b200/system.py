@@ -50,6 +50,10 @@ class System:
         self.exceptions = None     # float64[nx, 5]  i, j, q_i q_j (scaled), sigma, epsilon (scaled): the 1-4 pairs
         self.constraints = None    # float64[nc, 3]  i, j, distance (nm)
         self.remove_cm_motion = False
+        # -- OBC generalized Born implicit solvent (GBSAOBCForce, createSystem(implicitSolvent=OBC1|OBC2)); None: vacuum
+        self.gb_radius = None      # float64[n]  radius (nm)
+        self.gb_scale = None       # float64[n]  screening factor
+        self.gb_parameters = None  # (alpha, beta, gamma, offset, solute dielectric, solvent dielectric, sa_energy, probe radius)
         # -- OpenMM-style global parameters with their defaults (read by GlobalParameterState.from_system)
         self.global_parameters = {}
 
@@ -112,6 +116,10 @@ class System:
                       self.exceptions, self.constraints):
                 h.update(np.asarray(a, dtype=np.float64).tobytes())
             h.update(repr(self.remove_cm_motion).encode())
+            if getattr(self, 'gb_radius', None) is not None:   # (vacuum systems keep their hash)
+                for a in (self.gb_radius, self.gb_scale):
+                    h.update(np.asarray(a, dtype=np.float64).tobytes())
+                h.update(repr(tuple(float(v) for v in self.gb_parameters)).encode())
         return h.hexdigest()
 
     def __getstate__(self):

@@ -3,8 +3,9 @@
 Mirrors /root/reference/openmmtools/testsystems.py: ``HarmonicOscillator`` (:685-840) and
 ``LennardJonesFluid`` (:1872-2030) with the same constructor arguments, defaults and derived quantities
 (box edge from the reduced density, cutoff 3 sigma, switching distance cutoff - switch_width, sub-random
-initial positions), and ``AlanineDipeptideVacuum`` (:3352-3388) from the reference's AMBER input files (``amber.py``; the
-parsed parameters ship as data/alanine_dipeptide_vacuum.json).  The other reference systems are out of scope.
+initial positions), ``AlanineDipeptideVacuum`` (:3352-3388) and ``AlanineDipeptideImplicit`` (:3422-3459), and the toluene
+systems (:3533-3636) from the reference's AMBER input files (``amber.py``; the parsed parameters ship as data/*.json).  The
+other reference systems are out of scope.
 """
 import numpy as np
 from . import unit
@@ -127,6 +128,40 @@ class LennardJonesFluid(TestSystem):
         self.reduced_density = reduced_density
 
 
+def _load_data(name):
+    import json, os
+    return json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'data', name)))
+
+
+def _molecule(d, constraints, hydrogenMass):
+    """The System createSystem(constraints=constraints, nonbondedCutoff=None) builds from the parsed prmtop d (vacuum)."""
+    if hydrogenMass is not None:
+        raise NotImplementedError('hydrogen mass repartitioning is not provided')
+    name = getattr(constraints, '__name__', constraints)
+    if name not in ('HBonds', None):
+        raise NotImplementedError("constraints must be 'HBonds' or None")
+    system = System(MOLECULE, d['mass'])
+    system.charge = np.array(d['charge']); system.sigma = np.array(d['sigma']); system.epsilon = np.array(d['epsilon'])
+    hb = name == 'HBonds'
+    system.bonds = np.array([[b[0], b[1], b[2], b[3]] for b in d['bonds'] if not (hb and b[4])], dtype=np.float64).reshape(-1, 4)
+    system.constraints = np.array([[b[0], b[1], b[3]] for b in d['bonds'] if hb and b[4]], dtype=np.float64).reshape(-1, 3)
+    system.angles = np.array(d['angles'], dtype=np.float64).reshape(-1, 5)
+    system.torsions = np.array(d['torsions'], dtype=np.float64).reshape(-1, 7)
+    system.exclusions = np.array(d['exclusions'], dtype=np.int64).reshape(-1, 2)
+    system.exceptions = np.array(d['exceptions'], dtype=np.float64).reshape(-1, 5)
+    system.remove_cm_motion = True     # createSystem(removeCMMotion=True) is the default
+    return system
+
+
+def _add_obc(system, gb, **create_system_kwargs):
+    """createSystem(implicitSolvent=...): the file's GB radii and screening factors with the model's parameters."""
+    from .amber import obc_parameters
+    system.gb_parameters = obc_parameters(**create_system_kwargs)
+    system.gb_radius = np.array(gb['radii'], dtype=np.float64)
+    system.gb_scale = np.array(gb['screen'], dtype=np.float64)
+    return system
+
+
 class AlanineDipeptideVacuum(TestSystem):
     """Alanine dipeptide (ff96) in vacuum (testsystems.py:3352-3388): what AmberPrmtopFile.createSystem(implicitSolvent=None,
     constraints=constraints, nonbondedCutoff=None) builds from alanine-dipeptide.prmtop -- harmonic bonds and angles, periodic
@@ -137,26 +172,78 @@ class AlanineDipeptideVacuum(TestSystem):
 
     def __init__(self, constraints='HBonds', hydrogenMass=None, **kwargs):
         TestSystem.__init__(self, **kwargs)
-        import json, os
-        if hydrogenMass is not None:
-            raise NotImplementedError('hydrogen mass repartitioning is not provided')
-        name = getattr(constraints, '__name__', constraints)
-        if name not in ('HBonds', None):
-            raise NotImplementedError("constraints must be 'HBonds' or None")
-        d = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'data', 'alanine_dipeptide_vacuum.json')))
-        system = System(MOLECULE, d['mass'])
-        system.charge = np.array(d['charge']); system.sigma = np.array(d['sigma']); system.epsilon = np.array(d['epsilon'])
-        hb = name == 'HBonds'
-        system.bonds = np.array([[b[0], b[1], b[2], b[3]] for b in d['bonds'] if not (hb and b[4])], dtype=np.float64).reshape(-1, 4)
-        system.constraints = np.array([[b[0], b[1], b[3]] for b in d['bonds'] if hb and b[4]], dtype=np.float64).reshape(-1, 3)
-        system.angles = np.array(d['angles'], dtype=np.float64).reshape(-1, 5)
-        system.torsions = np.array(d['torsions'], dtype=np.float64).reshape(-1, 7)
-        system.exclusions = np.array(d['exclusions'], dtype=np.int64).reshape(-1, 2)
-        system.exceptions = np.array(d['exceptions'], dtype=np.float64).reshape(-1, 5)
-        system.remove_cm_motion = True     # createSystem(removeCMMotion=True) is the default
-        self.system = system
+        d = _load_data('alanine_dipeptide_vacuum.json')
+        self.system = _molecule(d, constraints, hydrogenMass)
         self.positions = unit.Quantity(np.array(d['positions'], dtype=np.float64), unit.nanometer)
         self.atom_names = list(d['names'])
+
+
+class AlanineDipeptideImplicit(TestSystem):
+    """Alanine dipeptide (ff96) in OBC1 implicit solvent (testsystems.py:3422-3459): AlanineDipeptideVacuum's force field
+    plus the GB model createSystem(implicitSolvent=OBC1) adds -- the prmtop's mbondi2 radii and screening factors, solvent
+    dielectric 78.5, the ACE non-polar term.
+
+    ``constraints``: 'HBonds' (the reference default, app.HBonds) or None."""
+
+    def __init__(self, constraints='HBonds', hydrogenMass=None, **kwargs):
+        TestSystem.__init__(self, **kwargs)
+        d = _load_data('alanine_dipeptide_vacuum.json')
+        self.system = _add_obc(_molecule(d, constraints, hydrogenMass), _load_data('alanine_dipeptide_implicit.json'),
+                               implicitSolvent='OBC1')
+        self.positions = unit.Quantity(np.array(d['positions'], dtype=np.float64), unit.nanometer)
+        self.atom_names = list(d['names'])
+
+
+class TolueneVacuum(TestSystem):
+    """Toluene GAFF/AM1-BCC in vacuum (testsystems.py:3533-3562), from benzene-toluene-implicit/solvent.{prmtop,inpcrd}."""
+
+    def __init__(self, constraints='HBonds', hydrogenMass=None, **kwargs):
+        TestSystem.__init__(self, **kwargs)
+        d = _load_data('toluene_implicit.json')
+        self.system = _molecule(d, constraints, hydrogenMass)
+        self.positions = unit.Quantity(np.array(d['positions'], dtype=np.float64), unit.nanometer)
+        self.atom_names = list(d['names'])
+
+
+class TolueneImplicit(TestSystem):
+    """Toluene GAFF/AM1-BCC in implicit solvent (testsystems.py:3568-3620): createSystem(**kwargs) with the defaults
+    implicitSolvent=OBC1, constraints=HBonds, nonbondedMethod=NoCutoff; the prmtop's mbondi radii.  OBC1 and OBC2 are
+    provided; HCT, GBn, GBn2, salt and cutoffs raise NotImplementedError."""
+
+    def __init__(self, **kwargs):
+        TestSystem.__init__(self)
+        kw = dict(implicitSolvent='OBC1', constraints='HBonds', hydrogenMass=None)
+        kw.update(kwargs)
+        d = _load_data('toluene_implicit.json')
+        constraints, hydrogenMass = kw.pop('constraints'), kw.pop('hydrogenMass')
+        self.system = _add_obc(_molecule(d, constraints, hydrogenMass), d, **kw)
+        self.positions = unit.Quantity(np.array(d['positions'], dtype=np.float64), unit.nanometer)
+        self.atom_names = list(d['names'])
+
+
+class TolueneImplicitHCT(TolueneImplicit):
+    def __init__(self, **kwargs):
+        TolueneImplicit.__init__(self, implicitSolvent='HCT', **kwargs)
+
+
+class TolueneImplicitOBC1(TolueneImplicit):
+    def __init__(self, **kwargs):
+        TolueneImplicit.__init__(self, implicitSolvent='OBC1', **kwargs)
+
+
+class TolueneImplicitOBC2(TolueneImplicit):
+    def __init__(self, **kwargs):
+        TolueneImplicit.__init__(self, implicitSolvent='OBC2', **kwargs)
+
+
+class TolueneImplicitGBn(TolueneImplicit):
+    def __init__(self, **kwargs):
+        TolueneImplicit.__init__(self, implicitSolvent='GBn', **kwargs)
+
+
+class TolueneImplicitGBn2(TolueneImplicit):
+    def __init__(self, **kwargs):
+        TolueneImplicit.__init__(self, implicitSolvent='GBn2', **kwargs)
 
 
 class LennardJonesGrid(TestSystem):   # pragma: no cover

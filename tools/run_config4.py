@@ -1,6 +1,8 @@
 """BASELINE.json configs[3]: T-REMD of testsystems.AlanineDipeptideVacuum, 128 temperature replicas 300-600 K, 1000 steps per
 iteration (ParallelTemperingSampler, swap-all), timed on one GPU; energies of the final configurations checked against the
-oracle.  usage: run_config4.py [iterations [K [n_steps]]]"""
+oracle.  usage: run_config4.py [--implicit] [iterations [K [n_steps]]]
+--implicit: AlanineDipeptideImplicit (OBC1 implicit solvent) in place of the vacuum system.  The card's name and power limit
+are printed with the times."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -14,13 +16,21 @@ if world > 1:
 if rank != 0:
     sys.stdout = open(os.devnull, 'w')
 from openmmtools_b200 import testsystems, states, mcmc, multistate, unit
-from oracle import oracle
+from oracle import oracle, implicit as oracle_implicit
 
+implicit = '--implicit' in sys.argv
+sys.argv = [v for v in sys.argv if v != '--implicit']
 n_it = int(sys.argv[1]) if len(sys.argv) > 1 else 10
 K = int(sys.argv[2]) if len(sys.argv) > 2 else 128
 n_steps = int(sys.argv[3]) if len(sys.argv) > 3 else 1000
 KB = 8.31446261815324e-3
-a = testsystems.AlanineDipeptideVacuum()
+a = testsystems.AlanineDipeptideImplicit() if implicit else testsystems.AlanineDipeptideVacuum()
+try:
+    import subprocess
+    print('card:', subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True,
+                                  text=True).stdout.strip().splitlines()[0], '| system:', type(a).__name__)
+except (OSError, IndexError):
+    print('card: unknown | system:', type(a).__name__)
 ts = states.ThermodynamicState(a.system, 300.0 * unit.kelvin)
 move = mcmc.LangevinSplittingDynamicsMove(timestep=2.0 * unit.femtosecond, collision_rate=5.0 / unit.picosecond, n_steps=n_steps)
 s = multistate.ParallelTemperingSampler(mcmc_moves=move, number_of_iterations=10 ** 9, seed=7)
@@ -39,7 +49,7 @@ print('config 4: K=%d, %d steps/iteration: %.2f ms per iteration (%.1f iteration
 e.phase_times(reset=True)
 t0 = time.time(); e.run_iterations(n_it, 'swap-all', s._seed, s._iteration + 1); dt = time.time() - t0
 print('fused device loop: %.2f ms per iteration (%.1f iterations/s)' % (1e3 * dt / n_it, n_it / dt))
-m = oracle.Molecule(a.system)
+m = (oracle_implicit if implicit else oracle).Molecule(a.system)
 T = np.array([st.temperature.value_in_unit(unit.kelvin) for st in s._thermodynamic_states])
 s._states_stale = True
 u = e.compute_energies()
