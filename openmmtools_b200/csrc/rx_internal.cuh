@@ -46,7 +46,7 @@ struct MixCtl {          // device-resident control block of the resumable mixin
     int rounds;          // statistics: speculation rounds executed
     long long slow_exp;  // statistics: exact exp() fallbacks
     long long log_count; // entries written to the commit log by this launch
-    long long aux;       // k_mix_walk2c: candidate index reached (extent of its sparse commit log)
+    long long aux;       // k_mix_walk2 / k_mix_walk2c: record reached (extent of their sparse commit log)
 };
 
 struct rx_state_move {

@@ -416,16 +416,9 @@ __global__ void __launch_bounds__(64) k_mix_walk_pow2(const SlotRec *__restrict_
             resolve();
             if (U & cm) {
                 if (undecided) {   // exact path for this lane: the f64 values from L2
-                    const unsigned a_ii = (i << logK) | (unsigned)si, a_jj = (j << logK) | (unsigned)sj;
-                    const double logp = swap_logp(u[a_ij], u[a_ji], u[a_ii], u[a_jj]);
-                    ge0 = logp >= 0.0;
-                    acc = ge0;
-                    if (!ge0) {
-                        const double dd = logp - (REC2 ? slot_logU(words, h + lane + 1) : rec[h + lane + 1].logU);
-                        if (dd > 1e-9) acc = true;
-                        else if (dd < -1e-9) acc = false;
-                        else { const unsigned s1 = h + lane + 1; acc = mt_double(words[2 * (size_t)s1], words[2 * (size_t)s1 + 1]) < rx_exp_cr(logp); }
-                    }
+                    const unsigned d = w2_exact_decision(u, K, ij, (unsigned)si, (unsigned)sj, words, 2 * (size_t)(h + lane + 1));
+                    ge0 = (d & 1u) != 0u;
+                    acc = (d & 2u) != 0u;
                     slow++;
                 }
                 resolve();
@@ -738,6 +731,12 @@ struct MixTrace {   // RX_TRACE_MIX=1: device-time breakdown of one swap-all cal
 
 static inline bool is_pow2(int k) { return k >= 2 && (k & (k - 1)) == 0; }
 
+// grid of the count kernels over n log entries: one thread per entry, at most 16 blocks per SM (grid-stride loop)
+static inline unsigned count_blocks(const rx_engine *h, long long n) {
+    const long long nb = (n + 255) / 256;
+    return (unsigned)(nb < h->n_sm * 16 ? nb : h->n_sm * 16);
+}
+
 enum { REC_NONE = 0, REC_SLOT = 1, REC_SLOT2 = 2, REC_WORD = 3, REC_CAND = 4 };   // what prepare_pass builds from the stream
 
 static inline size_t pass_need(long long remaining, bool fast, bool anyk = false) {
@@ -848,14 +847,13 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
     // filter mode: 16-byte SlotRec2 records, k_mix_walk2 for the bulk of a pass and k_mix_walk_pow2<U_FILTER24, true> for its tail
     const bool rec2 = (umode == U_FILTER24);
     const bool walk2 = rec2 && !getenv("RX_WALK_V1");
-    // any K <= 256 whose row image fits: the walker of k_mix_walk2 in candidate coordinates (rx_walk2c.cuh);
+    // any K <= 256 whose row image fits: the walker of k_mix_walk2 in candidate coordinates (k_mix_walk2c, rx_walk2c.cuh);
     // RX_WALK_ANY_V1=1 keeps the word-position walker (cross-check)
-    const size_t smem_w2c = (size_t)W2_RING * 16 + (size_t)K * 8 + (size_t)((3 * K + 1) & ~1) * K;
-    const bool candk = anyk && K <= 256 && smem_w2c <= 224 * 1024 && !getenv("RX_WALK_ANY_V1") && !getenv("RX_NO_FILTER");
+    const size_t smem_w2 = (size_t)W2_RING * 16 + (size_t)K * 8 + (size_t)((3 * K + 1) & ~1) * K;   // ring, replicas, image
+    const bool candk = anyk && K <= 256 && smem_w2 <= 224 * 1024 && !getenv("RX_WALK_ANY_V1") && !getenv("RX_NO_FILTER");
     const int kind = candk ? REC_CAND : (anyk ? REC_WORD : (!fast ? REC_NONE : (rec2 ? REC_SLOT2 : REC_SLOT)));
     const size_t smem_any_f64 = smem_base + (size_t)K * K * sizeof(double);
     const bool any_smem = anyk && smem_any_f64 <= 200 * 1024;
-    const size_t smem_w2 = (size_t)W2_RING * 16 + (size_t)K * 8 + (size_t)3 * K * K;
     size_t smem = !fast ? smem_small : (umode == U_F64_SMEM ? smem_f64 : (umode == U_FILTER24 ? smem_f24 : smem_base));
     // The walker is one latency-bound CTA: claim (almost) a whole SM's shared memory so that no other CTA -- in particular
     // the stream generator that runs concurrently on the side stream -- is scheduled onto the same SM and steals issue slots.
@@ -891,6 +889,24 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         (*launches)++;
     }
     tr.mark("filter build");
+    // The filter walker (k_mix_walk2 over slots, k_mix_walk2c over candidate indices) takes the bulk of a pass.  It logs the
+    // attempts it commits sparsely, one word per record (zero = no attempt started there), and reports the extent of that
+    // log in ctl.aux; the pass's tail kernel continues from ctl.head.  Both claim a whole SM like the other walkers.
+    auto filter_walk = [&](size_t nrec) -> int {
+        static_assert(sizeof(SlotRec2) == sizeof(SlotRec), "both record formats share the d_slots buffer");
+        if (smem_w2 > 226 * 1024) RX_FAIL(h, RX_ERR_INVALID, "internal: filter walker shared memory");
+        RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, nrec * sizeof(uint32_t), h->stream));
+        if (candk)
+            k_mix_walk2c<<<1, W2_THREADS, 226 * 1024, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos,
+                                                                    h->d_ctile + (h->ctile_cap / CAND_TILE + 4), h->d_u, K, h->d_perm,
+                                                                    h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
+        else
+            k_mix_walk2<<<1, W2_THREADS, 226 * 1024, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K,
+                                                                   logK, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
+        RX_CHECK_CUDA(h, cudaGetLastError());
+        *launches += 1;
+        return RX_OK;
+    };
     long long remaining = nswap;
     h->mix_stats[0] = h->mix_stats[1] = h->mix_stats[2] = h->mix_stats[4] = h->mix_stats[5] = 0;
     const uint64_t consumed0 = S.consumed;
@@ -932,15 +948,7 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
             if (umode == U_F64_SMEM)
                 k_mix_walk_pow2<U_F64_SMEM><<<1, 64, smem, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, nullptr, nullptr, h->d_ctl);
             else if (umode == U_FILTER24) {
-                if (walk2) {
-                    static_assert(sizeof(SlotRec2) == sizeof(SlotRec), "both record formats share the d_slots buffer");
-                    if (smem_w2 > smem) RX_FAIL(h, RX_ERR_INVALID, "internal: k_mix_walk2 shared memory");
-                    // sparse commit log: one word per slot, zero = no attempt started there
-                    RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, (size_t)nslots * sizeof(uint32_t), h->stream));
-                    k_mix_walk2<<<1, W2_THREADS, smem, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
-                    RX_CHECK_CUDA(h, cudaGetLastError());
-                    *launches += 1;
-                }
+                if (walk2 && (rc = filter_walk((size_t)nslots))) return rc;
                 k_mix_walk_pow2<U_FILTER24, true><<<1, 64, smem, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, h->d_filt, h->d_filt_scale, h->d_ctl);
             }
             else
@@ -957,32 +965,12 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
                 RX_CHECK_CUDA(h, cudaStreamWaitEvent(h->stream, h->ev_prepared, 0));
                 S.avail += ahead;
             }
-            if (walk2 && ctl.head > 0) {
-                long long nb = (ctl.head + 255) / 256;
-                if (nb > h->n_sm * 16) nb = h->n_sm * 16;
-                k_mix_count_slots<<<(unsigned)nb, 256, 0, h->stream>>>(h->d_slotlog, 0, ctl.head, M, h->d_nacc, h->d_nprop);
-                RX_CHECK_CUDA(h, cudaGetLastError());
-                *launches += 1;
-            }
-            if (ctl.log_count > 0) {
-                long long nb = (ctl.log_count + 255) / 256;
-                if (nb > h->n_sm * 16) nb = h->n_sm * 16;
-                k_mix_count<<<(unsigned)nb, 256, 0, h->stream>>>(h->d_log, ctl.log_count, M, h->d_nacc, h->d_nprop);
-                RX_CHECK_CUDA(h, cudaGetLastError());
-                *launches += 1;
-            }
-            tr.mark("adopt-ahead + count");
         } else {
             if (candk) {
-                // bulk of the pass: the walk2 organisation over candidate indices; the plain loop below finishes the pass
+                // bulk of the pass: the filter walker over candidate indices; the plain loop below finishes the pass
                 RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
-                RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, S.avail * sizeof(uint32_t), h->stream));
-                k_mix_walk2c<<<1, W2_THREADS, 226 * 1024, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos,
-                                                                        h->d_ctile + (h->ctile_cap / CAND_TILE + 4), h->d_u, K, h->d_perm,
-                                                                        h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
-                RX_CHECK_CUDA(h, cudaGetLastError());
+                if ((rc = filter_walk(S.avail))) return rc;
                 RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
-                *launches += 1;
             } else if (anyk) {
                 // bulk of the pass: speculative walker over word positions (claims the SM like the power-of-two walkers);
                 // what it leaves -- the last words of the pass -- is finished by the plain loop below
@@ -1005,22 +993,20 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
             if (anyk) {
                 float wms = 0;
                 if (cudaEventElapsedTime(&wms, h->ev_walk[0], h->ev_walk[1]) == cudaSuccess) h->mix_stats[4] += (long long)(wms * 1e3f);
-                if (candk && ctl.aux > 0) {
-                    long long nb = (ctl.aux + 255) / 256;
-                    if (nb > h->n_sm * 16) nb = h->n_sm * 16;
-                    k_mix_count_slots<<<(unsigned)nb, 256, 0, h->stream>>>(h->d_slotlog, 0, ctl.aux, M, h->d_nacc, h->d_nprop);
-                    RX_CHECK_CUDA(h, cudaGetLastError());
-                    *launches += 1;
-                }
-                if (!candk && ctl.log_count > 0) {
-                    long long nb = (ctl.log_count + 255) / 256;
-                    if (nb > h->n_sm * 16) nb = h->n_sm * 16;
-                    k_mix_count<<<(unsigned)nb, 256, 0, h->stream>>>(h->d_log, ctl.log_count, M, h->d_nacc, h->d_nprop);
-                    RX_CHECK_CUDA(h, cudaGetLastError());
-                    *launches += 1;
-                }
             }
         }
+        // count matrices from the commit logs (k_mix_walk_serial counts as it goes)
+        if (ctl.aux > 0) {   // the filter walker's sparse log
+            k_mix_count_slots<<<count_blocks(h, ctl.aux), 256, 0, h->stream>>>(h->d_slotlog, 0, ctl.aux, M, h->d_nacc, h->d_nprop);
+            RX_CHECK_CUDA(h, cudaGetLastError());
+            *launches += 1;
+        }
+        if (ctl.log_count > 0) {   // the dense log of k_mix_walk_pow2 / k_mix_walk_any
+            k_mix_count<<<count_blocks(h, ctl.log_count), 256, 0, h->stream>>>(h->d_log, ctl.log_count, M, h->d_nacc, h->d_nprop);
+            RX_CHECK_CUDA(h, cudaGetLastError());
+            *launches += 1;
+        }
+        tr.mark("adopt-ahead + count");
         if (ctl.remaining == remaining && consumed_words == 0 && need >= chunk_words)
             RX_FAIL(h, RX_ERR_INVALID, "internal: mixing made no progress");
         remaining = ctl.remaining;

@@ -1,4 +1,5 @@
-// rx_walk2c.cuh -- the walker of k_mix_walk2 for ANY K <= 256 (included by rx_mix.cu after rx_walk2.cuh).
+// rx_walk2c.cuh -- candidate coordinates for the filter walker k_mix_walk2c (rx_walk2.cuh) at ANY K <= 256 (included by
+// rx_mix.cu after rx_walk2.cuh).
 //
 // For K that is not a power of two numba's randint rejects words (numba/_random.c: low bit_length(K-1) bits of one word,
 // retried while >= K), so attempts have no fixed length in the word stream.  In CANDIDATE coordinates they do: let the
@@ -8,18 +9,8 @@
 // candidate c+1, and the next attempt starts at c + 2 + k, where k in {0, 1, 2} counts the candidates among those two
 // words -- a property of the stream alone.  So a state-independent pre-pass (flag, scan, scatter, records) gives one
 // 16-byte record per candidate index {i | j << 16, back-mask, f32 log-uniform of this attempt, k}, and the walker is
-// k_mix_walk2 with a window of 32 candidate indices and hops of 2, 3 or 4 instead of 1 or 2 (replicaexchange.py:321-349
-// bit for bit, like every other walker here).
-//
-// The visited chain for hops {2, 3, 4}.  With T = positions that would hop 3 (log_p < 0, k = 1) and F = positions that
-// would hop 4 (log_p < 0, k = 2): on ONE parity class ("grid") of positions the chain is the power-of-two chain (hop 2 =
-// next grid position, hop 4 = skip one), solved for all positions at once by the add-carry trick of k_mix_walk_pow2 on
-// stride-2 masks (the bit between two grid positions of an F-run is filled so that the carry runs through).  A visited T
-// switches to the other grid; there the steady-state pattern holds from the entry position on unless the steady state
-// skips the entry position, in which case the pattern of the F-run that contains it is complemented.  One grid phase per
-// visited T (a uniform loop: all masks are warp-wide values); a visited position whose hop would leave the window by more
-// than one position ends the round (a lane moves on by one window per round at most).  tests/test_walk_cand_logic_model.py is the
-// lane-level CPU model of this logic.
+// the one of k_mix_walk2 with a window of 32 candidate indices and hops of 2, 3 or 4 instead of 1 or 2 (its visited chain:
+// w2_chain_cand; replicaexchange.py:321-349 bit for bit, like every other walker here).
 #pragma once
 
 #define CAND_TILE 2048    // words per block of the flag/scan/scatter pre-pass
@@ -120,283 +111,6 @@ __global__ void __launch_bounds__(256) k_cand_records(const uint32_t *__restrict
     r.ij = i | (j << 16);
     r.backmask = bm;
     r.lu_next = __float_as_uint((float)((U == 0.0) ? LOGU_ZERO : log(U)));
-    r.alts = k;
+    r.k = k;
     rec[c] = r;
-}
-
-// The exact decision for the attempt at candidate index c under the states (si, sj): bit 0 = log_p >= 0, bit 1 = accepted.
-__device__ __noinline__ unsigned w2c_exact_decision(const SlotRec2 *__restrict__ rec, const uint32_t *__restrict__ words,
-                                                    const uint32_t *__restrict__ cpos, const double *__restrict__ u, unsigned c,
-                                                    unsigned si, unsigned sj, int K) {
-    const unsigned ij = rec[c].ij;
-    const size_t rowi = (size_t)(ij & 0xffffu) * K, rowj = (size_t)(ij >> 16) * K;
-    const double logp = swap_logp(u[rowi + sj], u[rowj + si], u[rowi + si], u[rowj + sj]);
-    if (logp >= 0.0) return 3u;
-    const size_t a = (size_t)cpos[c + 1] + 1;
-    const double U = mt_double(words[a], words[a + 1]);
-    const double dd = logp - ((U == 0.0) ? LOGU_ZERO : log(U));
-    bool acc;
-    if (dd > 1e-9) acc = true;
-    else if (dd < -1e-9) acc = false;
-    else acc = U < rx_exp_cr(logp);
-    return acc ? 2u : 0u;
-}
-
-// Visited chain of one window for hops {2, 3, 4} (window-order masks; see the header).  V: visited positions, valid below
-// and at the lowest bit of the returned forced stops Cf (visited positions at which the next round has to start).
-__device__ __forceinline__ void w2c_chain(unsigned Gw, unsigned K1w, unsigned K2w, unsigned &V, unsigned &Cf) {
-    const unsigned NG = ~Gw;
-    const unsigned T = NG & K1w, F = NG & K2w;
-    // steady state of both grids (every F-run assumed to start visited)
-    const unsigned XgE = F & 0x55555555u, XgO = F & 0xAAAAAAAAu;
-    const unsigned XpE = XgE | (XgE << 1), XpO = XgO | (XgO << 1);
-    const unsigned stE = XgE & ~(XgE << 2), stO = XgO & ~(XgO << 2);
-    const unsigned sEa = XpE + (stE & 0x11111111u), sEb = XpE + (stE & 0x44444444u);
-    const unsigned sOa = XpO + (stO & 0x22222222u), sOb = XpO + (stO & 0x88888888u);
-    const unsigned VE = 0x55555555u & ~(((sEa ^ XpE) & 0x44444444u) | ((sEb ^ XpE) & 0x11111111u));
-    const unsigned VO = 0xAAAAAAAAu & ~(((sOa ^ XpO) & 0x88888888u) | ((sOb ^ XpO) & 0x22222222u));
-    // one grid phase per visited T: from position s on the current grid up to its first visited T; the F-run that contains
-    // s is complemented if the steady state skips s (never the case for position 0: bit 0 of VE is set)
-    unsigned Vc = VE, Xc = XpE, gc = 0x55555555u, Vn = VO, Xn = XpO, gn = 0xAAAAAAAAu;
-    unsigned s = 1u;
-    V = 0u;
-    for (;;) {
-        const unsigned R = ((Xc + s) ^ Xc) & gc;
-        const unsigned Vg = (Vc ^ ((s & ~Vc) ? R : 0u)) & ~(s - 1u);
-        const unsigned Tv = Vg & T, t = Tv & (0u - Tv);
-        V |= Vg & ((t << 1) - 1u);          // t == 0 -> all
-        s = t << 3;                          // entry of the other grid (0: no further switch inside the window)
-        if (s == 0u) break;
-        unsigned x;
-        x = Vc; Vc = Vn; Vn = x;
-        x = Xc; Xc = Xn; Xn = x;
-        x = gc; gc = gn; gn = x;
-    }
-    // The next round has to start inside the window or right behind it (a lane moves on by one window per round at most): a
-    // visited position p ends the round if p + hop(p) > 32 -- position 31 always, 30 unless it hops 2, 29 if it hops 4.  The
-    // chain's last visited position either is such a position or hops to 32 exactly (then the whole window commits).
-    Cf = V & (0x80000000u | ((T | F) & 0x40000000u) | (F & 0x20000000u));
-}
-
-__global__ void __launch_bounds__(W2_THREADS) k_mix_walk2c(const SlotRec2 *__restrict__ rec, const uint32_t *__restrict__ words,
-                                                   const uint32_t *__restrict__ cpos, const uint32_t *__restrict__ ncand_p,
-                                                   const double *__restrict__ u, int K, int *__restrict__ perm_g,
-                                                   uint32_t *__restrict__ slot_log, const unsigned char *__restrict__ filt,
-                                                   const double *__restrict__ filt_rowabs, MixCtl *ctl) {
-    extern __shared__ uint4 s_w2[];
-    __shared__ unsigned long long s_ptrs[2];               // global base pointers of the round loop (see k_mix_walk2)
-    uint4 *s_ring = s_w2;                                  // [W2_RING] records
-    W2Replica *s_rep = (W2Replica *)(s_ring + W2_RING);    // [K]
-    unsigned char *s_q = (unsigned char *)(s_rep + K);     // image rows: u16 plane (2K bytes), u8 plane (K bytes), padded to even
-    const unsigned row_bytes = (3u * (unsigned)K + 1u) & ~1u, lo_off = 2u * (unsigned)K;
-    const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    {
-        const unsigned short *ghi = (const unsigned short *)filt;
-        const unsigned char *glo = filt + 2 * (size_t)K * K;
-        for (int row = warp; row < K; row += W2_THREADS / 32) {
-            unsigned char *rowp = s_q + (size_t)row_bytes * row;
-            for (int col = lane; col < K; col += 32) {
-                ((unsigned short *)rowp)[col] = ghi[(size_t)row * K + col];
-                rowp[lo_off + col] = glo[(size_t)row * K + col];
-            }
-        }
-    }
-    if (tid == 0) { s_ptrs[0] = (unsigned long long)__cvta_generic_to_global(slot_log); s_ptrs[1] = (unsigned long long)rec; }
-    __syncthreads();
-    float rowabs_max = 0.f;
-    for (int q = tid; q < K; q += W2_THREADS) {
-        W2Replica e;
-        e.state = perm_g[q];
-        const unsigned char *rowp = s_q + (size_t)row_bytes * q;
-        e.diag = __uint_as_float(__byte_perm((unsigned)((const unsigned short *)rowp)[e.state], (unsigned)rowp[lo_off + e.state], 0x1045));
-        s_rep[q] = e;
-    }
-    for (int q = lane; q < K; q += 32)
-        rowabs_max = fmaxf(rowabs_max, __fmul_ru(1.6e-14f, __fadd_ru(__double2float_ru(fabs(filt_rowabs[q])), 0.5f)));
-    for (int o = 16; o; o >>= 1) rowabs_max = fmaxf(rowabs_max, __shfl_xor_sync(0xffffffffu, rowabs_max, o));
-    const float eps_rows = __fadd_ru(__fadd_ru(rowabs_max, rowabs_max), 1e-9f);
-    __syncthreads();
-    if (warp != 0) return;
-    const uint4 *__restrict__ recs = (const uint4 *)rec;
-
-    const unsigned ncand = *ncand_p;
-    const unsigned nslots = ncand >= 3u ? ncand - 3u : 0u;   // records exist for c < ncand - 3
-    unsigned h = 0;                                          // a pass starts at candidate 0 (word position ctl->head == 0)
-    const long long remaining0 = ctl->remaining;
-    unsigned rem = remaining0 > 0x7fffffffLL ? 0x7fffffffu : (unsigned)remaining0;
-    const unsigned rem0 = rem;
-    unsigned rounds = 0, slow = 0;
-    const unsigned h_end = nslots >= 1200u ? nslots - 560u : 0u;
-    if (ctl->head == 0 && rem >= 130 && nslots >= 1200u && h + 99u <= h_end) {
-        const unsigned ring_base = __shfl_sync(0xffffffffu, (unsigned)__cvta_generic_to_shared((const void *)s_ring), 0);
-        const unsigned rep_base = __shfl_sync(0xffffffffu, (unsigned)__cvta_generic_to_shared((const void *)s_rep), 0);
-        const unsigned img_base = __shfl_sync(0xffffffffu, (unsigned)__cvta_generic_to_shared((const void *)s_q), 0);
-        unsigned r = h & 31u;                           // lane of window position 0
-        unsigned w = ((unsigned)lane - h) & 31u;        // this lane's window position
-        unsigned sA = h + w;                            // this lane's candidate index
-        const uint2 pl = w2_lds64((unsigned)__cvta_generic_to_shared((const void *)&s_ptrs[0]));
-        const uint2 pr = w2_lds64((unsigned)__cvta_generic_to_shared((const void *)&s_ptrs[1]));
-        const unsigned long long slot_log_r = ((unsigned long long)pl.y << 32) | pl.x;
-        const uint4 *recs_r = (const uint4 *)(((unsigned long long)pr.y << 32) | pr.x);
-        unsigned bmA, neqA, rowiA, rowjA, repiA, repjA, kA;
-        float luA, epsA;
-        unsigned iB, jB, repiB, repjB;
-        auto ahead = [&](const uint4 q) {
-            iB = q.x & 0xffffu; jB = q.x >> 16;
-            repiB = rep_base + (iB << 3); repjB = rep_base + (jB << 3);
-        };
-        for (unsigned k = 0; k < 16u; k++) w2_cp_async16(ring_base + (((sA + 32u * k) & (W2_RING - 1)) << 4), recs + (sA + 32u * k));
-        w2_cp_async_commit();
-        w2_cp_async_wait<0>();
-        __syncwarp();
-        {
-            const uint4 q = w2_lds128(ring_base + ((sA & (W2_RING - 1)) << 4));
-            const unsigned i = q.x & 0xffffu, j = q.x >> 16;
-            bmA = q.y; luA = __uint_as_float(q.z); kA = q.w;
-            neqA = i != j ? 0xffffffffu : 0u;
-            epsA = i != j ? eps_rows : -1e30f;
-            rowiA = img_base + i * row_bytes; rowjA = img_base + j * row_bytes;
-            repiA = rep_base + (i << 3); repjA = rep_base + (j << 3);
-        }
-        unsigned ridxB = (sA + 32u) & (W2_RING - 1);   // ring entry of the next record of this lane
-        uint4 qB = w2_lds128(ring_base + (ridxB << 4));
-        ahead(qB);
-        uint2 ei = w2_lds64(repiA), ej = w2_lds64(repjA);   // {state, diag} of both replicas
-        unsigned p_cm = 0, p_below = 0, p_chg = 0, p_entry = 0;
-        float f_ij = 0.f, f_ji = 0.f;
-        unsigned K1w = 0, K2w = 0;   // window-order masks of the positions with k == 1 / k == 2 (state independent)
-        auto commit = [&]() {
-            const unsigned p_advance = (unsigned)__popc(p_below);
-            const unsigned bit = 1u << w;
-            const bool p_mine = (p_cm & bit) != 0u;
-            const bool p_swaps = (p_cm & bit & p_chg) != 0u;
-            const bool p_promoted = (p_below & bit) != 0u;
-            if (p_swaps) {
-                w2_sts64(repiA, ej.x, __float_as_uint(f_ij));
-                w2_sts64(repjA, ei.x, __float_as_uint(f_ji));
-            }
-            __syncwarp();
-            const uint2 ein = w2_lds64(p_promoted ? repiB : repiA), ejn = w2_lds64(p_promoted ? repjB : repjA);
-            if (p_mine)
-                asm volatile("st.global.u32 [%0], %1;" ::"l"(slot_log_r + 4ull * sA), "r"(p_entry) : "memory");
-            if (p_promoted) {
-                bmA = qB.y; luA = __uint_as_float(qB.z); kA = qB.w;
-                neqA = iB != jB ? 0xffffffffu : 0u;
-                epsA = iB != jB ? eps_rows : -1e30f;
-                rowiA = img_base + iB * row_bytes; rowjA = img_base + jB * row_bytes;
-                repiA = repiB; repjA = repjB;
-                sA += 32u;
-                w2_cp_async16(ring_base + (((ridxB - 32u) & (W2_RING - 1)) << 4), recs_r + (sA + 480u));
-                ridxB = (ridxB + 32u) & (W2_RING - 1);
-            }
-            w2_cp_async_commit();
-            qB = w2_lds128(ring_base + (ridxB << 4));
-            h += p_advance;
-            r = (r + p_advance) & 31u;
-            rem -= __popc(p_cm);
-            ei = ein;
-            ej = ejn;
-            w = (w - p_advance) & 31u;
-            // the hop classes of the new window (off the chain: they only depend on the promotions)
-            const unsigned b1 = __ballot_sync(0xffffffffu, kA == 1u), b2 = __ballot_sync(0xffffffffu, kA == 2u);
-            K1w = __funnelshift_r(b1, b1, r); K2w = __funnelshift_r(b2, b2, r);
-        };
-        unsigned Cw = 0;
-        float bias = 0.f, lu_saved = 0.f;
-        bool injected = false;
-        for (;;) {
-            if (rem < 130u || h + 99u > h_end) break;
-            unsigned quota = min(min((rem - 97u) >> 5, (h_end - h - 66u) >> 5), injected ? 1u : 64u);
-            do {
-                commit();
-                rounds++;
-                const unsigned si = ei.x, sj = ej.x;
-                f_ij = w2_image_at(rowiA + 2u * sj, rowiA + lo_off + sj);
-                f_ji = w2_image_at(rowjA + 2u * si, rowjA + lo_off + si);
-                const float e0 = fmaf(fabsf(__uint_as_float(ei.y)) + fabsf(__uint_as_float(ej.y)), 3.2e-5f, epsA);
-                w2_cp_async_wait<8>();
-                ahead(qB);
-                bool ge0, acc, undecided;
-                w2_filter(__uint_as_float(ei.y), f_ij, __uint_as_float(ej.y) + bias, f_ji, e0, luA, ge0, acc, undecided);
-                const unsigned und = undecided ? 1u : 0u;
-                const bool changes = acc && neqA != 0u;
-                const unsigned G = __ballot_sync(0xffffffffu, ge0);
-                const unsigned A = __ballot_sync(0xffffffffu, changes);
-                const unsigned Gw = __funnelshift_r(G, G, r), Aw = __funnelshift_r(A, A, r);   // window order
-                unsigned V, Cf;
-                w2c_chain(Gw, K1w, K2w, V, Cf);
-                const unsigned VA = V & Aw;
-                unsigned earlier;   // bit 31-b: window position w-1-b is a visited state-changing swap
-                asm("shl.b32 %0, %1, %2;" : "=r"(earlier) : "r"(VA), "r"(32u - w));
-                const unsigned C = __ballot_sync(0xffffffffu, ((earlier & bmA) | und) != 0u);
-                Cw = (__funnelshift_r(C, C, r) | Cf) & V;   // empty: the whole window commits and the next round starts at 32
-                const unsigned low = Cw & (0u - Cw);
-                const unsigned below = low - 1u;
-                p_cm = V & below; p_below = below; p_chg = changes ? 0xffffffffu : 0u;
-                p_entry = (sj * (1u << LOG_STATE_BITS) + si) | (acc ? (1u << 31) | (1u << LOG_ACC_BIT) : (1u << 31));
-            } while (--quota != 0u && (Cw & 1u) == 0u);
-            const bool was_injected = injected;
-            luA = was_injected ? lu_saved : luA;
-            bias = 0.f;
-            injected = false;
-            if ((Cw & 1u) == 0u) continue;
-            commit();   // (nothing to commit: positions the lanes on the round that could not start)
-            w2_cp_async_wait<8>();
-            ahead(qB);
-            // rare: the filter could not decide the window's first lane -- exact decisions injected into one fast round
-            if (!was_injected) {
-                const unsigned si = ei.x, sj = ej.x;
-                const float f1 = w2_image_at(rowiA + 2u * sj, rowiA + lo_off + sj);
-                const float f2 = w2_image_at(rowjA + 2u * si, rowjA + lo_off + si);
-                const float e0 = fmaf(fabsf(__uint_as_float(ei.y)) + fabsf(__uint_as_float(ej.y)), 3.2e-5f, epsA);
-                bool ge0, acc, undecided;
-                w2_filter(__uint_as_float(ei.y), f1, __uint_as_float(ej.y), f2, e0, luA, ge0, acc, undecided);
-                lu_saved = luA;
-                if (undecided) {
-                    const unsigned d = w2c_exact_decision(rec, words, cpos, u, sA, si, sj, K);
-                    bias = (d & 1u) ? 1e30f : -1e20f;
-                    if (!(d & 1u)) luA = (d & 2u) ? -1e30f : 0.f;
-                    slow++;
-                }
-                __syncwarp();
-                injected = true;
-                continue;
-            }
-            // rarer still (non-finite energies): one exact attempt, exactly what the reference does
-            {
-                rounds++;
-                unsigned d = 0;
-                const unsigned si = ei.x, sj = ej.x;
-                f_ij = w2_image_at(rowiA + 2u * sj, rowiA + lo_off + sj);
-                f_ji = w2_image_at(rowjA + 2u * si, rowjA + lo_off + si);
-                if (w == 0u) { d = w2c_exact_decision(rec, words, cpos, u, sA, si, sj, K); slow++; }
-                __syncwarp();
-                const bool first_ge0 = __ballot_sync(0xffffffffu, (d & 1u) != 0u) != 0u;
-                const bool acc = (d & 2u) != 0u || (d & 1u) != 0u;
-                const unsigned k0 = (K1w & 1u) + 2u * (K2w & 1u);   // hop class of window position 0
-                p_cm = 1u;
-                p_below = first_ge0 ? 3u : (4u << k0) - 1u;         // 2 or 2 + k positions leave the window
-                p_chg = (acc && neqA != 0u) ? 0xffffffffu : 0u;
-                p_entry = (sj * (1u << LOG_STATE_BITS) + si) | (acc ? (1u << 31) | (1u << LOG_ACC_BIT) : (1u << 31));
-                commit();
-                w2_cp_async_wait<8>();
-                ahead(qB);
-                p_cm = p_below = 0;
-            }
-        }
-        commit();   // the round resolved last, if one is pending
-        w2_cp_async_wait<0>();
-        __syncwarp();
-        for (int q = lane; q < K; q += 32) perm_g[q] = s_rep[q].state;
-    }
-    slow = __reduce_add_sync(0xffffffffu, slow);
-    if (lane == 0) {
-        const long long remaining = remaining0 - (long long)(rem0 - rem);
-        if (h > 0) ctl->head = (long long)cpos[h];   // word position: the first word the next attempt can use as an index
-        ctl->aux = h;                                 // candidate index (extent of the sparse commit log)
-        ctl->remaining = remaining;
-        ctl->status = remaining > 0 ? 1 : 0;
-        ctl->rounds += (int)rounds;
-        ctl->slow_exp += slow;
-    }
 }
