@@ -297,6 +297,39 @@ typedef struct {
 } rx_propagate_plan;
 RX_API int rx_plan_propagate(const rx_propagate_query *query, rx_propagate_plan *plan);
 
+/* ---- constant pressure (RX_SYSTEM_LJ_ALCH) -------------------------------------------------------- */
+/* Replaces the MonteCarloBarostat that ThermodynamicState(system, temperature, pressure) adds (states.py:1761-1771):
+ * isotropic, at the temperature of the replica's state, one attempt every 25 steps (OpenMM's default frequency) inside
+ * rx_propagate.  An attempt draws dV uniform in +-volume_scale, scales positions about the origin by (V'/V)^(1/3)
+ * (every atom is its own molecule; velocities are not scaled) and accepts when w = dU + p dV - N kT ln(V'/V) <= 0 or
+ * u < exp(-w/kT); dU includes the change of the dispersion correction c_l / V.  volume_scale starts at 0.01 V and is
+ * divided by 1.1 (acceptance < 25 %) or multiplied by 1.1 up to 0.3 V (acceptance > 75 %) after every 10 attempts.
+ * A proposal with a box edge below twice the cutoff is rejected (and counted as an attempt).
+ *
+ * rx_set_pressures  switches the engine to NPT: pressure[M] in kJ/mol/nm^3 (1 bar = 0.0602214076 kJ/mol/nm^3) and the
+ *                   per-state dispersion-correction coefficients dispersion[M] in kJ/mol nm^3 (the correction at volume V
+ *                   is dispersion[l] / V; energy_offset of rx_set_states then holds the rest of the offset).  Every owned
+ *                   replica gets the box of rx_config and a fresh barostat state.  The energy matrix becomes
+ *                   u[k][l] = beta_l (U_l(x_k) + dispersion[l] / V_k + pressure[l] V_k) (states.py:1909-1917).
+ * rx_set_boxes / rx_get_boxes  edges[count][3] (nm) of replicas [first, first + count) (global indices, the owned ones).
+ * rx_set_barostat / rx_get_barostat  the barostat state of the same replicas (checkpoints); rx_set_boxes leaves it.
+ * rx_compute_energies_at_npt  rx_compute_energies_at for an NPT engine: the other states' pressures and dispersion
+ *                   coefficients [n] come with them (rx_compute_energies_at returns RX_ERR_INVALID on an NPT engine).
+ * rx_minimize minimises every replica at its own box. */
+typedef struct {
+    double volume_scale;       /* nm^3 */
+    int32_t step;              /* steps since the last attempt */
+    int32_t n_attempted, n_accepted;   /* since the last adaptation of volume_scale */
+    int32_t reserved;
+} rx_barostat_state;
+RX_API int rx_set_pressures(rx_engine *h, const double *pressure /*[M]*/, const double *dispersion /*[M]*/);
+RX_API int rx_set_boxes(rx_engine *h, int32_t first, int32_t count, const double *edges);
+RX_API int rx_get_boxes(rx_engine *h, int32_t first, int32_t count, double *edges);
+RX_API int rx_set_barostat(rx_engine *h, int32_t first, int32_t count, const rx_barostat_state *state);
+RX_API int rx_get_barostat(rx_engine *h, int32_t first, int32_t count, rx_barostat_state *state);
+RX_API int rx_compute_energies_at_npt(rx_engine *h, const rx_state_params *states, const double *pressure,
+                                      const double *dispersion, int32_t n, double *u_out);
+
 /* ---- multi-GPU ------------------------------------------------------------------------------------ */
 /* NCCL is loaded with dlopen(nccl_library_path).  Rank 0 creates an id (rx_comm_unique_id), the host code
  * distributes its bytes (torch.distributed / MPI / a file), every rank calls rx_comm_init.  Replaces

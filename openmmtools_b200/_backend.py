@@ -112,7 +112,11 @@ def alchemical_dispersion_correction(system, lambda_sterics):
 def check_compatible(thermodynamic_states):
     h0 = thermodynamic_states[0]._standard_system_hash
     sys0 = thermodynamic_states[0]._standard_system
+    npt = thermodynamic_states[0].pressure is not None
     for s in thermodynamic_states[1:]:
+        if (s.pressure is not None) != npt:
+            from .states import ThermodynamicsError
+            raise ThermodynamicsError(ThermodynamicsError.INCOMPATIBLE_ENSEMBLE)
         if s._standard_system_hash != h0:
             so = s._standard_system
             # harmonic oscillators may differ in K/x0/U0 (global parameters in the reference)
@@ -148,6 +152,35 @@ def engine_tables(thermodynamic_states):
     return sys0, dict(temperature=T, lambda_sterics=lam, energy_offset=off, ho_K=hoK, ho_x0=hox0)
 
 
+def pressure_tables(thermodynamic_states):
+    """NPT states: (pressure [M] in kJ/mol/nm^3, dispersion coefficients c_l [M] in kJ/mol nm^3), or None for NVT.
+
+    Both long-range corrections are proportional to 1/V, so c_l is the state's correction at the system's volume times
+    that volume; the engine adds c_l / V_k for replica k (and the per-state offset then carries no correction)."""
+    if thermodynamic_states[0].pressure is None:
+        return None
+    sys0 = check_compatible(thermodynamic_states)
+    V0 = abs(np.linalg.det(sys0.box_vectors))
+    base = lj_dispersion_correction(sys0)
+    p = np.array([s._pressure_md for s in thermodynamic_states])
+    cache = {}
+    c = np.zeros(len(thermodynamic_states))
+    for l, s in enumerate(thermodynamic_states):
+        lam = s._engine_parameters()['lambda_sterics'] if sys0.is_alchemical else 1.0
+        if lam not in cache:
+            cache[lam] = (base + alchemical_dispersion_correction(sys0, lam)) * V0
+        c[l] = cache[lam]
+    return p, c
+
+
+def box_edges(sampler_states):
+    """(K, 3) edges of the sampler states' rectangular boxes."""
+    b = np.stack([np.asarray(s._box_vectors, np.float64) for s in sampler_states])
+    if not np.allclose(b, np.einsum('kij,ij->kij', b, np.eye(3))):
+        raise NotImplementedError('only rectangular periodic boxes are provided')
+    return np.einsum('kii->ki', b).copy()
+
+
 def default_device(context_cache=None):
     import os
     idx = getattr(context_cache, 'device_index', None) if context_cache is not None else None
@@ -178,7 +211,12 @@ def build_engine(thermodynamic_states, n_replicas, device=0, rank=0, world_size=
     else:
         eng = Engine(_lib.RX_SYSTEM_HARMONIC, n_replicas, M, N, device=device, rank=rank, world_size=world_size)
         eng.set_particles(None, None, sys0.masses, None)
+    npt = pressure_tables(thermodynamic_states)
+    if npt is not None:
+        tab['energy_offset'] = np.zeros(M)   # (the dispersion corrections go to the engine as c_l / V)
     eng.set_states(**tab)
+    if npt is not None:
+        eng.set_pressures(*npt)
     return eng
 
 
@@ -191,6 +229,8 @@ def reduced_potentials(thermodynamic_states, sampler_state):
     eng = build_engine(list(thermodynamic_states), 1, device=default_device())
     try:
         eng.set_positions(sampler_state._positions[None])
+        if thermodynamic_states[0].pressure is not None:
+            eng.set_boxes(box_edges([sampler_state]))
         return eng.compute_energies()[0]
     finally:
         eng.close()

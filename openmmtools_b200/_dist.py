@@ -133,19 +133,30 @@ def _recv_exact(c, n):
     return bytes(buf)
 
 
+_NPT_RECORD = 7   # box edges (3), barostat volume_scale, step, n_attempted, n_accepted
+
+
 def _encode_shard(shard):
-    """[(k, x[N,3], v[N,3] | None, pe | None, ke | None), ...] -> bytes: count, then per item
-    <i k><i n_atoms><B has_v><B has_pe><B has_ke><d pe><d ke> + x (+ v) as little-endian float64."""
+    """[(k, x[N,3], v[N,3] | None, pe | None, ke | None[, npt | None]), ...] -> bytes: count, then per item
+    <i k><i n_atoms><B has_v><B has_pe><B has_ke><B has_npt><d pe><d ke> + x (+ v) (+ npt) as little-endian float64.
+    npt: a constant-pressure replica's box edges and barostat state, 7 float64 (the counters are exact in float64)."""
     import struct
     import numpy as np
     parts = [struct.pack('<i', len(shard))]
-    for k, x, v, pe, ke in shard:
+    for item in shard:
+        k, x, v, pe, ke = item[:5]
+        npt = item[5] if len(item) > 5 else None
         x = np.ascontiguousarray(x, dtype='<f8')
-        parts.append(struct.pack('<iiBBBdd', int(k), x.shape[0], v is not None, pe is not None, ke is not None,
-                                 0.0 if pe is None else float(pe), 0.0 if ke is None else float(ke)))
+        parts.append(struct.pack('<iiBBBBdd', int(k), x.shape[0], v is not None, pe is not None, ke is not None,
+                                 npt is not None, 0.0 if pe is None else float(pe), 0.0 if ke is None else float(ke)))
         parts.append(x.tobytes())
         if v is not None:
             parts.append(np.ascontiguousarray(v, dtype='<f8').tobytes())
+        if npt is not None:
+            npt = np.ascontiguousarray(npt, dtype='<f8')
+            if npt.shape != (_NPT_RECORD,):
+                raise ValueError('the constant-pressure record of a replica holds %d numbers' % _NPT_RECORD)
+            parts.append(npt.tobytes())
     return b''.join(parts)
 
 
@@ -159,12 +170,12 @@ def _decode_shard(buf):
         raise RuntimeError('gather: malformed shard')
     out = []
     for _ in range(count):
-        if off + struct.calcsize('<iiBBBdd') > len(buf):
+        if off + struct.calcsize('<iiBBBBdd') > len(buf):
             raise RuntimeError('gather: malformed shard')
-        k, n, hv, hp, hk, pe, ke = struct.unpack_from('<iiBBBdd', buf, off)
-        off += struct.calcsize('<iiBBBdd')
+        k, n, hv, hp, hk, hn, pe, ke = struct.unpack_from('<iiBBBBdd', buf, off)
+        off += struct.calcsize('<iiBBBBdd')
         nb = n * 24
-        if n < 0 or off + nb * (2 if hv else 1) > len(buf):
+        if n < 0 or off + nb * (2 if hv else 1) + (8 * _NPT_RECORD if hn else 0) > len(buf):
             raise RuntimeError('gather: malformed shard')
         x = np.frombuffer(buf, dtype='<f8', count=3 * n, offset=off).reshape(n, 3).copy()
         off += nb
@@ -172,7 +183,11 @@ def _decode_shard(buf):
         if hv:
             v = np.frombuffer(buf, dtype='<f8', count=3 * n, offset=off).reshape(n, 3).copy()
             off += nb
-        out.append((k, x, v, pe if hp else None, ke if hk else None))
+        npt = None
+        if hn:
+            npt = np.frombuffer(buf, dtype='<f8', count=_NPT_RECORD, offset=off).copy()
+            off += 8 * _NPT_RECORD
+        out.append((k, x, v, pe if hp else None, ke if hk else None, npt))
     return out
 
 

@@ -93,12 +93,18 @@ class Engine:
         arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0)
         self._check(self._lib.rx_set_states(self._h, C.cast(arr, C.c_void_p)))
 
-    def compute_energies_at(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None):
-        """u[K][n] of every replica at n other states (unsampled states); the resident matrix is untouched."""
+    def compute_energies_at(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None, pressure=None,
+                            dispersion=None):
+        """u[K][n] of every replica at n other states (unsampled states); the resident matrix is untouched.  An NPT engine
+        takes those states' pressures (kJ/mol/nm^3) and dispersion coefficients (kJ/mol nm^3) as well."""
         arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0)
         n = len(temperature)
         out = np.zeros((self.K, n))
-        self._check(self._lib.rx_compute_energies_at(self._h, C.cast(arr, C.c_void_p), n, _ptr(out)))
+        if pressure is None:
+            self._check(self._lib.rx_compute_energies_at(self._h, C.cast(arr, C.c_void_p), n, _ptr(out)))
+        else:
+            p, c = _c64(pressure, (n,)), _c64(dispersion, (n,))
+            self._check(self._lib.rx_compute_energies_at_npt(self._h, C.cast(arr, C.c_void_p), _ptr(p), _ptr(c), n, _ptr(out)))
         return out
 
     def set_integrator(self, timestep, collision_rate, n_steps, splitting='V R O R V'):
@@ -135,6 +141,47 @@ class Engine:
         """The move of one thermodynamic state where the states carry different moves (after set_integrator)."""
         self._check(self._lib.rx_set_state_integrator(self._h, int(state), float(timestep), float(collision_rate), int(n_steps),
                                                       splitting.replace(' ', '').encode(), int(bool(reassign_velocities))))
+
+    # -- constant pressure (rx_set_pressures)
+    def set_pressures(self, pressure, dispersion):
+        """Switch to NPT: per-state pressures (kJ/mol/nm^3) and dispersion coefficients c_l (kJ/mol nm^3, the correction
+        at volume V is c_l / V).  Every owned replica gets the engine's box and a fresh barostat state."""
+        p, c = _c64(pressure, (self.M,)), _c64(dispersion, (self.M,))
+        self._check(self._lib.rx_set_pressures(self._h, _ptr(p), _ptr(c)))
+
+    def set_boxes(self, edges, first=0):
+        """Box edges (count, 3) in nm of replicas [first, first + count)."""
+        e = _c64(edges)
+        if e.ndim != 2 or e.shape[1] != 3:
+            raise ValueError('edges must have shape (count, 3)')
+        self._check(self._lib.rx_set_boxes(self._h, first, e.shape[0], _ptr(e)))
+
+    def get_boxes(self, first=None, count=None):
+        first = self.k0 if first is None else first
+        count = (self.k1 - first) if count is None else count
+        out = np.zeros((count, 3))
+        self._check(self._lib.rx_get_boxes(self._h, first, count, _ptr(out)))
+        return out
+
+    _BARO_FIELDS = ('volume_scale', 'step', 'n_attempted', 'n_accepted')
+
+    def get_barostat(self, first=None, count=None):
+        """Barostat state of replicas [first, first + count): dict of arrays volume_scale, step, n_attempted, n_accepted."""
+        first = self.k0 if first is None else first
+        count = (self.k1 - first) if count is None else count
+        arr = (_lib.RxBarostatState * max(count, 1))()
+        self._check(self._lib.rx_get_barostat(self._h, first, count, C.cast(arr, C.c_void_p)))
+        return {f: np.array([getattr(arr[i], f) for i in range(count)], np.float64 if f == 'volume_scale' else np.int64)
+                for f in self._BARO_FIELDS}
+
+    def set_barostat(self, state, first=0):
+        count = len(state['volume_scale'])
+        arr = (_lib.RxBarostatState * max(count, 1))()
+        for i in range(count):
+            arr[i].volume_scale = float(state['volume_scale'][i])
+            for f in self._BARO_FIELDS[1:]:
+                setattr(arr[i], f, int(state[f][i]))
+        self._check(self._lib.rx_set_barostat(self._h, first, count, C.cast(arr, C.c_void_p)))
 
     # -- replica state
     def set_positions(self, xyz, first=0):

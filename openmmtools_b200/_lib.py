@@ -22,6 +22,7 @@ SYMBOLS = [
     'rx_propagate', 'rx_propagate_retry', 'rx_compute_energies', 'rx_compute_energies_at', 'rx_set_energies', 'rx_get_energies', 'rx_mix_seed',
     'rx_mix_skip', 'rx_mix_swap_all', 'rx_mix_swap_neighbors', 'rx_get_mix_counts', 'rx_mix_stream_position',
     'rx_run_iterations', 'rx_sams_set', 'rx_sams_step', 'rx_sams_get', 'rx_sams_run_iterations', 'rx_get_phase_times', 'rx_timer_mark', 'rx_timer_elapsed', 'rx_get_mix_stats', 'rx_selftest_exp', 'rx_plan_propagate', 'rx_comm_unique_id', 'rx_comm_init',
+    'rx_set_pressures', 'rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat', 'rx_compute_energies_at_npt',
 ]
 
 
@@ -54,6 +55,11 @@ class RxPropagateQuery(C.Structure):
 class RxPropagatePlan(C.Structure):
     _fields_ = [('cluster', C.c_int32), ('threads', C.c_int32), ('list_capacity', C.c_int32), ('sort_atoms', C.c_int32),
                 ('compact', C.c_int32), ('reserved', C.c_int32), ('smem_bytes', C.c_int64)]
+
+
+class RxBarostatState(C.Structure):
+    _fields_ = [('volume_scale', C.c_double), ('step', C.c_int32), ('n_attempted', C.c_int32), ('n_accepted', C.c_int32),
+                ('reserved', C.c_int32)]
 
 
 class RxMolecule(C.Structure):
@@ -130,6 +136,10 @@ def load():
     lib.rx_plan_propagate.argtypes = [C.POINTER(RxPropagateQuery), C.POINTER(RxPropagatePlan)]
     lib.rx_comm_unique_id.argtypes = [C.c_char_p, vp]
     lib.rx_comm_init.argtypes = [vp, C.c_char_p, vp]
+    lib.rx_set_pressures.argtypes = [vp, vp, vp]
+    lib.rx_compute_energies_at_npt.argtypes = [vp, vp, vp, vp, i32, vp]
+    for name in ('rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat'):
+        getattr(lib, name).argtypes = [vp, i32, i32, vp]
     if lib.rx_abi_version() != RX_ABI_VERSION:
         raise ImportError('librx_b200.so ABI version mismatch')
     _lib = lib

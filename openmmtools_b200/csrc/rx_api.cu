@@ -127,6 +127,7 @@ extern "C" void rx_destroy(rx_engine *h) {
     cudaFree(h->d_pos); cudaFree(h->d_vel); cudaFree(h->d_io); cudaFree(h->d_perm); cudaFree(h->d_u);
     cudaFree(h->d_nacc); cudaFree(h->d_nprop); cudaFree(h->d_pot); cudaFree(h->d_kin); cudaFree(h->d_nan);
     cudaFree(h->d_err); cudaFree(h->d_pairs);
+    cudaFree(h->d_npt); cudaFree(h->d_box); cudaFree(h->d_box_snap); cudaFree(h->d_baro); cudaFree(h->d_baro_snap);
     for (int i = 0; i < 8; i++) if (h->ev[i]) cudaEventDestroy(h->ev[i]);
     for (int i = 0; i < 2; i++) if (h->ev_user[i]) cudaEventDestroy(h->ev_user[i]);
     for (int i = 0; i < 2; i++) if (h->ev_walk[i]) cudaEventDestroy(h->ev_walk[i]);
@@ -323,11 +324,98 @@ extern "C" int rx_set_velocities(rx_engine *h, int32_t first, int32_t count, con
 }
 extern "C" int rx_get_positions(rx_engine *h, int32_t first, int32_t count, double *xyz) {
     ENTER(h);
-    return get_xyz(h, h->d_pos, first, count, xyz, h->cfg.system_kind == RX_SYSTEM_LJ_ALCH, "rx_get_positions");
+    // (an NPT replica's positions are left where the propagation wrapped them into its own box)
+    return get_xyz(h, h->d_pos, first, count, xyz, h->cfg.system_kind == RX_SYSTEM_LJ_ALCH && !h->npt, "rx_get_positions");
 }
 extern "C" int rx_get_velocities(rx_engine *h, int32_t first, int32_t count, double *xyz) {
     ENTER(h);
     return get_xyz(h, h->d_vel, first, count, xyz, false, "rx_get_velocities");
+}
+
+// ---- constant pressure -------------------------------------------------------------------------------------------------
+extern "C" int rx_set_pressures(rx_engine *h, const double *pressure, const double *dispersion) {
+    ENTER(h);
+    if (h->cfg.system_kind != RX_SYSTEM_LJ_ALCH) RX_FAIL(h, RX_ERR_INVALID, "rx_set_pressures: constant pressure needs a periodic LJ engine");
+    if (!pressure || !dispersion) RX_FAIL(h, RX_ERR_INVALID, "rx_set_pressures: null argument");
+    const int M = h->cfg.n_states, n = h->kloc > 0 ? h->kloc : 1;
+    std::vector<double2> tab(M);
+    for (int l = 0; l < M; l++) {
+        if (!(pressure[l] > 0) || !isfinite(pressure[l]) || !isfinite(dispersion[l]))
+            RX_FAIL(h, RX_ERR_INVALID, "rx_set_pressures: need finite pressures > 0 and finite dispersion coefficients");
+        tab[l] = make_double2(pressure[l], dispersion[l]);
+    }
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (!h->d_npt) {
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_npt, sizeof(double2) * M));
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_box, sizeof(double4) * n));
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_box_snap, sizeof(double4) * n));
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_baro, sizeof(rx_barostat_state) * n));
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_baro_snap, sizeof(rx_barostat_state) * n));
+    }
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_npt, tab.data(), sizeof(double2) * M, cudaMemcpyHostToDevice));
+    const double *L = h->cfg.box;
+    std::vector<double4> b(n, make_double4(L[0], L[1], L[2], 0.0));
+    rx_barostat_state s0;
+    memset(&s0, 0, sizeof(s0));
+    s0.volume_scale = 0.01 * L[0] * L[1] * L[2];   // MonteCarloBarostat's initial volume scale
+    std::vector<rx_barostat_state> s(n, s0);
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_box, b.data(), sizeof(double4) * n, cudaMemcpyHostToDevice));
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_baro, s.data(), sizeof(rx_barostat_state) * n, cudaMemcpyHostToDevice));
+    h->npt = true;
+    h->have_snapshot = false;   // (a snapshot without boxes cannot restore an NPT replica)
+    return RX_OK;
+}
+
+// Copies between caller rows [first, first + count) and the owned replicas' rows of a per-replica device table.
+template <typename T>
+static int replica_rows(rx_engine *h, T *dev, int first, int count, T *host, bool to_device, const char *who) {
+    if (!h->npt) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": the engine has no pressure (rx_set_pressures)");
+    if (!host) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": null buffer");
+    int lo, n, skip;
+    int rc = local_range(h, first, count, &lo, &n, &skip);
+    if (rc) return rc;
+    if (n == 0) return RX_OK;
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (to_device) RX_CHECK_CUDA(h, cudaMemcpy(dev + lo, host + skip, sizeof(T) * n, cudaMemcpyHostToDevice));
+    else RX_CHECK_CUDA(h, cudaMemcpy(host + skip, dev + lo, sizeof(T) * n, cudaMemcpyDeviceToHost));
+    return RX_OK;
+}
+
+extern "C" int rx_set_boxes(rx_engine *h, int32_t first, int32_t count, const double *edges) {
+    ENTER(h);
+    if (!edges || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_set_boxes: bad arguments");
+    std::vector<double4> b((size_t)count);
+    for (int i = 0; i < count; i++) {
+        for (int d = 0; d < 3; d++)
+            if (!(edges[3 * i + d] >= 2.0 * h->cfg.r_cutoff) || !isfinite(edges[3 * i + d]))
+                RX_FAIL(h, RX_ERR_INVALID, "rx_set_boxes: every box edge must be at least twice the cutoff");
+        b[i] = make_double4(edges[3 * i], edges[3 * i + 1], edges[3 * i + 2], 0.0);
+    }
+    return replica_rows(h, h->d_box, first, count, b.data(), true, "rx_set_boxes");
+}
+extern "C" int rx_get_boxes(rx_engine *h, int32_t first, int32_t count, double *edges) {
+    ENTER(h);
+    if (!edges || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_get_boxes: bad arguments");
+    std::vector<double4> b((size_t)count, make_double4(0.0, 0.0, 0.0, 0.0));
+    int rc = replica_rows(h, h->d_box, first, count, b.data(), false, "rx_get_boxes");
+    if (rc) return rc;
+    int lo, n, skip;
+    local_range(h, first, count, &lo, &n, &skip);
+    for (int i = skip; i < skip + n; i++) { edges[3 * i] = b[i].x; edges[3 * i + 1] = b[i].y; edges[3 * i + 2] = b[i].z; }
+    return RX_OK;
+}
+extern "C" int rx_set_barostat(rx_engine *h, int32_t first, int32_t count, const rx_barostat_state *state) {
+    ENTER(h);
+    if (!state || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_set_barostat: bad arguments");
+    for (int i = 0; i < count; i++)
+        if (!(state[i].volume_scale > 0) || state[i].step < 0 || state[i].n_attempted < 0 || state[i].n_accepted < 0)
+            RX_FAIL(h, RX_ERR_INVALID, "rx_set_barostat: need volume_scale > 0 and non-negative counters");
+    return replica_rows(h, h->d_baro, first, count, const_cast<rx_barostat_state *>(state), true, "rx_set_barostat");
+}
+extern "C" int rx_get_barostat(rx_engine *h, int32_t first, int32_t count, rx_barostat_state *state) {
+    ENTER(h);
+    if (!state || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_get_barostat: bad arguments");
+    return replica_rows(h, h->d_baro, first, count, state, false, "rx_get_barostat");
 }
 
 bool rxi_is_pinned(const rx_engine *h, const void *p, size_t bytes) {
@@ -518,36 +606,61 @@ extern "C" int rx_get_energies(rx_engine *h, double *u) {
     return RX_OK;
 }
 
-extern "C" int rx_compute_energies_at(rx_engine *h, const rx_state_params *st, int32_t n, double *u_out) {
-    ENTER(h);
-    int rc = check_ready(h, "rx_compute_energies_at");
+// Energies at n other states; pressure / dispersion (NPT engines only, else NULL) are those states' (p, c) tables.
+static int energies_at(rx_engine *h, const rx_state_params *st, const double *pressure, const double *dispersion, int32_t n,
+                       double *u_out, const char *who) {
+    int rc = check_ready(h, who);
     if (rc) return rc;
-    if (!st || !u_out || n < 1) RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at: bad arguments");
+    if (!st || !u_out || n < 1) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": bad arguments");
     std::vector<StateDev> hs;
-    rc = convert_states(h, st, n, hs, "rx_compute_energies_at");
+    rc = convert_states(h, st, n, hs, who);
     if (rc) return rc;
+    std::vector<double2> tab;
+    if (pressure) {
+        for (int l = 0; l < n; l++) {
+            if (!(pressure[l] > 0) || !isfinite(pressure[l]) || !isfinite(dispersion[l]))
+                RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": need finite pressures > 0 and finite dispersion coefficients");
+            tab.push_back(make_double2(pressure[l], dispersion[l]));
+        }
+    }
     const int K = h->cfg.n_replicas;
     StateDev *d_st = nullptr;
     double *d_out = nullptr;
+    double2 *d_tab = nullptr;
     RX_CHECK_CUDA(h, cudaMalloc(&d_st, sizeof(StateDev) * n));
     cudaError_t e = cudaMalloc(&d_out, sizeof(double) * (size_t)K * n);
-    if (e != cudaSuccess) { cudaFree(d_st); RX_FAIL(h, RX_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e)); }
+    if (e == cudaSuccess && pressure) e = cudaMalloc(&d_tab, sizeof(double2) * n);
+    if (e != cudaSuccess) { cudaFree(d_st); cudaFree(d_out); RX_FAIL(h, RX_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e)); }
     int launches = 0;
     cudaMemcpyAsync(d_st, hs.data(), sizeof(StateDev) * n, cudaMemcpyHostToDevice, h->stream);
+    if (pressure) cudaMemcpyAsync(d_tab, tab.data(), sizeof(double2) * n, cudaMemcpyHostToDevice, h->stream);
     cudaMemsetAsync(d_out, 0, sizeof(double) * (size_t)K * n, h->stream);
-    rc = rxi_compute_energy_rows_at(h, d_st, n, d_out, &launches);
+    rc = rxi_compute_energy_rows_at(h, d_st, n, d_out, &launches, d_tab);
     if (!rc) rc = rxi_allgather_rows(h, d_out, n);
     if (!rc) {
         e = cudaMemcpyAsync(u_out, d_out, sizeof(double) * (size_t)K * n, cudaMemcpyDeviceToHost, h->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-        if (e != cudaSuccess) { h->err = std::string("rx_compute_energies_at: ") + cudaGetErrorString(e); rc = RX_ERR_CUDA; }
+        if (e != cudaSuccess) { h->err = std::string(who) + ": " + cudaGetErrorString(e); rc = RX_ERR_CUDA; }
     }
     cudaStreamSynchronize(h->stream);
     cudaFree(d_st);
     cudaFree(d_out);
+    cudaFree(d_tab);
     if (rc) return rc;
     h->phase_launches[2] += launches;
     return check_device_error(h);
+}
+
+extern "C" int rx_compute_energies_at(rx_engine *h, const rx_state_params *st, int32_t n, double *u_out) {
+    ENTER(h);
+    return energies_at(h, st, nullptr, nullptr, n, u_out, "rx_compute_energies_at");
+}
+
+extern "C" int rx_compute_energies_at_npt(rx_engine *h, const rx_state_params *st, const double *pressure,
+                                          const double *dispersion, int32_t n, double *u_out) {
+    ENTER(h);
+    if (!pressure || !dispersion) RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at_npt: null argument");
+    return energies_at(h, st, pressure, dispersion, n, u_out, "rx_compute_energies_at_npt");
 }
 
 extern "C" int rx_mix_seed(rx_engine *h, int32_t stream, uint32_t seed) {

@@ -230,14 +230,18 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
 // PS: per-state moves (the integrator parameters come from `moves[state]` instead of `p`).
 // COMPACT: the layout above 1024 atoms (DESIGN 4.2): position buffers strided by N instead of RX_MAX_ATOMS and 8-byte
 // parameter records (sqrt_eps, alch) -- sigma rides in the position's w -- so that 4096 atoms leave room for a list.
-template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false>
+// NPT: the box is the replica's (box[r], kept in f64 there) and a Monte Carlo barostat attempt opens every 25th step
+// (rx_b200.h, rx_set_pressures); npt[state] = (pressure, dispersion coefficient), min_edge = twice the cutoff.
+template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false, bool NPT = false>
 __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *__restrict__ atom,
                                                     const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                     float4 *__restrict__ pos, float4 *__restrict__ vel, int k0,
                                                     uint2 key, uint32_t iteration, int reassign,
                                                     double *__restrict__ pot, double *__restrict__ kin,
                                                     int *__restrict__ nan_flag, const int *__restrict__ only,
-                                                    const MoveDev *__restrict__ moves) {
+                                                    const MoveDev *__restrict__ moves, double4 *__restrict__ box,
+                                                    rx_barostat_state *__restrict__ baro, const double2 *__restrict__ npt,
+                                                    double min_edge) {
     extern __shared__ float4 s_dyn[];
     // (the whole cluster takes this exit together: `only` is indexed by replica)
     if (only && !only[k0 + blockIdx.x / CL]) return;   // a retry launch propagates the replicas that failed, nothing else
@@ -273,6 +277,19 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     };
     const StateDev st = states[perm[k]];
     const PairLam lam = {(float)st.la, (float)st.ob};
+    // NPT: the replica's box (f64, and the float edges and inverses the kernel uses instead of p's) and barostat state
+    double bx = 0.0, by = 0.0, bz = 0.0;
+    float fLx = 0.f, fLy = 0.f, fLz = 0.f, fiLx = 0.f, fiLy = 0.f, fiLz = 0.f;
+    rx_barostat_state bs = {};
+    double2 nst = {};
+    if constexpr (NPT) {
+        const double4 b4 = box[r];
+        bx = b4.x; by = b4.y; bz = b4.z;
+        bs = baro[r];
+        nst = npt[perm[k]];
+        fLx = (float)bx; fLy = (float)by; fLz = (float)bz;
+        fiLx = (float)(1.0 / bx); fiLy = (float)(1.0 / by); fiLz = (float)(1.0 / bz);
+    }
     // the move: the launch's, or the one of this replica's state
     const MoveDev *mv = PS ? moves + perm[k] : nullptr;
     const float m_dt = PS ? mv->dt : p.dt, m_a = PS ? mv->a : p.a, m_b = PS ? mv->b : p.b;
@@ -309,6 +326,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
 
     bool use_list = lj && p.maxnb > 0;
     bool have_list = false;        // an outer list exists
+    bool built_once = false;       // NPT: an outer list was built in this launch (a volume move clears have_list only)
     int n_all = 0, n_inner = 0;
     float xi = x, yi = y, zi = z;  // position at the last partition
     int cur = 1;                   // position buffer of the latest force evaluation (0: s_dyn, 1: s_dyn + pos1)
@@ -361,9 +379,17 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
                 const unsigned ql = nb_t + (unsigned)lo * stride;
                 const unsigned e = lds_u16(ql);
                 const float4 pj = s_pos[e];
-                const float dx = min_image_f(x - pj.x, p.Lx, p.iLx), dy = min_image_f(y - pj.y, p.Ly, p.iLy),
-                            dz = min_image_f(z - pj.z, p.Lz, p.iLz);
-                if (dx * dx + dy * dy + dz * dz < p.rin2) lo++;
+                float d2;
+                if constexpr (NPT) {
+                    const float dx = min_image_f(x - pj.x, fLx, fiLx), dy = min_image_f(y - pj.y, fLy, fiLy),
+                                dz = min_image_f(z - pj.z, fLz, fiLz);
+                    d2 = dx * dx + dy * dy + dz * dz;
+                } else {
+                    const float dx = min_image_f(x - pj.x, p.Lx, p.iLx), dy = min_image_f(y - pj.y, p.Ly, p.iLy),
+                                dz = min_image_f(z - pj.z, p.Lz, p.iLz);
+                    d2 = dx * dx + dy * dy + dz * dz;
+                }
+                if (d2 < p.rin2) lo++;
                 else {
                     const unsigned qh = nb_t + (unsigned)hi * stride;
                     sts_u16(ql, lds_u16(qh));
@@ -381,9 +407,16 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         if (active) {
             for (int j = 0; j < p.N; j++) {
                 const float4 pj = s_pos[j];
-                const float dx = min_image_f(x - pj.x, p.Lx, p.iLx), dy = min_image_f(y - pj.y, p.Ly, p.iLy),
-                            dz = min_image_f(z - pj.z, p.Lz, p.iLz);
-                const float r2 = dx * dx + dy * dy + dz * dz;
+                float r2;
+                if constexpr (NPT) {
+                    const float dx = min_image_f(x - pj.x, fLx, fiLx), dy = min_image_f(y - pj.y, fLy, fiLy),
+                                dz = min_image_f(z - pj.z, fLz, fiLz);
+                    r2 = dx * dx + dy * dy + dz * dz;
+                } else {
+                    const float dx = min_image_f(x - pj.x, p.Lx, p.iLx), dy = min_image_f(y - pj.y, p.Ly, p.iLy),
+                                dz = min_image_f(z - pj.z, p.Lz, p.iLz);
+                    r2 = dx * dx + dy * dy + dz * dz;
+                }
                 if (r2 < p.rl2 && j != a) {
                     if (cnt < p.maxnb) s_nb[cnt * nthr + t] = (unsigned short)j;
                     cnt++;
@@ -393,6 +426,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         s_ref[t] = make_float4(x, y, z, 0.f);
         n_all = cnt;
         have_list = true;
+        if constexpr (NPT) built_once = true;
         if (cluster_or(cnt > p.maxnb)) use_list = false;  // denser than the capacity: all-pairs from now on (the whole cluster)
     };
     // Make the list valid for the positions in buffer s_pos (all threads call this together).
@@ -401,7 +435,8 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         const float mx = x - rf.x, my = y - rf.y, mz = z - rf.z;
         const bool far = !have_list || (active && mx * mx + my * my + mz * mz > p.half_out2);
         if (cluster_or(far)) {
-            const bool first = !have_list;
+            bool first = !have_list;
+            if constexpr (NPT) first = !built_once;   // (a rebuild after a volume move needs no counting pass)
             build_outer(s_pos);
             if (use_list) partition(s_pos);
             if (first && p.sort_atoms && use_list) {  // the first build only counted neighbours for the sort
@@ -415,6 +450,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
 
     PairCtx pc;
     pc.Lx = p.Lx; pc.Ly = p.Ly; pc.Lz = p.Lz; pc.iLx = p.iLx; pc.iLy = p.iLy; pc.iLz = p.iLz; pc.rc2 = p.rc2;
+    if constexpr (NPT) { pc.Lx = fLx; pc.Ly = fLy; pc.Lz = fLz; pc.iLx = fiLx; pc.iLy = fiLy; pc.iLz = fiLz; }
     pc.lam = lam;
     const int N = p.N;
     // Publish the current positions and make the neighbour list valid for them: one barrier unless a list is rebuilt.
@@ -453,9 +489,86 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         }
     };
 
+    // ---- NPT: the Monte Carlo barostat (DESIGN 4.2) -------------------------------------------------------------
+    // (the whole body is a discarded statement in the NVT instantiations, which compile exactly as without it)
+    uint32_t n_baro = 0;   // attempts in this launch: the counter of the barostat's Philox stream
+    auto barostat = [&]() {
+        if constexpr (NPT) {
+            auto cluster_sync = [&]() { if (CL == 1) __syncthreads(); else cg::this_cluster().sync(); };
+            // Cluster-wide sum of the per-atom energies in fixed point (2^-24 kJ/mol): integer additions are associative, so the
+            // total -- and every accept decision -- is the same bits in every block, at every cluster width and thread
+            // assignment.  False in `fine` when some term is not finite or too large for the format (the move is then rejected).
+            auto energy_sum = [&](float e, bool &fine) -> long long {
+                unsigned long long *acc = (unsigned long long *)s_red;   // [0] sum, [1] terms out of range (in block 0)
+                if (q == 0 && t < 2) acc[t] = 0ull;
+                cluster_sync();
+                const bool ok = !(fabsf(e) >= 67108864.0f) && !isnan(e);
+                unsigned long long v = ok ? (unsigned long long)__double2ll_rn((double)e * 16777216.0) : 0ull, bad = ok ? 0ull : 1ull;
+                for (int o = 16; o > 0; o >>= 1) { v += __shfl_xor_sync(0xffffffffu, v, o); bad += __shfl_xor_sync(0xffffffffu, bad, o); }
+                unsigned long long *dst = acc;
+                if (CL > 1) dst = cg::this_cluster().map_shared_rank(acc, 0);
+                if ((t & 31) == 0) { atomicAdd(dst, v); if (bad) atomicAdd(dst + 1, bad); }
+                cluster_sync();
+                const long long total = (long long)dst[0];
+                fine = dst[1] == 0ull;
+                cluster_sync();   // every block has read the sums before they are cleared again
+                return total;
+            };
+            auto set_box = [&](double X, double Y, double Z) {
+                fLx = (float)X; fLy = (float)Y; fLz = (float)Z;
+                fiLx = (float)(1.0 / X); fiLy = (float)(1.0 / Y); fiLz = (float)(1.0 / Z);
+                pc.Lx = fLx; pc.Ly = fLy; pc.Lz = fLz; pc.iLx = fiLx; pc.iLy = fiLy; pc.iLz = fiLz;
+            };
+            float e0;
+            compute_forces(true, e0);   // (forces already valid come out the same bits: same list, same order)
+            f_valid = true;
+            bool fine0;
+            const long long U0 = energy_sum(e0, fine0);
+            const uint4 rr = philox4x32_10(make_uint4(n_baro++, 0xA0000000u, k, iteration), key);
+            const double u1 = ((double)rr.x + 0.5) * 2.3283064365386963e-10, u2 = ((double)rr.y + 0.5) * 2.3283064365386963e-10;
+            const double V = bx * by * bz, dV = bs.volume_scale * (2.0 * u1 - 1.0), V1 = V + dV;
+            const double sc = V1 > 0.0 ? cbrt(V1 / V) : 0.0;
+            bs.n_attempted++;
+            if (fine0 && bx * sc >= min_edge && by * sc >= min_edge && bz * sc >= min_edge) {
+                const int c_old = cur;   // the buffer holding the unscaled positions of every atom
+                const float sf = (float)sc;
+                x *= sf; y *= sf; z *= sf;
+                set_box(bx * sc, by * sc, bz * sc);
+                have_list = false;       // the list is rebuilt for the scaled box (and again after a rejection)
+                f_valid = false;
+                float e1;
+                compute_forces(true, e1);
+                f_valid = true;
+                bool fine1;
+                const long long U1 = energy_sum(e1, fine1);
+                const double kT = st.kT;
+                const double w = (double)(U1 - U0) * (1.0 / 16777216.0) + nst.y * (1.0 / V1 - 1.0 / V) + nst.x * dV -
+                                 (double)p.N * kT * log(V1 / V);
+                if (fine1 && (w <= 0.0 || u2 < exp(-w / kT))) {
+                    bx *= sc; by *= sc; bz *= sc;
+                    bs.n_accepted++;
+                } else {
+                    // the thread's atom may have changed in the rebuild: its unscaled position comes from the old buffer
+                    if (active) { const float4 o = (s_dyn + (c_old ? pos1 : 0))[a]; x = o.x; y = o.y; z = o.z; }
+                    set_box(bx, by, bz);
+                    have_list = false;
+                    f_valid = false;
+                }
+            }
+            if (bs.n_attempted >= 10) {
+                if (bs.n_accepted < 0.25 * bs.n_attempted) { bs.volume_scale /= 1.1; bs.n_attempted = bs.n_accepted = 0; }
+                else if (bs.n_accepted > 0.75 * bs.n_attempted) {
+                    bs.volume_scale = fmin(bs.volume_scale * 1.1, 0.3 * V);
+                    bs.n_attempted = bs.n_accepted = 0;
+                }
+            }
+        }
+    };
+
     uint32_t ocount = 0;
     float dummy;
     for (int s = 0; s < m_steps; s++) {
+        if constexpr (NPT) { if (++bs.step >= 25) { bs.step = 0; barostat(); } }
         for (int q = 0; q < m_nprog; q++) {
             const char op = PS ? mv->prog[q] : p.prog[q];
             if (op == 'V') {
@@ -501,13 +614,20 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         }
     }
     if (t == 0 && q == 0) {
-        pot[k] = U + st.offset;
+        if constexpr (NPT) {
+            pot[k] = U + st.offset + nst.y / (bx * by * bz);
+            box[r] = make_double4(bx, by, bz, 0.0);
+            baro[r] = bs;
+        } else {
+            pot[k] = U + st.offset;
+        }
         kin[k] = KE;
         nan_flag[k] = (any_bad || !isfinite(U)) ? 1 : 0;
     }
     if (active) {
         if (lj) {  // getState(enforcePeriodicBox=True), mcmc.py:731
-            x -= p.Lx * floorf(x * p.iLx); y -= p.Ly * floorf(y * p.iLy); z -= p.Lz * floorf(z * p.iLz);
+            if constexpr (NPT) { x -= fLx * floorf(x * fiLx); y -= fLy * floorf(y * fiLy); z -= fLz * floorf(z * fiLz); }
+            else { x -= p.Lx * floorf(x * p.iLx); y -= p.Ly * floorf(y * p.iLy); z -= p.Lz * floorf(z * p.iLz); }
         }
         pos[(size_t)r * p.N + a] = make_float4(x, y, z, 0.f);
         vel[(size_t)r * p.N + a] = make_float4(vx, vy, vz, 0.f);
@@ -546,11 +666,14 @@ __device__ __forceinline__ double switch_d(const EnParams &p, double r) {
     return 1.0 + t * t * t * (-10.0 + t * (15.0 - 6.0 * t));
 }
 
+// NPT: the replica's box from box[r], and u[k][l] gains beta_l (c_l / V_k + p_l V_k), npt[l] = (p_l, c_l).
+template <bool NPT = false>
 __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *__restrict__ atom_d,
                                                      const int *__restrict__ alch_list,
                                                      const StateDev *__restrict__ states,
                                                      const float4 *__restrict__ pos, int k0, double2 *__restrict__ pairs,
-                                                     double *__restrict__ u, int *__restrict__ err) {
+                                                     double *__restrict__ u, int *__restrict__ err,
+                                                     const double4 *__restrict__ box, const double2 *__restrict__ npt) {
     extern __shared__ double s_en[];
     double *sx = s_en, *sy = s_en + p.N, *sz = s_en + 2 * p.N;
     __shared__ double s_red[32];
@@ -558,6 +681,7 @@ __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *
     __shared__ double s_U0;
     __shared__ int s_npairs;
     const int r = blockIdx.x, k = k0 + r, t = threadIdx.x, nt = blockDim.x;
+    if constexpr (NPT) { const double4 b = box[r]; p.Lx = b.x; p.Ly = b.y; p.Lz = b.z; }
     for (int q = t; q < p.N; q += nt) {
         const float4 x4 = pos[(size_t)r * p.N + q];
         sx[q] = (double)x4.x; sy[q] = (double)x4.y; sz[q] = (double)x4.z;
@@ -658,7 +782,13 @@ __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *
             const double x = p.c_is_6 ? 1.0 / D : pow(D, -6.0 / p.sc_c);
             Ua += st.la * pr.y * x * (x - 1.0);
         }
-        u[(size_t)k * p.M + l] = st.beta * (U0s + Ua + st.offset);
+        if constexpr (NPT) {
+            const double V = p.Lx * p.Ly * p.Lz;
+            const double2 pc = npt[l];
+            u[(size_t)k * p.M + l] = st.beta * (U0s + Ua + st.offset + pc.y / V + pc.x * V);
+        } else {
+            u[(size_t)k * p.M + l] = st.beta * (U0s + Ua + st.offset);
+        }
     }
 }
 
@@ -953,13 +1083,20 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
     lc.attrs = at;
     lc.numAttrs = 1;
     const uint32_t it32 = (uint32_t)iteration;
-#define RX_LAUNCH_PROPAGATE(C6, SW, CL, PS, CP)                                                                           \
+    const double min_edge = 2.0 * h->cfg.r_cutoff;
+    const bool npt = h->npt;
+#define RX_LAUNCH_PROPAGATE_NPT(C6, SW, CL, PS, CP, NP)                                                                   \
     do {                                                                                                                   \
         if (smem > 48 * 1024)                                                                                              \
-            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_propagate<C6, SW, CL, PS, CP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        RX_CHECK_CUDA(h, cudaLaunchKernelEx(&lc, k_propagate<C6, SW, CL, PS, CP>, p, (const float4 *)h->d_atom, (const StateDev *)h->d_states, \
+            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_propagate<C6, SW, CL, PS, CP, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        RX_CHECK_CUDA(h, cudaLaunchKernelEx(&lc, k_propagate<C6, SW, CL, PS, CP, NP>, p, (const float4 *)h->d_atom, (const StateDev *)h->d_states, \
                                             (const int *)h->d_perm, h->d_pos, h->d_vel, h->k0, key, it32, reassign, h->d_pot, \
-                                            h->d_kin, h->d_nan, d_only, (const MoveDev *)h->d_moves));                    \
+                                            h->d_kin, h->d_nan, d_only, (const MoveDev *)h->d_moves, h->d_box, h->d_baro,  \
+                                            (const double2 *)h->d_npt, min_edge));                                         \
+    } while (0)
+#define RX_LAUNCH_PROPAGATE(C6, SW, CL, PS, CP)                                                                           \
+    do {                                                                                                                   \
+        if (npt) RX_LAUNCH_PROPAGATE_NPT(C6, SW, CL, PS, CP, true); else RX_LAUNCH_PROPAGATE_NPT(C6, SW, CL, PS, CP, false); \
     } while (0)
 // above 1024 atoms: the compact layout over 2, 4 or 8 blocks, per-state moves or not
 #define RX_LAUNCH_PROPAGATE_COMPACT(C6, SW, PS)                                                                           \
@@ -979,6 +1116,7 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
 #undef RX_LAUNCH_PROPAGATE_COMPACT
 #undef RX_LAUNCH_PROPAGATE_CL
 #undef RX_LAUNCH_PROPAGATE
+#undef RX_LAUNCH_PROPAGATE_NPT
     RX_CHECK_CUDA(h, cudaGetLastError());
     (*launches)++;
     return RX_OK;
@@ -996,8 +1134,22 @@ int rxi_snapshot_state(rx_engine *h) {
     }
     RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_pos_snap, h->d_pos, bytes, cudaMemcpyDeviceToDevice, h->stream));
     RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_vel_snap, h->d_vel, bytes, cudaMemcpyDeviceToDevice, h->stream));
+    if (h->npt) {
+        RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_box_snap, h->d_box, sizeof(double4) * h->kloc, cudaMemcpyDeviceToDevice, h->stream));
+        RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_baro_snap, h->d_baro, sizeof(rx_barostat_state) * h->kloc, cudaMemcpyDeviceToDevice, h->stream));
+    }
     h->have_snapshot = true;
     return RX_OK;
+}
+
+// NPT: the box and barostat state of the failed replicas go back to the snapshot as well.
+__global__ void k_restore_failed_npt(const int *__restrict__ nan_flag, int k0, int kloc, const double4 *__restrict__ box_snap,
+                                     const rx_barostat_state *__restrict__ baro_snap, double4 *__restrict__ box,
+                                     rx_barostat_state *__restrict__ baro) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= kloc || !nan_flag[k0 + r]) return;
+    box[r] = box_snap[r];
+    baro[r] = baro_snap[r];
 }
 
 __global__ void k_restore_failed(const int *__restrict__ nan_flag, int *__restrict__ retry, int k0, int N,
@@ -1025,6 +1177,11 @@ int rxi_restore_failed(rx_engine *h) {
     k_restore_failed<<<h->kloc, 256, 0, h->stream>>>(h->d_nan, h->d_retry, h->k0, h->cfg.n_atoms, h->d_pos_snap, h->d_vel_snap,
                                                     h->d_pos, h->d_vel);
     RX_CHECK_CUDA(h, cudaGetLastError());
+    if (h->npt) {
+        k_restore_failed_npt<<<(h->kloc + 127) / 128, 128, 0, h->stream>>>(h->d_nan, h->k0, h->kloc, h->d_box_snap, h->d_baro_snap,
+                                                                          h->d_box, h->d_baro);
+        RX_CHECK_CUDA(h, cudaGetLastError());
+    }
     return RX_OK;
 }
 
@@ -1040,12 +1197,19 @@ int rxi_restore_failed(rx_engine *h) {
 // sums are added in that order, so the result does not depend on scheduling.  Shared memory: [stride] positions, then
 // [stride] parameter records, stride = RX_MAX_ATOMS (APT = 1) or N.
 // ---------------------------------------------------------------------------------------------------
-template <bool C6, bool SW, int APT>
+// NPT: every replica at its own box (box[r]).
+template <bool C6, bool SW, int APT, bool NPT = false>
 __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__restrict__ atom,
                                                    const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                    float4 *__restrict__ pos, int k0, float tol_rms, int max_iter,
-                                                   double *__restrict__ rms_out, int *__restrict__ iters_out) {
+                                                   double *__restrict__ rms_out, int *__restrict__ iters_out,
+                                                   const double4 *__restrict__ box) {
     extern __shared__ float4 s_dyn[];
+    if constexpr (NPT) {
+        const double4 b = box[blockIdx.x];
+        p.Lx = (float)b.x; p.Ly = (float)b.y; p.Lz = (float)b.z;
+        p.iLx = (float)(1.0 / b.x); p.iLy = (float)(1.0 / b.y); p.iLz = (float)(1.0 / b.z);
+    }
     const int stride = APT == 1 ? RX_MAX_ATOMS : p.N;
     float4 *s_pos = s_dyn, *s_par = s_dyn + stride;
     __shared__ float s_part[32][3];
@@ -1174,20 +1338,23 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
     const bool wide = N > RX_MAX_ATOMS;
     const int threads = wide ? ((N + 4 * 32 - 1) / (4 * 32)) * 32 : ((N + 31) / 32) * 32;
     const size_t smem = (size_t)2 * (wide ? N : RX_MAX_ATOMS) * sizeof(float4);
-#define RX_LAUNCH_MINIMIZE(C6, SW)                                                                                         \
+#define RX_LAUNCH_MINIMIZE_NPT(C6, SW, NP)                                                                                 \
     do {                                                                                                                   \
         if (wide) {                                                                                                        \
-            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_minimize<C6, SW, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            k_minimize<C6, SW, 4><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
-                                                                         (float)tolerance, max_iterations, d_rms, d_iters); \
+            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_minimize<C6, SW, 4, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            k_minimize<C6, SW, 4, NP><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
+                                                                             (float)tolerance, max_iterations, d_rms, d_iters, h->d_box); \
         } else {                                                                                                           \
-            k_minimize<C6, SW, 1><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
-                                                                         (float)tolerance, max_iterations, d_rms, d_iters); \
+            k_minimize<C6, SW, 1, NP><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
+                                                                             (float)tolerance, max_iterations, d_rms, d_iters, h->d_box); \
         }                                                                                                                  \
     } while (0)
+#define RX_LAUNCH_MINIMIZE(C6, SW)                                                                                         \
+    do { if (h->npt) RX_LAUNCH_MINIMIZE_NPT(C6, SW, true); else RX_LAUNCH_MINIMIZE_NPT(C6, SW, false); } while (0)
     if (p.c_is_6) { if (p.use_switch) RX_LAUNCH_MINIMIZE(true, true); else RX_LAUNCH_MINIMIZE(true, false); }
     else { if (p.use_switch) RX_LAUNCH_MINIMIZE(false, true); else RX_LAUNCH_MINIMIZE(false, false); }
 #undef RX_LAUNCH_MINIMIZE
+#undef RX_LAUNCH_MINIMIZE_NPT
     RX_CHECK_CUDA(h, cudaGetLastError());
     return RX_OK;
 }
@@ -1211,7 +1378,8 @@ int rxi_randomize_velocities(rx_engine *h, uint64_t seed, uint64_t stream_id) {
 
 // Energy rows of the owned replicas at `n_states` states described by the device table `d_states`, written to
 // d_out[K][n_states] (rows [k0, k0+kloc)).  The resident table/matrix are the default.
-int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_states, double *d_out, int *launches) {
+int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_states, double *d_out, int *launches,
+                               const double2 *d_npt_tab) {
     if (h->kloc == 0) return RX_OK;
     const rx_config &c = h->cfg;
     if (c.system_kind == RX_SYSTEM_MOLECULE) {
@@ -1236,17 +1404,22 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     p.c_is_6 = (c.softcore_c == 6.0); p.sc_c = c.softcore_c;
     p.pair_cap = h->pair_cap;
     const size_t smem = (size_t)3 * c.n_atoms * sizeof(double);
-    const int rco = smem_opt_in(h, (const void *)k_energy_rows, (int)smem);
+    if (h->npt && !d_npt_tab)
+        RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at: a constant-pressure engine needs the states' pressures (rx_compute_energies_at_npt)");
+    if (!h->npt && d_npt_tab)
+        RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at_npt: the engine has no pressure (rx_set_pressures)");
+    auto kern = h->npt ? k_energy_rows<true> : k_energy_rows<false>;
+    const int rco = smem_opt_in(h, (const void *)kern, (int)smem);
     if (rco) return rco;
-    k_energy_rows<<<h->kloc, 512, smem, h->stream>>>(p, h->d_atom_d, h->d_alch_list, d_states, h->d_pos, h->k0,
-                                                    (double2 *)h->d_pairs, d_out, h->d_err);
+    kern<<<h->kloc, 512, smem, h->stream>>>(p, h->d_atom_d, h->d_alch_list, d_states, h->d_pos, h->k0,
+                                           (double2 *)h->d_pairs, d_out, h->d_err, h->d_box, d_npt_tab);
     RX_CHECK_CUDA(h, cudaGetLastError());
     (*launches)++;
     return RX_OK;
 }
 
 int rxi_compute_energy_rows(rx_engine *h, int *launches) {
-    return rxi_compute_energy_rows_at(h, h->d_states, h->cfg.n_states, h->d_u, launches);
+    return rxi_compute_energy_rows_at(h, h->d_states, h->cfg.n_states, h->d_u, launches, h->npt ? h->d_npt : nullptr);
 }
 
 

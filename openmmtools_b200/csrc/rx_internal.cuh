@@ -123,6 +123,11 @@ struct rx_engine {
     // timing
     double phase_ms[4] = {0, 0, 0, 0};
     long long phase_launches[4] = {0, 0, 0, 0};
+    // constant pressure (rx_set_pressures): per owned replica box (x, y, z, -) and barostat state, per state (p, c)
+    bool npt = false;
+    double4 *d_box = nullptr, *d_box_snap = nullptr;
+    rx_barostat_state *d_baro = nullptr, *d_baro_snap = nullptr;
+    double2 *d_npt = nullptr;
     // nccl
     void *nccl_lib = nullptr;
     void *nccl_comm = nullptr;
@@ -186,7 +191,8 @@ void rxi_free_implicit_solvent(rx_engine *h);
 int rxi_snapshot_state(rx_engine *h);   // positions + velocities at the start of a propagation
 int rxi_restore_failed(rx_engine *h);   // replicas with a NaN flag go back to the snapshot; d_retry = the flags
 int rxi_compute_energy_rows(rx_engine *h, int *launches);  // fills d_u rows [k0, k0+kloc)
-int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_states, double *d_out, int *launches);
+int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_states, double *d_out, int *launches,
+                               const double2 *d_npt_tab = nullptr);   // NPT: (pressure, dispersion) of those states
 int rxi_randomize_velocities(rx_engine *h, uint64_t seed, uint64_t stream_id);
 int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_rms, int *d_iters);  // [K] each
 int rxi_convert_in(rx_engine *h, float4 *dst, int first_local, int count, const double *host_xyz, bool is_vel);

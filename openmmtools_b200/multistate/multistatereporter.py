@@ -34,6 +34,7 @@ class MultiStateReporter:
         'states': ('i4', lambda K, M: (K,)),
         'accepted': ('i4', lambda K, M: (M, M)),
         'proposed': ('i4', lambda K, M: (M, M)),
+        'volumes': ('f8', lambda K, M: (K,)),      # constant-pressure runs only
     }
 
     def __init__(self, storage, open_mode=None, checkpoint_interval=50, checkpoint_storage=None,
@@ -231,6 +232,14 @@ class MultiStateReporter:
 
     def read_replica_thermodynamic_states(self, iteration=slice(None)):
         return self._read_record('states', iteration).astype(np.int64)
+
+    def write_volumes(self, volumes, iteration):
+        """Box volume (nm^3) of every replica at this iteration: the reference's 'volumes' f8[iteration, replica]
+        (multistatereporter.py:1640-1651), written by constant-pressure runs."""
+        self._write_record('volumes', iteration, volumes)
+
+    def read_volumes(self, iteration=slice(None)):
+        return self._read_record('volumes', iteration)
 
     def write_mixing_statistics(self, n_accepted_matrix, n_proposed_matrix, iteration):
         self._write_record('accepted', iteration, n_accepted_matrix)

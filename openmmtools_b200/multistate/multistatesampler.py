@@ -225,6 +225,9 @@ class MultiStateSampler:
         if self._seed is None:
             self._seed = extra.get('seed')
         self._create_engine()
+        if 'barostat' in extra:     # the NPT run continues with the barostat state it had at the checkpoint
+            self._engine.set_barostat({k: np.asarray(v)[self._engine.k0:self._engine.k1] for k, v in extra['barostat'].items()},
+                                      first=self._engine.k0)
         # energies of the checkpoint iteration are what the next mixing uses
         self._engine.set_energies(self._energy_thermodynamic_states)
         # put the two MT19937 streams back where they were
@@ -453,11 +456,17 @@ class MultiStateSampler:
                 s._velocities = self._host_v[r]
         # (the dirty flag is cleared by _sync_sampler_states, which also re-attaches the energies)
 
+    @property
+    def _npt(self):
+        return self._thermodynamic_states[0].pressure is not None
+
     def _upload_sampler_states(self):
         e = self._engine
         K = len(self._sampler_states)
         x = np.stack([s._positions for s in self._sampler_states])
         e.set_positions(x)
+        if self._npt:     # each replica propagates in its own box
+            e.set_boxes(_backend.box_edges(self._sampler_states))
         have_v = [s._velocities is not None for s in self._sampler_states]
         if all(have_v):
             e.set_velocities(np.stack([s._velocities for s in self._sampler_states]))
@@ -484,6 +493,9 @@ class MultiStateSampler:
             e.get_positions(out=self._host_x)
             e.get_velocities(out=self._host_v)
         pot, kin = e.get_replica_energies()
+        if self._npt and e.k1 > e.k0:     # the barostat's boxes go back into the SamplerStates like the positions
+            for r, edges in enumerate(e.get_boxes()):
+                self._sampler_states[e.k0 + r]._box_vectors = np.diag(edges)
         st = self._host_store
         if st is not None:
             st.pot[:] = pot[e.k0:e.k1]
@@ -580,6 +592,8 @@ class MultiStateSampler:
         if self._reporter is not None:
             if self._world_size > 1:
                 self._gather_sampler_states()
+                if self._npt:
+                    self._last_npt_records = self._gather_npt_records()
             if self._rank == 0:
                 self._reporter.write_sampler_states(self._sampler_states, self._iteration, extra=self._checkpoint_extra())
 
@@ -646,8 +660,13 @@ class MultiStateSampler:
         if self._unsampled_states:
             # energies at states that are evaluated but never sampled (multistatesampler.py:1452-1456,1489-1494)
             if self._unsampled_table is None:
-                _, self._unsampled_table = _backend.engine_tables(list(self._thermodynamic_states[:1]) + list(self._unsampled_states))
+                both = list(self._thermodynamic_states[:1]) + list(self._unsampled_states)
+                _, self._unsampled_table = _backend.engine_tables(both)
                 self._unsampled_table = {k: v[1:] for k, v in self._unsampled_table.items()}
+                npt = _backend.pressure_tables(both)
+                if npt is not None:     # (the dispersion corrections go to the engine as c_l / V)
+                    self._unsampled_table.update(energy_offset=np.zeros(len(self._unsampled_states)), pressure=npt[0][1:],
+                                                 dispersion=npt[1][1:])
             self._energy_unsampled_states[:, :] = self._engine.compute_energies_at(**self._unsampled_table)
 
     # ------------------------------------------------------------------ bookkeeping
@@ -672,10 +691,15 @@ class MultiStateSampler:
 
     def _checkpoint_extra(self):
         e = self._engine
-        return dict(seed=int(self._seed), iteration=int(self._iteration),
-                    mt_numba_words=int(e.mix_stream_position(_lib.RX_STREAM_NUMBA)),
-                    mt_numpy_words=int(e.mix_stream_position(_lib.RX_STREAM_NUMPY)),
-                    equil_counter=int(getattr(self, '_equil_counter', 0)))
+        extra = dict(seed=int(self._seed), iteration=int(self._iteration),
+                     mt_numba_words=int(e.mix_stream_position(_lib.RX_STREAM_NUMBA)),
+                     mt_numpy_words=int(e.mix_stream_position(_lib.RX_STREAM_NUMPY)),
+                     equil_counter=int(getattr(self, '_equil_counter', 0)))
+        if self._npt:     # (rank 0: the records gathered for this iteration's report)
+            rec = self._last_npt_records if self._world_size > 1 else self._local_npt_records()
+            extra['barostat'] = dict(volume_scale=rec[:, 3].tolist(),
+                                     **{f: [int(q) for q in rec[:, c]] for c, f in ((4, 'step'), (5, 'n_attempted'), (6, 'n_accepted'))})
+        return extra
 
     def _report_iteration(self):
         """multistatesampler.py:1191-1207: states, checkpointed positions, mixing statistics, energies, commit marker."""
@@ -689,11 +713,14 @@ class MultiStateSampler:
             self._sync_sampler_states()
             if self._world_size > 1:
                 self._gather_sampler_states()
+        npt = self._last_npt_records = self._gather_npt_records() if self._npt else None
         if self._rank != 0:
             self._report_iteration_items()
             return
         r = self._reporter
         r.write_replica_thermodynamic_states(self._replica_thermodynamic_states, it)
+        if npt is not None:      # the reference's per-iteration 'volumes' (multistatereporter.py:1640-1651)
+            r.write_volumes(np.prod(npt[:, :3], axis=1), it)
         if checkpoint or analysis:
             r.write_sampler_states(self._sampler_states, it, extra=self._checkpoint_extra())
         r.write_mixing_statistics(self._n_accepted_matrix, self._n_proposed_matrix, it)
@@ -712,14 +739,45 @@ class MultiStateSampler:
         if comm is None:
             from .._dist import default_communicator
             comm = self._communicator = default_communicator()
-        shard = [(k, s._positions, s._velocities) + s._energies_md()
-                 for k, s in zip(range(e.k0, e.k1), self._sampler_states[e.k0:e.k1])]
+        npt = self._local_npt_records() if self._npt else None
+        shard = [(k, s._positions, s._velocities) + s._energies_md() + (None if npt is None else npt[r],)
+                 for r, (k, s) in enumerate(zip(range(e.k0, e.k1), self._sampler_states[e.k0:e.k1]))]
         gathered = comm.gather_object(shard)
         if self._rank == 0:
             for part in gathered:
-                for k, x, v, pe, ke in part:
+                for k, x, v, pe, ke, rec in part:
                     if not (e.k0 <= k < e.k1):   # (this rank's own states are already current)
                         self._sampler_states[k]._update(x, v, pe, ke)
+                        if rec is not None:
+                            self._sampler_states[k]._box_vectors = np.diag(rec[:3])
+
+    def _local_npt_records(self):
+        """(K_loc, 7): box edges and barostat state (volume_scale, step, n_attempted, n_accepted) of the owned replicas."""
+        e = self._engine
+        if e.k1 == e.k0:
+            return np.zeros((0, 7))
+        b = e.get_barostat()
+        return np.column_stack([e.get_boxes(), b['volume_scale'], b['step'], b['n_attempted'], b['n_accepted']])
+
+    def _gather_npt_records(self):
+        """(K, 7) records of every replica on rank 0 (None elsewhere); every rank takes part."""
+        rec = self._local_npt_records()
+        if self._world_size == 1:
+            return rec
+        e = self._engine
+        comm = self._communicator
+        if comm is None:
+            from .._dist import default_communicator
+            comm = self._communicator = default_communicator()
+        shard = [(k, np.zeros((0, 3)), None, None, None, rec[r]) for r, k in enumerate(range(e.k0, e.k1))]
+        gathered = comm.gather_object(shard)
+        if self._rank != 0:
+            return None
+        out = np.zeros((self.n_replicas, 7))
+        for part in gathered:
+            for item in part:
+                out[item[0]] = item[5]
+        return out
 
     # ------------------------------------------------------------------ online analysis (multistatesampler.py:1625-1695)
     @staticmethod

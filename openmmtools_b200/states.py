@@ -5,8 +5,9 @@ Mirrors /root/reference/openmmtools/states.py: ``ThermodynamicState`` (:385), ``
 ``create_thermodynamic_state_protocol`` (:39-141).  No OpenMM objects are held: the "system" is a
 :class:`openmmtools_b200.system.System` parameter record, and energies are evaluated by the CUDA engine
 (``ThermodynamicState.reduced_potential`` -> ``rx_compute_energies``).  OpenMM-typed methods
-(``create_context``, ``apply_to_context`` ...) raise ``NotImplementedError``; NPT plumbing (pressure,
-barostats, surface tension; states.py:1510-1843) is out of scope (the configurations are NVT).
+(``create_context``, ``apply_to_context`` ...) raise ``NotImplementedError``.  A pressure puts a periodic LJ system in the
+NPT ensemble with an isotropic Monte Carlo barostat that the CUDA engine runs (states.py:1741-1771); surface tensions
+and anisotropic or membrane barostats are not provided.
 """
 import copy
 import numpy as np
@@ -29,6 +30,7 @@ class ThermodynamicsError(Exception):
         INCOMPATIBLE_SAMPLER_STATE: 'The sampler state has a different number of particles.',
         INCOMPATIBLE_ENSEMBLE: 'Cannot apply to a context in a different thermodynamic ensemble.',
         UNSUPPORTED_BAROSTAT: 'NPT ensembles are outside the GPU replica-exchange hot path.',
+        BAROSTATED_NONPERIODIC: 'Non-periodic systems cannot have a barostat.',
     }
 
     def __init__(self, code, *args):
@@ -57,7 +59,13 @@ class GlobalParameterError(Exception):
 
 # ------------------------------------------------------------------------------------------------------
 class ThermodynamicState:
-    """Thermodynamic state of a system: (system, temperature) in the NVT ensemble (states.py:385-1926)."""
+    """Thermodynamic state of a system (states.py:385-1926): (system, temperature) in the NVT ensemble, or
+    (system, temperature, pressure) in the NPT ensemble.
+
+    A pressure adds what ``MonteCarloBarostat(pressure, temperature)`` adds in the reference (states.py:1761-1771): an
+    isotropic Monte Carlo volume move at the state's temperature, attempted every 25 steps (OpenMM's default frequency,
+    fixed here).  Only periodic systems take a pressure; surface tensions are not provided.
+    """
 
     def __init__(self, system, temperature=None, pressure=None, surface_tension=None):
         if not isinstance(system, System):
@@ -65,12 +73,14 @@ class ThermodynamicState:
                             '(see openmmtools_b200.testsystems); got %r' % type(system))
         if temperature is None:
             raise ThermodynamicsError(ThermodynamicsError.NONE_TEMPERATURE)
-        if pressure is not None or surface_tension is not None:
-            raise NotImplementedError('pressure / surface tension (NPT) are outside the replica-exchange hot path')
+        if surface_tension is not None:
+            raise NotImplementedError('surface tension (membrane barostats) is outside the replica-exchange hot path')
         self._standard_system = system.copy()
         self._standard_system_hash = self._standard_system.standard_hash()
         self._temperature = None
+        self._pressure = None
         self.temperature = temperature
+        self.pressure = pressure
 
     # -- system
     @property
@@ -113,15 +123,33 @@ class ThermodynamicState:
 
     @property
     def pressure(self):
-        return None
+        """Pressure of the NPT ensemble, or None in the NVT ensemble (states.py:679-703)."""
+        return None if self._pressure is None else self._pressure * unit.bar
 
     @pressure.setter
     def pressure(self, value):
-        if value is not None:
-            raise NotImplementedError('NPT is outside the replica-exchange hot path')
+        if value is None:
+            self._pressure = None
+            return
+        if not self.is_periodic:
+            raise ThermodynamicsError(ThermodynamicsError.BAROSTATED_NONPERIODIC)
+        if not (isinstance(value, unit.Quantity) and value.unit.is_compatible(unit.bar)):
+            raise TypeError('pressure must be a Quantity with units of pressure (e.g. 1.0 * unit.bar), got %r' % (value,))
+        p = float(value / unit.bar)
+        if not p > 0:
+            raise ValueError('pressure must be positive')
+        self._pressure = p
+
+    @property
+    def _pressure_md(self):
+        """The pressure in kJ/mol/nm^3 (1 bar = 0.0602214076 kJ/mol/nm^3), or None."""
+        if self._pressure is None:
+            return None
+        return float(unit.to_md(self._pressure * unit.bar * unit.AVOGADRO_CONSTANT_NA))
 
     @property
     def barostat(self):
+        """None: the barostat is not an object here (the engine runs it); see ``pressure``."""
         return None
 
     @property
@@ -168,8 +196,10 @@ class ThermodynamicState:
 
     # -- compatibility
     def is_state_compatible(self, thermodynamic_state):
-        """Same standard system, i.e. the two states differ only in thermodynamic parameters (states.py:994-1050)."""
-        return self._standard_system_hash == thermodynamic_state._standard_system_hash
+        """Same standard system and ensemble, i.e. the two states differ only in thermodynamic parameters
+        (states.py:994-1050)."""
+        return (self._standard_system_hash == thermodynamic_state._standard_system_hash and
+                (self._pressure is None) == (thermodynamic_state._pressure is None))
 
     def is_context_compatible(self, context):
         raise NotImplementedError('no OpenMM Context on the GPU path')
@@ -184,7 +214,7 @@ class ThermodynamicState:
     def _engine_parameters(self):
         s = self._standard_system
         return dict(temperature=self._temperature, lambda_sterics=s.global_parameters.get('lambda_sterics', 1.0),
-                    ho_K=s.ho_K, ho_x0=s.ho_x0, ho_U0=s.ho_U0)
+                    ho_K=s.ho_K, ho_x0=s.ho_x0, ho_U0=s.ho_U0, pressure=self._pressure_md)
 
     # -- copies share the (immutable) standard system like the reference (states.py:1235-1253)
     def __copy__(self):
@@ -206,6 +236,7 @@ class ThermodynamicState:
 
     def __setstate__(self, d):
         self.__dict__.update(d)
+        self.__dict__.setdefault('_pressure', None)
 
 
 # ------------------------------------------------------------------------------------------------------
