@@ -40,7 +40,7 @@ struct SlotRec {        // one 2-word "slot" of the stream, state independent (p
 };
 
 struct MixCtl {          // device-resident control block of the resumable mixing kernels
-    long long head;      // in: first unconsumed word (serial) / slot (pow2);  out: same after the call
+    long long head;      // in: first unconsumed word (K not a power of two) / slot (power-of-two K);  out: same after the call
     long long remaining; // attempts still to do
     int status;          // 0 done, 1 need more words
     int rounds;          // statistics: speculation rounds executed

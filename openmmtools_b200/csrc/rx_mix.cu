@@ -13,7 +13,9 @@
 // even word ("slot"), so a parallel pre-pass turns the stream into slot records (i, j, log U, overlap mask)
 // and ONE warp then walks the chain speculatively: 32 lanes evaluate 32 consecutive slots under the current
 // permutation, the visited-slot chain is resolved with a carry-propagation bit trick, and the longest prefix
-// in which no visited slot touches a replica swapped earlier in the same window is committed.
+// in which no visited slot touches a replica swapped earlier in the same window is committed.  The filter walkers
+// (rx_walk2.cuh, rx_walk2c.cuh) take the bulk of a pass for K <= 256; the exact walker (rx_walk_exact.cuh) finishes
+// their passes over slots and walks every pass of larger K.
 #include "rx_internal.cuh"
 #include <type_traits>
 #include <math.h>
@@ -170,310 +172,18 @@ int rxi_selftest_exp(rx_engine *h, const double *x, double *y, int n) {
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Slot records (state independent, fully parallel).
+// The speculative chain walkers: the filter walkers (rx_walk2.cuh, rx_walk2c.cuh) and the exact walker
+// (rx_walk_exact.cuh).  Their state-independent records (slot records: k_slots_build, rx_walk2.cuh) are built in
+// parallel; each logs the attempts it commits as packed (si, sj, accepted) entries, bit 31 set.
 // ------------------------------------------------------------------------------------------------------
 #define LOGU_ZERO (-745.5)  /* stands in for log(0): exp(x) == 0 <=> x < -745.13 */
-
-__global__ void __launch_bounds__(256) k_slots_build(const uint32_t *__restrict__ words, long long nslots,
-                                                     uint32_t mask, SlotRec *__restrict__ rec) {
-    __shared__ uint32_t s_ij[256 + 32];
-    long long s0 = (long long)blockIdx.x * 256;
-    int t = threadIdx.x;
-    // tile: slots s0-32 .. s0+255
-    for (int q = t; q < 256 + 32; q += 256) {
-        long long s = s0 - 32 + q;
-        uint32_t ij = 0xffffffffu;
-        if (s >= 0 && s < nslots) ij = (words[2 * s] & mask) | ((words[2 * s + 1] & mask) << 16);
-        s_ij[q] = ij;
-    }
-    __syncthreads();
-    long long s = s0 + t;
-    if (s >= nslots) return;
-    uint32_t w0 = words[2 * s], w1 = words[2 * s + 1];
-    uint32_t ij = s_ij[t + 32];
-    uint32_t i = ij & 0xffffu, j = ij >> 16;
-    uint32_t bm = 0;
-#pragma unroll
-    for (int b = 0; b < 31; b++) {
-        uint32_t o = s_ij[t + 32 - 1 - b];
-        uint32_t oi = o & 0xffffu, oj = o >> 16;
-        bool hit = (o != 0xffffffffu) && (oi == i || oi == j || oj == i || oj == j);
-        bm |= (hit ? 1u : 0u) << (31 - b);
-    }
-    double U = mt_double(w0, w1);
-    SlotRec r;
-    r.ij = ij;
-    r.backmask = bm;
-    r.logU = (U == 0.0) ? LOGU_ZERO : log(U);
-    rec[s] = r;
-}
-
-// ------------------------------------------------------------------------------------------------------
-// The speculative chain walker.  K must be a power of two <= 16384.
-//
-// One warp walks (a second one only helps with the prologue).  The slot records come from DRAM (written once by the
-// pre-pass, read once) into a 1024-slot shared-memory ring by cp.async that the walker issues itself, 512 slots ahead.
-// Per round the warp (1) reads 32 records from the ring, (2) looks up the current states of both replicas, (3) fetches
-// u[i,sj], u[j,si] and the maintained diagonal d[k] = u[k, perm[k]], (4) evaluates log_p and the accept test, (5) resolves
-// the visited chain and staleness with ballots and bit tricks, (6) commits the valid prefix: permutation + diagonal
-// in shared memory and ONE coalesced store of packed (si, sj, accepted) entries into a commit log (the count
-// matrices are built from the log afterwards by k_mix_count, in parallel).
-// (Round 1 had a producer warp and a ring synchronised by fences and volatile flags; the single warp with hardware-tracked
-// copies is racecheck-clean and costs ~6 more instructions per round.)
-//
-// Where the energies live (UMODE):
-//   U_FILTER24   the default for K <= 256 (at K = 256 the 512 KB of f64 do not fit; at smaller K the f32 filter is
-//                still faster than f64 comparisons): shared memory holds a 24-bit floating image of every row
-//                (delta = u - rowmin as a float32 truncated to sign + 8 exponent + 15 mantissa bits) that gives log_p
-//                to within a RIGOROUS bound eps = 3.2e-5 * sum|delta| + tiny; the decision is taken from the image, in
-//                f32, whenever it is more than eps away from both thresholds (log_p = 0 and log_p = log U); a round
-//                whose committed prefix contains an undecided lane is redone with the exact f64 values from L2.
-//                The result is therefore still bit-identical.
-//   U_F64_SMEM   the f64 matrix itself is in shared memory (K <= 128; RX_F64_SMEM=1 or RX_NO_FILTER=1)
-//   U_GLOBAL     exact f64 values from L2 every round (any larger K, or K = 256 with RX_NO_FILTER=1)
-//
-// The walker's round is one dependent chain (~105 instructions); what shortens it: no f64 on the chain, no
-// data-dependent branch besides the loop's (one loop condition, predicated commit), no sub-word shared stores (a
-// byte-wide permutation table is slower), the absolute-to-relative lane
-// conversion as one shift (back-mask bit order), and nothing re-derived from special registers inside the loop.
-// ------------------------------------------------------------------------------------------------------
 #define LOG_ACC_BIT 28
 #define LOG_STATE_BITS 14
-#define RING 1024
-enum { U_F64_SMEM = 0, U_FILTER24 = 1, U_GLOBAL = 2 };
 #include "rx_walk2.cuh"
-
-struct WalkShared {     // control words shared by the two warps
-    volatile unsigned prod;   // records [0, prod) of this pass are in the ring (modulo RING)
-    volatile unsigned head;   // walker position
-    volatile unsigned done;
-};
-#include "rx_walk_any.cuh"
+#include "rx_walk_exact.cuh"
 #include "rx_walk2c.cuh"
 
-// REC2: the records are SlotRec2 (rx_walk2.cuh); only with U_FILTER24, where this kernel finishes the passes of k_mix_walk2.
-template <int UMODE, bool REC2 = false>
-__global__ void __launch_bounds__(64) k_mix_walk_pow2(const SlotRec *__restrict__ rec, const uint32_t *__restrict__ words,
-                                                      unsigned nslots, const double *__restrict__ u, int K, int logK,
-                                                      int *__restrict__ perm_g, uint32_t *__restrict__ commit_log,
-                                                      const unsigned char *__restrict__ filt,
-                                                      const double *__restrict__ filt_rowabs, MixCtl *ctl) {
-    extern __shared__ double s_mix[];
-    // layout: ring[RING] 16-byte records | diag[K] f64 | (rowabs[K]) | (u f64 [K*K]) | perm[K] i32 | (image: u16[K*K] + u8[K*K])
-    uint4 *s_ring = (uint4 *)s_mix;
-    double *s_diag = s_mix + 2 * RING;
-    double *s_rowabs = s_diag + K;                                   // [K] |row minimum| (U_FILTER24 only)
-    double *s_u = s_rowabs + (UMODE == U_FILTER24 ? K : 0);
-    int *s_perm = (int *)(s_u + (UMODE == U_F64_SMEM ? (size_t)K * K : 0));
-    unsigned char *s_q = (unsigned char *)(s_perm + K);   // 24-bit image: int16 high plane [K*K] then uint8 low plane [K*K]
-    // (the warp index through a shuffle: warp-uniform for the compiler, see k_mix_walk2)
-    const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    for (int q = tid; q < K; q += 64) {
-        const int st = perm_g[q];
-        s_perm[q] = st;
-        s_diag[q] = u[((size_t)q << logK) + st];
-        // per-row share of the f64-rounding bound, f32 rounded up: 1.6e-14 (|row minimum| + 1/2)
-        if (UMODE == U_FILTER24) ((float *)s_rowabs)[q] = __fmul_ru(1.6e-14f, __fadd_ru(__double2float_ru(filt_rowabs[q]), 0.5f));
-    }
-    if (UMODE == U_F64_SMEM)
-        for (int q = tid; q < K * K; q += 64) s_u[q] = u[q];
-    if (UMODE == U_FILTER24) {
-        const uint32_t *src = (const uint32_t *)filt;
-        uint32_t *dst = (uint32_t *)s_q;
-        for (int q = tid; q < (3 * K * K) / 4; q += 64) dst[q] = src[q];
-    }
-    const unsigned head0 = (unsigned)ctl->head;
-    __syncthreads();
-    if (warp != 0) return;   // (the second warp only helps with the prologue)
-
-    // The records come into the ring by cp.async issued by the walker itself, 640 slots ahead, topped up every 8 rounds;
-    // completion is tracked by the hardware (cp.async.wait_group), the warp barrier at the end of a round makes the data
-    // visible to all lanes.  No second warp,
-    // no flags, no fences: nothing for racecheck to find.
-    // (32-bit shared address through a shuffle: it then lives in a register instead of being re-derived from SR_CgaCtaId
-    // every round)
-    const unsigned ring_addr = __shfl_sync(0xffffffffu, (unsigned)__cvta_generic_to_shared((const void *)s_ring), 0);
-    const uint4 *recs = (const uint4 *)rec;
-    unsigned filled = head0;
-    auto refill = [&](unsigned h_now) {
-        while (filled < h_now + 640u && filled < nslots) {
-            if (filled + (unsigned)lane < nslots)
-                w2_cp_async16(ring_addr + (((filled + (unsigned)lane) & (RING - 1)) << 4), recs + (filled + lane));
-            filled += 32u;
-        }
-        w2_cp_async_commit();
-    };
-    refill(head0);
-    w2_cp_async_wait<0>();
-    __syncwarp();
-
-    // ---------------- walker (warp 0).  The loop is latency bound (one warp, one dependent chain per round), so it is
-    // written for a short instruction stream: 32-bit indices, cached producer position, head published every 8 rounds.
-    unsigned h = head0;
-    const long long remaining0 = ctl->remaining;
-    unsigned rem = remaining0 > 0x7fffffffLL ? 0x7fffffffu : (unsigned)remaining0;   // attempts this launch may still do
-    const unsigned rem0 = rem;
-    unsigned logpos = (unsigned)ctl->log_count, rounds = 0, slow = 0;   // the log continues where k_mix_walk2 stopped
-    const unsigned lt_mask = (1u << lane) - 1u;
-    const unsigned sh_amt = 32u - (unsigned)lane;
-    const unsigned short *s_qhi = (const unsigned short *)s_q;            // [K*K] sign, exponent, 7 mantissa bits
-    const unsigned char *s_qlo = s_q + 2 * (size_t)K * K;                  // [K*K] next 8 mantissa bits
-    unsigned wpos = (h + (unsigned)lane) & (RING - 1);   // this lane's ring slot
-    // One round.  TAIL = the launch's attempt budget may end inside the window (checked only in the last rounds).
-    auto round = [&](auto tail_tag) {
-        constexpr bool TAIL = decltype(tail_tag)::value;
-        rounds++;
-        const unsigned w = wpos;   // (h + lane) & (RING - 1), carried from round to round
-        const uint4 rq = w2_lds128(ring_addr + (w << 4));
-        const uint32_t ij = rq.x, backmask = rq.y;
-        // the uniform an attempt here would draw belongs to the NEXT slot (SlotRec: its f64 logU is words z, w of the record)
-        double logU_next = 0.0;
-        if (UMODE != U_FILTER24 || !REC2) {
-            const uint2 lw = w2_lds64(ring_addr + (((w + 1) & (RING - 1)) << 4) + 8u);
-            logU_next = __hiloint2double((int)lw.y, (int)lw.x);
-        }
-        const unsigned i = ij & 0xffffu, j = ij >> 16;
-        const int si = s_perm[i], sj = s_perm[j];
-        const unsigned a_ij = (i << logK) | (unsigned)sj, a_ji = (j << logK) | (unsigned)si;
-        bool ge0, acc, undecided = false;
-        double e_ij = 0.0, e_ji = 0.0;   // exact off-diagonal values, needed by the commit (new diagonal)
-        if (UMODE == U_FILTER24) {
-            // image of u: 24-bit floats of delta = u - rowmin; logp~ = (d_ii - d_ij) + (d_jj - d_ji), |logp~ - logp_ref| <= eps
-            const unsigned a_ii = (i << logK) | (unsigned)si, a_jj = (j << logK) | (unsigned)sj;
-            // (hi << 16) | (lo << 8) in one byte permute
-            const float f_ii = __uint_as_float(__byte_perm((unsigned)s_qhi[a_ii], (unsigned)s_qlo[a_ii], 0x1045));
-            const float f_ij = __uint_as_float(__byte_perm((unsigned)s_qhi[a_ij], (unsigned)s_qlo[a_ij], 0x1045));
-            const float f_jj = __uint_as_float(__byte_perm((unsigned)s_qhi[a_jj], (unsigned)s_qlo[a_jj], 0x1045));
-            const float f_ji = __uint_as_float(__byte_perm((unsigned)s_qhi[a_ji], (unsigned)s_qlo[a_ji], 0x1045));
-            // All in f32.  Every image value is within 2^-15 (relative) of the true delta (truncation to a 15-bit
-            // mantissa + f32 rounding); the f32 additions below add at most 2^-23 of the magnitudes; the f64 rounding
-            // of the reference's own three additions and of our centring is <= 64 ulp(f64) of the magnitudes.
-            const float lp = (f_ii - f_ij) + (f_jj - f_ji);
-            const float mag = (fabsf(f_ii) + fabsf(f_ij)) + (fabsf(f_jj) + fabsf(f_ji));
-            // the guard band's 1e-9 rides in eps (a slightly wider eps for the sign test is only more conservative);
-            // 1.6e-14 mag is inside the slack of 3.2e-5
-            const float eps = fmaf(mag, 3.2e-5f, (((const float *)s_rowabs)[i] + ((const float *)s_rowabs)[j]) + 1e-9f);
-            // log of the uniform, rounded to f32 by the producer: |lu - logU| <= 2^-24 |lu|; d carries one more rounding
-            // (SlotRec2: the f32 log-uniform of the next slot is the third word of this slot's own record)
-            const float lu = REC2 ? __uint_as_float(rq.z) : (float)logU_next;
-            const float d = lp - lu;
-            const float mar = fmaf(fabsf(lp) + fabsf(lu), 1.3e-7f, eps);
-            // |lp| > eps decides the sign of log_p, |d| > mar decides the comparison with the uniform (NaN: undecided)
-            const bool dec_lp = fabsf(lp) > eps, dec_d = fabsf(d) > mar;
-            // i == j: the reference's log_p is exactly 0 for finite energies (-(e+e)+e+e), accepted without a draw
-            const bool same = (i == j) && (fabsf(f_ii) <= 3.0e38f);
-            ge0 = (dec_lp && lp > 0.f) || same;
-            acc = ge0 || (dec_lp && dec_d && d > 0.f);
-            const bool decided = ge0 || (dec_lp && dec_d);
-            undecided = !decided;   // resolved below, and only if the lane turns out to matter
-        } else {
-            e_ij = (UMODE == U_F64_SMEM) ? s_u[a_ij] : u[a_ij];
-            e_ji = (UMODE == U_F64_SMEM) ? s_u[a_ji] : u[a_ji];
-            const double logp = swap_logp(e_ij, e_ji, s_diag[i], s_diag[j]);
-            const double d = logp - logU_next;
-            ge0 = logp >= 0.0;
-            acc = ge0 || d > 1e-9;
-            const bool ambiguous = !ge0 && fabs(d) <= 1e-9;   // NaN compares false: rejected, like the reference
-            if (__any_sync(0xffffffffu, ambiguous)) {
-                if (ambiguous) {  // too close to call in the log domain: do exactly what the reference does
-                    const unsigned s1 = h + lane + 1;
-                    acc = mt_double(words[2 * (size_t)s1], words[2 * (size_t)s1 + 1]) < rx_exp_cr(logp);
-                    slow++;
-                }
-            }
-        }
-        unsigned V, C, low, cm, n, advance;
-        auto resolve = [&]() {
-            const unsigned G = __ballot_sync(0xffffffffu, ge0);
-            const unsigned A = __ballot_sync(0xffffffffu, acc && i != j);   // accepted and really changing the permutation
-            // Visited chain: from a visited slot s the next attempt starts at s+1 if log_p >= 0 (no uniform drawn) else
-            // at s+2.  skip[s+1] = NG[s] & ~skip[s]: inside a run of NG ones the skip flag alternates, so skip[s] =
-            // parity of (s - run start); runs are split by the parity of their start with an add-carry (32-bit adds +
-            // carry out).
-            const unsigned X = ~G;
-            const unsigned starts = X & ~(X << 1);
-            const unsigned SE = starts & 0x55555555u, SO = starts & 0xAAAAAAAAu;
-            const unsigned sumE = X + SE, sumO = X + SO;
-            const unsigned skip = (((sumE ^ X) & ~SE) & 0xAAAAAAAAu) | (((sumO ^ X) & ~SO) & 0x55555555u);
-            V = ~skip;
-            const unsigned VA = V & A;  // visited, accepted, really changing the permutation
-            // lane t is stale if an earlier visited state-changing swap in this window shares a replica with it
-            unsigned earlier;   // bit 31-b: lane t-1-b is a visited state-changing swap (shl by 32 gives 0 for lane 0)
-            asm("shl.b32 %0, %1, %2;" : "=r"(earlier) : "r"(VA), "r"(sh_amt));
-            C = __ballot_sync(0xffffffffu, (earlier & backmask) != 0u) & V;
-            low = C & (0u - C);
-            cm = V & (low - 1u);           // low == 0 -> all lanes
-            n = __popc(cm);
-            // bit 32 (even position) of the skip word can only be set by the carry of an odd-start run
-            advance = C ? (unsigned)__popc(low - 1u) : 32u + (sumO < X ? 1u : 0u);
-        };
-        if (UMODE == U_FILTER24) {
-            // The filter's undecided lanes carry arbitrary ge0/acc.  Bits of V, C and cm below the lowest undecided
-            // visited lane do not depend on them (the chain and the staleness test only look downwards), so the round
-            // is resolved speculatively and redone with exact values only when such a lane lies inside the committed
-            // prefix -- the ballot of the undecided lanes is off the critical path and rarely matters.
-            const unsigned U = __ballot_sync(0xffffffffu, undecided);
-            resolve();
-            if (U & cm) {
-                if (undecided) {   // exact path for this lane: the f64 values from L2
-                    const unsigned d = w2_exact_decision(u, K, ij, (unsigned)si, (unsigned)sj, words, 2 * (size_t)(h + lane + 1));
-                    ge0 = (d & 1u) != 0u;
-                    acc = (d & 2u) != 0u;
-                    slow++;
-                }
-                resolve();
-            }
-        } else {
-            resolve();
-        }
-        if (TAIL && n > rem) {
-            unsigned pos = 0;  // the first visited lane we must NOT run: the (rem+1)-th set bit of cm
-            for (unsigned cnt = 0; pos < 32; pos++)
-                if ((cm >> pos) & 1u) { if (cnt == rem) break; cnt++; }
-            cm &= (1u << pos) - 1u;
-            n = rem;
-            advance = pos;
-        }
-        // commit: everything is computed by every lane, only the stores are predicated (no divergent block)
-        const bool mine = (cm >> lane) & 1u;
-        const unsigned log_at = logpos + __popc(cm & lt_mask);
-        const uint32_t entry = (uint32_t)si | ((uint32_t)sj << LOG_STATE_BITS) | ((acc ? 1u : 0u) << LOG_ACC_BIT);
-        const bool swaps = mine && acc && i != j;  // an i == j lane must not write: a later committed lane may swap this replica
-        if (mine) commit_log[log_at] = entry;
-        if (swaps) { s_perm[i] = sj; s_perm[j] = si; }
-        if (UMODE != U_FILTER24) { if (swaps) { s_diag[i] = e_ij; s_diag[j] = e_ji; } }   // the image needs no f64 diagonal
-        logpos += n;
-        h += advance;
-        wpos = (wpos + advance) & (RING - 1);
-        rem -= n;
-        // every 8 rounds (at most 264 slots): top the ring up to 640 slots ahead and wait for all copies but the ones just
-        // issued -- what the next 8 rounds read (< h + 298) was issued at the previous top-up or earlier (>= h + 376 then)
-        if ((rounds & 7u) == 0u) { refill(h); w2_cp_async_wait<1>(); }
-        __syncwarp();
-    };
-    while (rem > 0 && h + 33 <= nslots) {
-        if (rem >= 33) {
-            // main loop: a round commits at most 32 attempts, so the budget cannot end inside it
-            do { round(std::false_type()); } while (rem >= 33u && h + 33u <= nslots);
-        } else {
-            round(std::true_type());
-        }
-    }
-    w2_cp_async_wait<0>();
-    for (int q = lane; q < K; q += 32) perm_g[q] = s_perm[q];
-    slow = __reduce_add_sync(0xffffffffu, slow);
-    if (lane == 0) {
-        const long long remaining = remaining0 - (long long)(rem0 - rem);
-        ctl->head = h;
-        ctl->remaining = remaining;
-        ctl->status = remaining > 0 ? 1 : 0;
-        ctl->rounds += (int)rounds;
-        ctl->slow_exp += slow;
-        ctl->log_count = logpos;
-    }
-}
-
-// 24-bit row image of the energy matrix for the U_FILTER24 walker: delta = u[k,l] - min_l u[k,l] as a float32 truncated to
+// 24-bit row image of the energy matrix for the filter walkers: delta = u[k,l] - min_l u[k,l] as a float32 truncated to
 // its top 24 bits (sign, 8 exponent, 15 mantissa bits), stored as a uint16 plane followed by a uint8 plane.  Relative
 // precision 2^-15 per entry, so huge entries (a decoupled atom overlapping another one evaluated at lambda = 1) cost no
 // precision where the decisions are made.  absmax_out[k] = max |u[k,:]| (inf for rows with non-finite values).
@@ -507,13 +217,15 @@ __global__ void k_mix_filter_build(const double *__restrict__ u, int K, unsigned
     if (t == 0) { scale[k] = fabs(lo); absmax_out[k] = anybad ? INFINITY : am; }
 }
 
-// Build the (symmetric) proposal / acceptance count matrices from the commit log (replicaexchange.py:339-349).
+// Build the (symmetric) proposal / acceptance count matrices from entries [0, n) of a commit log (replicaexchange.py:339-349):
+// the exact walker's dense log, or the filter walkers' sparse one (one word per record); bit 31 = an attempt is logged there.
 __global__ void k_mix_count(const uint32_t *__restrict__ commit_log, long long n, int M, unsigned long long *__restrict__ nacc,
                             unsigned long long *__restrict__ nprop) {
     long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (; t < n; t += stride) {
         const uint32_t e = commit_log[t];
+        if (!(e >> 31)) continue;
         const uint32_t si = e & ((1u << LOG_STATE_BITS) - 1u), sj = (e >> LOG_STATE_BITS) & ((1u << LOG_STATE_BITS) - 1u);
         atomicAdd(&nprop[(size_t)si * M + sj], 1ull);
         atomicAdd(&nprop[(size_t)sj * M + si], 1ull);
@@ -802,9 +514,9 @@ static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, bool fas
             for (unsigned m = (unsigned)(K - 1); m; m >>= 1) nbits++;
             k_words_build<<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, K, 0xffffffffu >> (32 - nbits), (WordRec *)h->d_slots);
         } else if (rec2)
-            k_slots_build2<<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec2 *)h->d_slots);
+            k_slots_build<true><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec2 *)h->d_slots);
         else
-            k_slots_build<<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), h->d_slots);
+            k_slots_build<false><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), h->d_slots);
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
     }
@@ -831,53 +543,37 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         return RX_OK;
     }
     const bool fast = is_pow2(K) && K <= (1 << LOG_STATE_BITS);
-    // any other K up to 4095: the speculative walker over word positions (rx_walk_any.cuh); RX_WALK_SERIAL=1: the plain loop
+    // any other K up to 4095: the speculative walker over word positions (rx_walk_exact.cuh); RX_WALK_SERIAL=1: the plain loop
     const bool anyk = !fast && K >= 3 && K <= ANY_MAX_K && !getenv("RX_WALK_SERIAL");
     int logK = 0;
     while ((1 << logK) < K) logK++;
     const size_t smem_small = (size_t)K * sizeof(int);
-    // ring (lu 8 + ij 4 + bm 4) + diag + perm
-    const size_t smem_base = (size_t)RING * 16 + (size_t)K * (sizeof(double) + sizeof(int));
-    const size_t smem_f64 = smem_base + (size_t)K * K * sizeof(double);
-    const size_t smem_f24 = smem_base + (size_t)K * sizeof(double) + (size_t)3 * K * K;
-    int umode = U_GLOBAL;
-    // the f32 row-image filter wherever it fits (K <= 256): it beats the f64 comparisons of U_F64_SMEM at every size
-    if (fast && smem_f24 <= 224 * 1024 && !getenv("RX_NO_FILTER") && !getenv("RX_F64_SMEM")) umode = U_FILTER24;
-    else if (fast && smem_f64 <= 200 * 1024) umode = U_F64_SMEM;
-    // filter mode: 16-byte SlotRec2 records, k_mix_walk2 for the bulk of a pass and k_mix_walk_pow2<U_FILTER24, true> for its tail
-    const bool rec2 = (umode == U_FILTER24);
-    const bool walk2 = rec2 && !getenv("RX_WALK_V1");
+    // ring + diag + rowabs + perm + image
+    const size_t smem_f24 = (size_t)RING * 16 + (size_t)K * (2 * sizeof(double) + sizeof(int)) + (size_t)3 * K * K;
+    // The f32 row-image filter wherever it fits (K <= 256; at K = 256 the 512 KB of f64 would not fit in shared memory, and at
+    // smaller K the filter is still faster than f64 comparisons): 16-byte SlotRec2 records, k_mix_walk2 for the bulk of a pass
+    // and k_mix_walk_pow2<true> for its tail.  Otherwise (RX_NO_FILTER=1: every K) exact f64 values from L2.
+    const bool rec2 = fast && smem_f24 <= 224 * 1024 && !getenv("RX_NO_FILTER");
     // any K <= 256 whose row image fits: the walker of k_mix_walk2 in candidate coordinates (k_mix_walk2c, rx_walk2c.cuh);
     // RX_WALK_ANY_V1=1 keeps the word-position walker (cross-check)
     const size_t smem_w2 = (size_t)W2_RING * 16 + (size_t)K * 8 + (size_t)((3 * K + 1) & ~1) * K;   // ring, replicas, image
     const bool candk = anyk && K <= 256 && smem_w2 <= 224 * 1024 && !getenv("RX_WALK_ANY_V1") && !getenv("RX_NO_FILTER");
     const int kind = candk ? REC_CAND : (anyk ? REC_WORD : (!fast ? REC_NONE : (rec2 ? REC_SLOT2 : REC_SLOT)));
-    const size_t smem_any_f64 = smem_base + (size_t)K * K * sizeof(double);
-    const bool any_smem = anyk && smem_any_f64 <= 200 * 1024;
-    size_t smem = !fast ? smem_small : (umode == U_F64_SMEM ? smem_f64 : (umode == U_FILTER24 ? smem_f24 : smem_base));
-    // The walker is one latency-bound CTA: claim (almost) a whole SM's shared memory so that no other CTA -- in particular
-    // the stream generator that runs concurrently on the side stream -- is scheduled onto the same SM and steals issue slots.
-    size_t smem_base_launch = smem_base;
-    if (fast) {
-        // 226 KB + this kernel's static shared memory + the generator's 8 KB exceed the SM's 228 KB
-        if (smem < 226 * 1024) smem = 226 * 1024;
-        smem_base_launch = 226 * 1024;
-    }
+    // The walkers are one latency-bound CTA each: they claim (almost) a whole SM's shared memory so that no other CTA -- in
+    // particular the stream generator that runs concurrently on the side stream -- is scheduled onto the same SM and steals
+    // issue slots.  226 KB + the kernel's static shared memory + the generator's 8 KB exceed the SM's 228 KB.
+    const int smem_walk = 226 * 1024;
     if (!fast) {
-        if (smem > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_serial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (candk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2c, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-        if (anyk) {
-            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_any<U_F64_SMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_any<U_GLOBAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-        }
+        if (smem_small > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_serial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_small));
+        if (candk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2c, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
+        if (anyk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_any, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
     } else {
-        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<U_F64_SMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<U_FILTER24, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<U_GLOBAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_base_launch));
+        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
+        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
+        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
     }
     tr.mark("func attributes");
-    if (umode == U_FILTER24 || candk) {
+    if (rec2 || candk) {
         if (!h->d_filt) {
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt, (size_t)3 * K * K + 16));
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt_scale, sizeof(double) * 2 * K));
@@ -894,14 +590,14 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
     // log in ctl.aux; the pass's tail kernel continues from ctl.head.  Both claim a whole SM like the other walkers.
     auto filter_walk = [&](size_t nrec) -> int {
         static_assert(sizeof(SlotRec2) == sizeof(SlotRec), "both record formats share the d_slots buffer");
-        if (smem_w2 > 226 * 1024) RX_FAIL(h, RX_ERR_INVALID, "internal: filter walker shared memory");
+        if (smem_w2 > (size_t)smem_walk) RX_FAIL(h, RX_ERR_INVALID, "internal: filter walker shared memory");
         RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, nrec * sizeof(uint32_t), h->stream));
         if (candk)
-            k_mix_walk2c<<<1, W2_THREADS, 226 * 1024, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos,
+            k_mix_walk2c<<<1, W2_THREADS, smem_walk, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos,
                                                                     h->d_ctile + (h->ctile_cap / CAND_TILE + 4), h->d_u, K, h->d_perm,
                                                                     h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
         else
-            k_mix_walk2<<<1, W2_THREADS, 226 * 1024, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K,
+            k_mix_walk2<<<1, W2_THREADS, smem_walk, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K,
                                                                    logK, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
         RX_CHECK_CUDA(h, cudaGetLastError());
         *launches += 1;
@@ -945,14 +641,11 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
                 *launches += 1;
             }
             RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
-            if (umode == U_F64_SMEM)
-                k_mix_walk_pow2<U_F64_SMEM><<<1, 64, smem, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, nullptr, nullptr, h->d_ctl);
-            else if (umode == U_FILTER24) {
-                if (walk2 && (rc = filter_walk((size_t)nslots))) return rc;
-                k_mix_walk_pow2<U_FILTER24, true><<<1, 64, smem, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, h->d_filt, h->d_filt_scale, h->d_ctl);
-            }
-            else
-                k_mix_walk_pow2<U_GLOBAL><<<1, 64, smem_base_launch, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, nullptr, nullptr, h->d_ctl);
+            if (rec2) {
+                if ((rc = filter_walk((size_t)nslots))) return rc;
+                k_mix_walk_pow2<true><<<1, 64, smem_walk, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, h->d_filt, h->d_filt_scale, h->d_ctl);
+            } else
+                k_mix_walk_pow2<false><<<1, 64, smem_walk, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, nullptr, nullptr, h->d_ctl);
             RX_CHECK_CUDA(h, cudaGetLastError());
             RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
             tr.mark("walker");
@@ -975,15 +668,12 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
                 // bulk of the pass: speculative walker over word positions (claims the SM like the power-of-two walkers);
                 // what it leaves -- the last words of the pass -- is finished by the plain loop below
                 RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
-                if (any_smem)
-                    k_mix_walk_any<U_F64_SMEM><<<1, 64, 226 * 1024, h->stream>>>((const WordRec *)h->d_slots, S.d_words, (unsigned)S.avail, h->d_u, K, h->d_perm, h->d_log, h->d_ctl);
-                else
-                    k_mix_walk_any<U_GLOBAL><<<1, 64, 226 * 1024, h->stream>>>((const WordRec *)h->d_slots, S.d_words, (unsigned)S.avail, h->d_u, K, h->d_perm, h->d_log, h->d_ctl);
+                k_mix_walk_any<<<1, 64, smem_walk, h->stream>>>((const WordRec *)h->d_slots, S.d_words, (unsigned)S.avail, h->d_u, K, h->d_perm, h->d_log, h->d_ctl);
                 RX_CHECK_CUDA(h, cudaGetLastError());
                 RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
                 *launches += 1;
             }
-            k_mix_walk_serial<<<1, 32, smem, h->stream>>>(S.d_words, (long long)S.avail, h->d_u, K, M, h->d_perm, h->d_nacc,
+            k_mix_walk_serial<<<1, 32, smem_small, h->stream>>>(S.d_words, (long long)S.avail, h->d_u, K, M, h->d_perm, h->d_nacc,
                                                         h->d_nprop, h->d_ctl);
             RX_CHECK_CUDA(h, cudaGetLastError());
             *launches += 1;
@@ -997,7 +687,7 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         }
         // count matrices from the commit logs (k_mix_walk_serial counts as it goes)
         if (ctl.aux > 0) {   // the filter walker's sparse log
-            k_mix_count_slots<<<count_blocks(h, ctl.aux), 256, 0, h->stream>>>(h->d_slotlog, 0, ctl.aux, M, h->d_nacc, h->d_nprop);
+            k_mix_count<<<count_blocks(h, ctl.aux), 256, 0, h->stream>>>(h->d_slotlog, ctl.aux, M, h->d_nacc, h->d_nprop);
             RX_CHECK_CUDA(h, cudaGetLastError());
             *launches += 1;
         }

@@ -2,7 +2,7 @@
 // systems: k_mix_walk2 walks SLOTS (power-of-two K <= 256: an attempt starts on every even word), k_mix_walk2c walks
 // CANDIDATE indices (any other K <= 256: the words that numba's randint accepts, rx_walk2c.cuh).
 //
-// Same algorithm and the same results as k_mix_walk_pow2<U_FILTER24> (replicaexchange.py:321-349 bit for bit); what
+// Same algorithm and the same results as k_mix_walk_pow2<true> (replicaexchange.py:321-349 bit for bit); what
 // changes is the length of the dependent chain of one speculation round:
 //   * lane <-> record mapping is FIXED (lane = record index mod 32) and the window [h, h+32) rotates over the lanes, so a
 //     lane keeps its record in registers until the record leaves the window and its next record (index + 32) is
@@ -15,7 +15,7 @@
 //   * every lane copies its own records into a shared-memory ring with cp.async, 15 windows ahead of use (see W2_RING).
 // The coordinate systems differ in the visited chain (w2_chain_slots / w2_chain_cand), in where an attempt's uniform
 // lies in the stream, and in the ends of the pass.  The walkers run the bulk of a pass; the last < 600 records / < 130
-// attempts are left to k_mix_walk_pow2<U_FILTER24, true> (slots, on the same records) or k_mix_walk_serial (candidates).
+// attempts are left to k_mix_walk_pow2<true> (slots, on the same records, rx_walk_exact.cuh) or k_mix_walk_serial (candidates).
 #pragma once
 
 struct SlotRec2 {        // 16 bytes, one attempt's record (per slot or per candidate index), state independent
@@ -25,14 +25,17 @@ struct SlotRec2 {        // 16 bytes, one attempt's record (per slot or per cand
     uint32_t k;          // candidates: hop class, the attempt moves on by 2 + k candidates when it draws a uniform; slots: 0
 };
 
-// f64 log-uniform of slot s, exactly as k_slots_build computes it
+// f64 log-uniform of slot s
 __device__ __forceinline__ double slot_logU(const uint32_t *__restrict__ words, unsigned s) {
     const double U = mt_double(words[2 * (size_t)s], words[2 * (size_t)s + 1]);
     return (U == 0.0) ? LOGU_ZERO : log(U);
 }
 
-__global__ void __launch_bounds__(256) k_slots_build2(const uint32_t *__restrict__ words, long long nslots, uint32_t mask,
-                                                      SlotRec2 *__restrict__ rec) {
+// Slot records, state independent: the replica indices of slot s, its back-mask over the 31 slots before it, and (SlotRec) the
+// f64 log-uniform of the slot itself or (SlotRec2) the f32 log-uniform of the next slot, the draw of an attempt at s.
+template <bool REC2>
+__global__ void __launch_bounds__(256) k_slots_build(const uint32_t *__restrict__ words, long long nslots, uint32_t mask,
+                                                     std::conditional_t<REC2, SlotRec2, SlotRec> *__restrict__ rec) {
     __shared__ uint32_t s_ij[256 + 31];
     const long long s0 = (long long)blockIdx.x * 256;
     const int t = threadIdx.x;
@@ -55,18 +58,26 @@ __global__ void __launch_bounds__(256) k_slots_build2(const uint32_t *__restrict
         const bool hit = (o != 0xffffffffu) && (oi == i || oi == j || oj == i || oj == j);
         bm |= (hit ? 1u : 0u) << (31 - b);
     }
-    SlotRec2 r;
-    r.ij = ij;
-    r.backmask = bm;
-    float lu = 0.f;
-    if (s + 1 < nslots) lu = (float)slot_logU(words, (unsigned)(s + 1));
-    r.lu_next = __float_as_uint(lu);
-    r.k = 0;
-    rec[s] = r;
+    if constexpr (REC2) {
+        SlotRec2 r;
+        r.ij = ij;
+        r.backmask = bm;
+        float lu = 0.f;
+        if (s + 1 < nslots) lu = (float)slot_logU(words, (unsigned)(s + 1));
+        r.lu_next = __float_as_uint(lu);
+        r.k = 0;
+        rec[s] = r;
+    } else {
+        SlotRec r;
+        r.ij = ij;
+        r.backmask = bm;
+        r.logU = slot_logU(words, (unsigned)s);
+        rec[s] = r;
+    }
 }
 
 // The filter's decision for one (i, j, si, sj): image values d_x = image of u[x, s_x] - rowmin_x (the maintained diagonal)
-// and f_xy = image of u[x, s_y] - rowmin_x.  Same rigorous bound as k_mix_walk_pow2<U_FILTER24> (see its derivation there;
+// and f_xy = image of u[x, s_y] - rowmin_x.  Same rigorous bound as k_mix_walk_pow2<true> (see its derivation there;
 // the factor 3.2e-5 leaves 5 % over the 2^-15 + 2^-23 the roundings need, far more than the re-association below costs):
 //   e0  = 3.2e-5 (|d_i| + |d_j|) + eps0        as soon as the states are known (before the image loads return),
 //   eps = 3.2e-5 (|f_ij| + |f_ji|) + e0,       lp = (d_i - f_ij) + (d_j - f_ji),
@@ -515,22 +526,4 @@ __global__ void __launch_bounds__(W2_THREADS) k_mix_walk2c(const SlotRec2 *__res
                                                    const double *__restrict__ filt_rowabs, MixCtl *ctl) {
     const unsigned ncand = *ncand_p;   // records exist for c < ncand - 3
     w2_walk<true>(rec, words, cpos, ncand >= 3u ? ncand - 3u : 0u, u, K, 0, perm_g, slot_log, filt, filt_rowabs, ctl);
-}
-
-// Count matrices from the sparse commit log of the filter walkers (one word per record, bit 31 = an attempt started there).
-__global__ void k_mix_count_slots(const uint32_t *__restrict__ slot_log, long long s0, long long s1, int M,
-                                  unsigned long long *__restrict__ nacc, unsigned long long *__restrict__ nprop) {
-    long long t = s0 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    const long long stride = (long long)gridDim.x * blockDim.x;
-    for (; t < s1; t += stride) {
-        const uint32_t e = slot_log[t];
-        if (!(e >> 31)) continue;
-        const uint32_t si = e & ((1u << LOG_STATE_BITS) - 1u), sj = (e >> LOG_STATE_BITS) & ((1u << LOG_STATE_BITS) - 1u);
-        atomicAdd(&nprop[(size_t)si * M + sj], 1ull);
-        atomicAdd(&nprop[(size_t)sj * M + si], 1ull);
-        if ((e >> LOG_ACC_BIT) & 1u) {
-            atomicAdd(&nacc[(size_t)si * M + sj], 1ull);
-            atomicAdd(&nacc[(size_t)sj * M + si], 1ull);
-        }
-    }
 }

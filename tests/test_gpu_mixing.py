@@ -92,8 +92,8 @@ def test_swap_all_full_size_vs_oracle(K, model, seed):
 @pytest.mark.parametrize('path', ['default', 'serial', 'words'])
 def test_swap_all_any_k_vs_oracle(monkeypatch, K, model, nswap, seed, path):
     """K that is not a power of two.  default: the walk2 organisation in candidate coordinates (k_mix_walk2c, K <= 256) or the
-    walker over word positions (k_mix_walk_any: above 256, or everywhere with RX_WALK_ANY_V1=1 -- the f64 matrix in shared
-    memory up to K ~ 150, from L2 above); with RX_WALK_SERIAL=1 the plain loop; three iterations each."""
+    walker over word positions (k_mix_walk_any: above 256, or everywhere with RX_WALK_ANY_V1=1 -- exact f64 values from
+    L2); with RX_WALK_SERIAL=1 the plain loop; three iterations each."""
     from oracle import oracle
     serial = path == 'serial'
     if serial:
@@ -289,11 +289,11 @@ def test_swap_all_with_nonfinite_and_huge_energies(K):
         e.close()
 
 
-@pytest.mark.parametrize('env,K,model', [('RX_F64_SMEM', 16, 'flat'), ('RX_F64_SMEM', 64, 'normal'), ('RX_F64_SMEM', 128, 'flat'),
+@pytest.mark.parametrize('env,K,model', [('RX_NO_FILTER', 16, 'flat'), ('RX_NO_FILTER', 64, 'normal'), ('RX_NO_FILTER', 128, 'flat'),
                                          ('RX_NO_FILTER', 64, 'flat'), ('RX_NO_FILTER', 256, 'flat')])
 def test_swap_all_other_energy_placements_vs_oracle(monkeypatch, env, K, model):
-    """The walker variants the default selection no longer reaches: the f64 matrix in shared memory (RX_F64_SMEM /
-    RX_NO_FILTER at K <= 128) and the exact values from L2 every round (RX_NO_FILTER at K = 256)."""
+    """The exact walker over slots at K <= 256, which the default selection does not reach there (it runs the row-image
+    filter): RX_NO_FILTER=1 selects k_mix_walk_pow2<false>, the exact f64 values from L2 every round."""
     from oracle import oracle
     monkeypatch.setenv(env, '1')
     u = energies(model, K, 977 + K)

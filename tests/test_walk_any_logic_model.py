@@ -1,4 +1,4 @@
-"""Lane-level CPU model of k_mix_walk_any's control logic (openmmtools_b200/csrc/rx_walk_any.cuh): per-word-position
+"""Lane-level CPU model of k_mix_walk_any's control logic (openmmtools_b200/csrc/rx_walk_exact.cuh): per-word-position
 records (rejection-sampled indices, length, back-mask), the window of 32 word positions, the hop chain by pointer
 jumping over the lanes (four doublings), staleness, prefix commit, the budget tail and the hand-over to
 the plain loop.  The model must reproduce the sequential reference loop (replicaexchange.py:321-349 with numba's

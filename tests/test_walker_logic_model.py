@@ -1,4 +1,4 @@
-"""A CPU model of the speculative walker's ROUND LOGIC (openmmtools_b200/csrc/rx_mix.cu, k_mix_walk_pow2), checked against
+"""A CPU model of the speculative walker's ROUND LOGIC (openmmtools_b200/csrc/rx_walk_exact.cuh, k_mix_walk_pow2), checked against
 the golden vectors of the real reference loop.  It restates, with Python integers, exactly the bit arithmetic of the
 kernel -- slot records with the back-mask in bit order 31-b, the add-carry resolution of the visited chain, staleness
 from `shl(VA, 32 - lane) & backmask`, the committed prefix and the advance -- so that a change of that logic can be

@@ -1,5 +1,5 @@
 """One swap-all call (for ncu captures of the walkers): the K=256 LJ energy matrix, or with K given, a K x K sub-matrix of it
-(any K <= 256: k_mix_walk_any for K not a power of two).  usage: mix_once.py [nswap [K]]"""
+(any K <= 256: k_mix_walk2c for K not a power of two).  usage: mix_once.py [nswap [K]]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

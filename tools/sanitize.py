@@ -7,7 +7,7 @@ from energy_models import energies
 from openmmtools_b200 import testsystems, alchemy, states, mcmc, multistate, unit
 from openmmtools_b200._engine import Engine
 
-# mixing kernels: pow2 small, K=256 (row image, k_mix_walk2 + tail), K not a power of two (k_cand_* + k_mix_walk2c + plain tail;
+# mixing kernels: pow2 small, K=256 (row image, k_mix_walk2 + k_mix_walk_pow2<true> tail), K not a power of two (k_cand_* + k_mix_walk2c + plain tail;
 # above 256 k_words_build + k_mix_walk_any), neighbours
 for K, n in ((16, 4096), (256, 60000), (12, 1728), (100, 30000), (255, 20000), (300, 20000)):
     e = Engine(0, K, K)
