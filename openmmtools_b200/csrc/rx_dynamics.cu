@@ -55,28 +55,33 @@ __device__ __forceinline__ float fast_rcp(float x) { float y; asm("rcp.approx.ft
 __device__ __forceinline__ float fast_rsqrt(float x) { float y; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 // ---------------------------------------------------------------------------------------------------
+// A Langevin splitting move: the launch's (DynParams::move), or one entry per thermodynamic state when the states carry
+// different moves (multistatesampler.py:906-910: one MCMCMove per state; a replica is propagated with the move of the
+// state it is in).  Built by make_move only.
+struct MoveDev {
+    float dt, a, b;             // timestep, O-step coefficients exp(-gamma h), sqrt(1-exp(-2 gamma h))
+    int n_steps, n_prog, nV, nR, reassign;
+    char prog[RX_MAX_PROGRAM];
+    double dt_d, a_d, b_d;      // the same in f64 (the molecule kernel)
+};
+
+// A periodic box in float: the edges and their inverses.
+struct BoxF { float Lx, Ly, Lz, iLx, iLy, iLz; };
+__host__ __device__ __forceinline__ BoxF box_f(double X, double Y, double Z) {
+    return {(float)X, (float)Y, (float)Z, (float)(1.0 / X), (float)(1.0 / Y), (float)(1.0 / Z)};
+}
+
 struct DynParams {
     int N, kind;
-    float Lx, Ly, Lz, iLx, iLy, iLz;
+    BoxF box;                   // (NPT: each replica has its own, box[r])
     float rc2, rs2, rs, inv_w;  // cutoff^2, switch^2, switch, 1/(rc-rs)
     int use_switch, annihilate, c_is_6;
     float sc_c;                 // softcore_c
-    float dt, a, b;             // timestep, O-step coefficients exp(-gamma h), sqrt(1-exp(-2 gamma h))
-    double dt_d, a_d, b_d;      // the same in f64 (the molecule kernel)
-    int n_steps, n_prog, nV, nR, nO;
     int maxnb;                  // Verlet-list capacity per atom (0: all-pairs only)
     int sort_atoms;             // re-deal atoms to threads by neighbour count at every list build
     float rl2, rin2;            // (cutoff + skin_out)^2, (cutoff + skin_in)^2
     float half_in2, half_out2;  // (skin_in/2)^2, ((skin_out - skin_in)/2)^2
-    char prog[RX_MAX_PROGRAM];
-};
-
-// One entry per thermodynamic state when the states carry different moves (multistatesampler.py:906-910: one MCMCMove per
-// state); a replica is propagated with the move of the state it is in.
-struct MoveDev {
-    float dt, a, b;
-    int n_steps, n_prog, nV, nR, nO, reassign;
-    char prog[RX_MAX_PROGRAM];
+    MoveDev move;
 };
 
 struct PairLam { float la, ob; };
@@ -153,10 +158,20 @@ __device__ __forceinline__ float min_image_f(float d, float L, float iL) {
     const float n = __fadd_rn(__fmaf_rn(d, iL, 12582912.0f), -12582912.0f);
     return __fmaf_rn(-L, n, d);
 }
+// The minimum image of the displacement (dx, dy, dz), in place; returns its square.
+__device__ __forceinline__ float image_r2(const BoxF &b, float &dx, float &dy, float &dz) {
+    dx = min_image_f(dx, b.Lx, b.iLx); dy = min_image_f(dy, b.Ly, b.iLy); dz = min_image_f(dz, b.Lz, b.iLz);
+    return dx * dx + dy * dy + dz * dz;
+}
+// Wrap a position into the box (getState(enforcePeriodicBox=True), mcmc.py:731).
+__device__ __forceinline__ void wrap_into(const BoxF &b, float &x, float &y, float &z) {
+    x -= b.Lx * floorf(x * b.iLx); y -= b.Ly * floorf(y * b.iLy); z -= b.Lz * floorf(z * b.iLz);
+}
 
-// Everything the pair loop needs that does not change inside a launch, gathered in registers once.
+// What the pair loop needs about atom i and its surroundings, gathered in registers before the loop.
 struct PairCtx {
-    float Lx, Ly, Lz, iLx, iLy, iLz, rc2;
+    BoxF box;
+    float rc2;
     float x, y, z, sig_i, se_i;
     bool alch_i;
     PairLam lam;
@@ -169,9 +184,8 @@ __device__ __forceinline__ void pair_term(const DynParams &p, const PairCtx &c, 
                                           float &ax, float &ay, float &az, float &en) {
     const unsigned aj = pos_base + 16u * j;
     const float4 pj = lds_f4(aj);
-    const float dx = min_image_f(c.x - pj.x, c.Lx, c.iLx), dy = min_image_f(c.y - pj.y, c.Ly, c.iLy),
-                dz = min_image_f(c.z - pj.z, c.Lz, c.iLz);
-    const float r2 = dx * dx + dy * dy + dz * dz;
+    float dx = c.x - pj.x, dy = c.y - pj.y, dz = c.z - pj.z;
+    const float r2 = image_r2(c.box, dx, dy, dz);
     if (r2 < c.rc2) {
         const float2 qj = lds_f2(P8 ? (unsigned)par_off + 8u * j : aj + (unsigned)par_off);
         const bool alch_j = qj.y != 0.f;
@@ -227,7 +241,7 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
 // barrier becomes a cluster barrier.  The displacement votes are cluster wide, so the lists are rebuilt at the same steps and
 // with the same contents as in one block: trajectories do not depend on CL (each atom sums its own list in list order, noise
 // is keyed by atom id).
-// PS: per-state moves (the integrator parameters come from `moves[state]` instead of `p`).
+// PS: per-state moves (the move comes from `moves[state]` instead of `p.move`).
 // COMPACT: the layout above 1024 atoms (DESIGN 4.2): position buffers strided by N instead of RX_MAX_ATOMS and 8-byte
 // parameter records (sqrt_eps, alch) -- sigma rides in the position's w -- so that 4096 atoms leave room for a list.
 // NPT: the box is the replica's (box[r], kept in f64 there) and a Monte Carlo barostat attempt opens every 25th step
@@ -236,7 +250,7 @@ template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false, bool 
 __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *__restrict__ atom,
                                                     const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                     float4 *__restrict__ pos, float4 *__restrict__ vel, int k0,
-                                                    uint2 key, uint32_t iteration, int reassign,
+                                                    uint2 key, uint32_t iteration,
                                                     double *__restrict__ pot, double *__restrict__ kin,
                                                     int *__restrict__ nan_flag, const int *__restrict__ only,
                                                     const MoveDev *__restrict__ moves, double4 *__restrict__ box,
@@ -277,9 +291,9 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     };
     const StateDev st = states[perm[k]];
     const PairLam lam = {(float)st.la, (float)st.ob};
-    // NPT: the replica's box (f64, and the float edges and inverses the kernel uses instead of p's) and barostat state
+    // the box the kernel computes in; NPT: the replica's (also kept in f64) and its barostat state
+    BoxF bf = p.box;
     double bx = 0.0, by = 0.0, bz = 0.0;
-    float fLx = 0.f, fLy = 0.f, fLz = 0.f, fiLx = 0.f, fiLy = 0.f, fiLz = 0.f;
     rx_barostat_state bs = {};
     double2 nst = {};
     if constexpr (NPT) {
@@ -287,17 +301,14 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         bx = b4.x; by = b4.y; bz = b4.z;
         bs = baro[r];
         nst = npt[perm[k]];
-        fLx = (float)bx; fLy = (float)by; fLz = (float)bz;
-        fiLx = (float)(1.0 / bx); fiLy = (float)(1.0 / by); fiLz = (float)(1.0 / bz);
+        bf = box_f(bx, by, bz);
     }
     // the move: the launch's, or the one of this replica's state
-    const MoveDev *mv = PS ? moves + perm[k] : nullptr;
-    const float m_dt = PS ? mv->dt : p.dt, m_a = PS ? mv->a : p.a, m_b = PS ? mv->b : p.b;
-    const int m_steps = PS ? mv->n_steps : p.n_steps, m_nprog = PS ? mv->n_prog : p.n_prog, m_nV = PS ? mv->nV : p.nV,
-              m_nR = PS ? mv->nR : p.nR;
+    const MoveDev &mv = PS ? moves[perm[k]] : p.move;
+    const float m_a = mv.a, m_b = mv.b;   // (read once: the loop reads them under branches)
+    const int m_steps = mv.n_steps, m_nprog = mv.n_prog;
     // (the program is interpreted: the compiler does not hoist these divisions out of the step loop; same values, same bits)
-    const float h_V = m_dt / (float)m_nV, h_R = m_dt / (float)m_nR;
-    if (PS) reassign = mv->reassign;
+    const float h_V = mv.dt / (float)mv.nV, h_R = mv.dt / (float)mv.nR;
     float sig_i, se_i, inv_m, sigma_v;
     bool alch_i;
     auto load_atom = [&]() {
@@ -309,7 +320,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     float4 x4 = active ? pos[(size_t)r * p.N + a] : make_float4(0, 0, 0, 0);
     float4 v4 = active ? vel[(size_t)r * p.N + a] : make_float4(0, 0, 0, 0);
     float x = x4.x, y = x4.y, z = x4.z, vx = v4.x, vy = v4.y, vz = v4.z;
-    if (reassign && active) {  // context.setVelocitiesToTemperature, mcmc.py:711
+    if (mv.reassign && active) {  // context.setVelocitiesToTemperature, mcmc.py:711
         const float3 g = philox_normal3(philox4x32_10(make_uint4(a, 0x80000000u, k, iteration), key));
         vx = sigma_v * g.x; vy = sigma_v * g.y; vz = sigma_v * g.z;
     }
@@ -379,17 +390,8 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
                 const unsigned ql = nb_t + (unsigned)lo * stride;
                 const unsigned e = lds_u16(ql);
                 const float4 pj = s_pos[e];
-                float d2;
-                if constexpr (NPT) {
-                    const float dx = min_image_f(x - pj.x, fLx, fiLx), dy = min_image_f(y - pj.y, fLy, fiLy),
-                                dz = min_image_f(z - pj.z, fLz, fiLz);
-                    d2 = dx * dx + dy * dy + dz * dz;
-                } else {
-                    const float dx = min_image_f(x - pj.x, p.Lx, p.iLx), dy = min_image_f(y - pj.y, p.Ly, p.iLy),
-                                dz = min_image_f(z - pj.z, p.Lz, p.iLz);
-                    d2 = dx * dx + dy * dy + dz * dz;
-                }
-                if (d2 < p.rin2) lo++;
+                float dx = x - pj.x, dy = y - pj.y, dz = z - pj.z;
+                if (image_r2(bf, dx, dy, dz) < p.rin2) lo++;
                 else {
                     const unsigned qh = nb_t + (unsigned)hi * stride;
                     sts_u16(ql, lds_u16(qh));
@@ -407,17 +409,8 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         if (active) {
             for (int j = 0; j < p.N; j++) {
                 const float4 pj = s_pos[j];
-                float r2;
-                if constexpr (NPT) {
-                    const float dx = min_image_f(x - pj.x, fLx, fiLx), dy = min_image_f(y - pj.y, fLy, fiLy),
-                                dz = min_image_f(z - pj.z, fLz, fiLz);
-                    r2 = dx * dx + dy * dy + dz * dz;
-                } else {
-                    const float dx = min_image_f(x - pj.x, p.Lx, p.iLx), dy = min_image_f(y - pj.y, p.Ly, p.iLy),
-                                dz = min_image_f(z - pj.z, p.Lz, p.iLz);
-                    r2 = dx * dx + dy * dy + dz * dz;
-                }
-                if (r2 < p.rl2 && j != a) {
+                float dx = x - pj.x, dy = y - pj.y, dz = z - pj.z;
+                if (image_r2(bf, dx, dy, dz) < p.rl2 && j != a) {
                     if (cnt < p.maxnb) s_nb[cnt * nthr + t] = (unsigned short)j;
                     cnt++;
                 }
@@ -448,10 +441,10 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         }
     };
 
+    // The pair loop's context holds a second copy of bf, which the barostat refreshes with it: with bf alone (however it
+    // reaches the pair loop) most NPT instantiations spill more (DESIGN 4.2).
     PairCtx pc;
-    pc.Lx = p.Lx; pc.Ly = p.Ly; pc.Lz = p.Lz; pc.iLx = p.iLx; pc.iLy = p.iLy; pc.iLz = p.iLz; pc.rc2 = p.rc2;
-    if constexpr (NPT) { pc.Lx = fLx; pc.Ly = fLy; pc.Lz = fLz; pc.iLx = fiLx; pc.iLy = fiLy; pc.iLz = fiLz; }
-    pc.lam = lam;
+    pc.box = bf; pc.rc2 = p.rc2; pc.lam = lam;
     const int N = p.N;
     // Publish the current positions and make the neighbour list valid for them: one barrier unless a list is rebuilt.
     auto publish = [&]() {
@@ -514,11 +507,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
                 cluster_sync();   // every block has read the sums before they are cleared again
                 return total;
             };
-            auto set_box = [&](double X, double Y, double Z) {
-                fLx = (float)X; fLy = (float)Y; fLz = (float)Z;
-                fiLx = (float)(1.0 / X); fiLy = (float)(1.0 / Y); fiLz = (float)(1.0 / Z);
-                pc.Lx = fLx; pc.Ly = fLy; pc.Lz = fLz; pc.iLx = fiLx; pc.iLy = fiLy; pc.iLz = fiLz;
-            };
+            auto set_box = [&](double X, double Y, double Z) { bf = box_f(X, Y, Z); pc.box = bf; };
             float e0;
             compute_forces(true, e0);   // (forces already valid come out the same bits: same list, same order)
             f_valid = true;
@@ -570,7 +559,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     for (int s = 0; s < m_steps; s++) {
         if constexpr (NPT) { if (++bs.step >= 25) { bs.step = 0; barostat(); } }
         for (int q = 0; q < m_nprog; q++) {
-            const char op = PS ? mv->prog[q] : p.prog[q];
+            const char op = mv.prog[q];
             if (op == 'V') {
                 if (!f_valid) { compute_forces(false, dummy); f_valid = true; }
                 const float h = h_V;
@@ -625,10 +614,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         nan_flag[k] = (any_bad || !isfinite(U)) ? 1 : 0;
     }
     if (active) {
-        if (lj) {  // getState(enforcePeriodicBox=True), mcmc.py:731
-            if constexpr (NPT) { x -= fLx * floorf(x * fiLx); y -= fLy * floorf(y * fiLy); z -= fLz * floorf(z * fiLz); }
-            else { x -= p.Lx * floorf(x * p.iLx); y -= p.Ly * floorf(y * p.iLy); z -= p.Lz * floorf(z * p.iLz); }
-        }
+        if (lj) wrap_into(bf, x, y, z);
         pos[(size_t)r * p.N + a] = make_float4(x, y, z, 0.f);
         vel[(size_t)r * p.N + a] = make_float4(vx, vy, vz, 0.f);
     }
@@ -863,25 +849,31 @@ static int smem_opt_in(rx_engine *h, const void *kern, int dyn) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-static int fill_dyn(rx_engine *h, DynParams &p) {
+// The move of a splitting program (V, R, O substeps) run n_steps times with timestep dt and friction gamma.
+static MoveDev make_move(double dt, double gamma, int n_steps, const char *program, int reassign) {
+    MoveDev d;
+    memset(&d, 0, sizeof(d));
+    int n = 0, nV = 0, nR = 0, nO = 0;
+    for (const char *q = program; *q; q++, n++) { if (*q == 'V') nV++; else if (*q == 'R') nR++; else nO++; d.prog[n] = *q; }
+    d.n_prog = n; d.nV = nV; d.nR = nR;
+    d.dt = (float)dt; d.n_steps = n_steps; d.reassign = reassign;
+    const double hO = dt / (nO > 0 ? nO : 1);   // integrators.py:1141-1146
+    d.dt_d = dt; d.a_d = exp(-gamma * hO); d.b_d = sqrt(1.0 - exp(-2.0 * gamma * hO));
+    d.a = (float)d.a_d; d.b = (float)d.b_d;
+    return d;
+}
+
+static int fill_dyn(rx_engine *h, DynParams &p, int reassign) {
     const rx_config &c = h->cfg;
     memset(&p, 0, sizeof(p));
     p.N = c.n_atoms; p.kind = c.system_kind;
-    p.Lx = (float)c.box[0]; p.Ly = (float)c.box[1]; p.Lz = (float)c.box[2];
-    p.iLx = (float)(1.0 / c.box[0]); p.iLy = (float)(1.0 / c.box[1]); p.iLz = (float)(1.0 / c.box[2]);
+    p.box = box_f(c.box[0], c.box[1], c.box[2]);
     p.rc2 = (float)(c.r_cutoff * c.r_cutoff); p.rs2 = (float)(c.r_switch * c.r_switch); p.rs = (float)c.r_switch;
     p.inv_w = (float)(1.0 / (c.r_cutoff - c.r_switch));
     p.use_switch = c.use_switch; p.annihilate = c.annihilate_sterics;
     p.c_is_6 = (c.softcore_c == 6.0); p.sc_c = (float)c.softcore_c;
-    p.dt = (float)h->dt; p.n_steps = h->n_steps;
-    int nV = 0, nR = 0, nO = 0, n = 0;
-    for (const char *q = h->program; *q; q++, n++) { if (*q == 'V') nV++; else if (*q == 'R') nR++; else nO++; p.prog[n] = *q; }
-    p.n_prog = n; p.nV = nV; p.nR = nR; p.nO = nO;
     p.maxnb = 0; p.sort_atoms = 0; p.rl2 = p.rin2 = p.rc2; p.half_in2 = p.half_out2 = 0.f;
-    const double hO = h->dt / (nO > 0 ? nO : 1);   // integrators.py:1141-1146
-    p.a = (float)exp(-h->gamma * hO);
-    p.b = (float)sqrt(1.0 - exp(-2.0 * h->gamma * hO));
-    p.dt_d = h->dt; p.a_d = exp(-h->gamma * hO); p.b_d = sqrt(1.0 - exp(-2.0 * h->gamma * hO));
+    p.move = make_move(h->dt, h->gamma, h->n_steps, h->program, reassign);
     return RX_OK;
 }
 
@@ -892,15 +884,7 @@ int rxi_upload_state_moves(rx_engine *h) {
     std::vector<MoveDev> tab((size_t)M);
     for (int l = 0; l < M; l++) {
         const rx_state_move &m = h->state_moves[(size_t)l];
-        MoveDev &d = tab[(size_t)l];
-        memset(&d, 0, sizeof(d));
-        int n = 0, nV = 0, nR = 0, nO = 0;
-        for (const char *q = m.program; *q; q++, n++) { if (*q == 'V') nV++; else if (*q == 'R') nR++; else nO++; d.prog[n] = *q; }
-        d.n_prog = n; d.nV = nV; d.nR = nR; d.nO = nO;
-        d.dt = (float)m.dt; d.n_steps = m.n_steps; d.reassign = m.reassign;
-        const double hO = m.dt / (nO > 0 ? nO : 1);   // integrators.py:1141-1146
-        d.a = (float)exp(-m.gamma * hO);
-        d.b = (float)sqrt(1.0 - exp(-2.0 * m.gamma * hO));
+        tab[(size_t)l] = make_move(m.dt, m.gamma, m.n_steps, m.program, m.reassign);
     }
     if (!h->d_moves) RX_CHECK_CUDA(h, cudaMalloc(&h->d_moves, sizeof(MoveDev) * (size_t)M));
     RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_moves, tab.data(), sizeof(MoveDev) * (size_t)M, cudaMemcpyHostToDevice, h->stream));
@@ -1018,10 +1002,48 @@ int rxi_plan_propagate(const rx_propagate_query *q, rx_propagate_plan *o, std::s
     return RX_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Launch tables: runtime choices to template arguments, over the instantiations that exist and no others.
+// ---------------------------------------------------------------------------------------------------
+// f(std::true_type) or f(std::false_type): a runtime flag as a template argument.
+template <typename F> static auto with_flag(bool b, F &&f) { return b ? f(std::true_type{}) : f(std::false_type{}); }
+
+// Launch one instantiation; opt_in: first allow it lc.dynamicSmemBytes of dynamic shared memory (above the 48 KB default).
+template <typename... P, typename... A>
+static int launch_kernel(rx_engine *h, const cudaLaunchConfig_t &lc, bool opt_in, void (*kern)(P...), A... args) {
+    if (opt_in)
+        RX_CHECK_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lc.dynamicSmemBytes));
+    RX_CHECK_CUDA(h, cudaLaunchKernelEx(&lc, kern, args...));
+    return RX_OK;
+}
+
+// The (CL, PS, COMPACT) layouts of k_propagate, one for each kind of plan rxi_plan_propagate makes: up to 1024 atoms one
+// block per replica, split over 2 or 4 when the replicas would leave SMs idle (or RX_CLUSTER asks), per-state moves
+// always unsplit; above 1024 atoms the compact layout over 2, 4 or 8 blocks, with or without per-state moves.
+template <int CL_, bool PS_, bool COMPACT_> struct Layout {
+    static constexpr int cl = CL_;
+    static constexpr bool ps = PS_, compact = COMPACT_;
+};
+template <typename... L> struct LayoutList {};
+using PropagateLayouts = LayoutList<
+    Layout<1, false, false>, Layout<2, false, false>, Layout<4, false, false>,  // <= 1024 atoms; 2 or 4: few replicas
+    Layout<1, true, false>,                                                      // <= 1024 atoms, per-state moves
+    Layout<2, false, true>, Layout<4, false, true>, Layout<8, false, true>,      // > 1024 atoms
+    Layout<2, true, true>, Layout<4, true, true>, Layout<8, true, true>>;        // > 1024 atoms, per-state moves
+
+// f(Layout<...>) for the layout of the plan; false when no instantiation has it.
+template <typename F, int... CL, bool... PS, bool... CP>
+static bool with_layout(LayoutList<Layout<CL, PS, CP>...>, const rx_propagate_plan &plan, bool per_state, int &rc, F &&f) {
+    bool found = false;
+    ((!found && plan.cluster == CL && per_state == PS && (plan.compact != 0) == CP ? (found = true, rc = f(Layout<CL, PS, CP>{}))
+                                                                                  : 0), ...);
+    return found;
+}
+
 int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign, int *launches, const int *d_only) {
     if (h->kloc == 0) return RX_OK;
     DynParams p;
-    fill_dyn(h, p);
+    fill_dyn(h, p, reassign);
     const int N = h->cfg.n_atoms;
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
         if (!h->state_moves.empty()) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_propagate: per-state moves are not provided for molecules");
@@ -1035,7 +1057,7 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         const int dyn = md->dyn_shared_bytes + (gb ? gb->prop_bytes : 0);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
-        kern<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
+        kern<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p.move, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
                                                             (double *)h->d_vel, h->k0, mkey, (uint32_t)iteration, reassign, h->d_pot,
                                                             h->d_kin, h->d_nan, d_only, gb ? *gb : MolGB{});
         RX_CHECK_CUDA(h, cudaGetLastError());
@@ -1085,38 +1107,21 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
     const uint32_t it32 = (uint32_t)iteration;
     const double min_edge = 2.0 * h->cfg.r_cutoff;
     const bool npt = h->npt;
-#define RX_LAUNCH_PROPAGATE_NPT(C6, SW, CL, PS, CP, NP)                                                                   \
-    do {                                                                                                                   \
-        if (smem > 48 * 1024)                                                                                              \
-            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_propagate<C6, SW, CL, PS, CP, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        RX_CHECK_CUDA(h, cudaLaunchKernelEx(&lc, k_propagate<C6, SW, CL, PS, CP, NP>, p, (const float4 *)h->d_atom, (const StateDev *)h->d_states, \
-                                            (const int *)h->d_perm, h->d_pos, h->d_vel, h->k0, key, it32, reassign, h->d_pot, \
-                                            h->d_kin, h->d_nan, d_only, (const MoveDev *)h->d_moves, h->d_box, h->d_baro,  \
-                                            (const double2 *)h->d_npt, min_edge));                                         \
-    } while (0)
-#define RX_LAUNCH_PROPAGATE(C6, SW, CL, PS, CP)                                                                           \
-    do {                                                                                                                   \
-        if (npt) RX_LAUNCH_PROPAGATE_NPT(C6, SW, CL, PS, CP, true); else RX_LAUNCH_PROPAGATE_NPT(C6, SW, CL, PS, CP, false); \
-    } while (0)
-// above 1024 atoms: the compact layout over 2, 4 or 8 blocks, per-state moves or not
-#define RX_LAUNCH_PROPAGATE_COMPACT(C6, SW, PS)                                                                           \
-    do {                                                                                                                   \
-        if (cl == 8) RX_LAUNCH_PROPAGATE(C6, SW, 8, PS, true); else if (cl == 4) RX_LAUNCH_PROPAGATE(C6, SW, 4, PS, true); \
-        else RX_LAUNCH_PROPAGATE(C6, SW, 2, PS, true);                                                                     \
-    } while (0)
-#define RX_LAUNCH_PROPAGATE_CL(C6, SW)                                                                                    \
-    do {                                                                                                                   \
-        if (plan.compact) { if (per_state) RX_LAUNCH_PROPAGATE_COMPACT(C6, SW, true); else RX_LAUNCH_PROPAGATE_COMPACT(C6, SW, false); } \
-        else if (per_state) RX_LAUNCH_PROPAGATE(C6, SW, 1, true, false);                                                   \
-        else if (cl == 4) RX_LAUNCH_PROPAGATE(C6, SW, 4, false, false); else if (cl == 2) RX_LAUNCH_PROPAGATE(C6, SW, 2, false, false); \
-        else RX_LAUNCH_PROPAGATE(C6, SW, 1, false, false);                                                                 \
-    } while (0)
-    if (p.c_is_6) { if (p.use_switch) RX_LAUNCH_PROPAGATE_CL(true, true); else RX_LAUNCH_PROPAGATE_CL(true, false); }
-    else { if (p.use_switch) RX_LAUNCH_PROPAGATE_CL(false, true); else RX_LAUNCH_PROPAGATE_CL(false, false); }
-#undef RX_LAUNCH_PROPAGATE_COMPACT
-#undef RX_LAUNCH_PROPAGATE_CL
-#undef RX_LAUNCH_PROPAGATE
-#undef RX_LAUNCH_PROPAGATE_NPT
+    int rc = RX_OK;
+    const bool found = with_flag(p.c_is_6, [&](auto c6) {
+        return with_flag(p.use_switch, [&](auto sw) {
+            return with_flag(npt, [&](auto np) {
+                return with_layout(PropagateLayouts{}, plan, per_state, rc, [&](auto L) {
+                    return launch_kernel(h, lc, smem > 48 * 1024, k_propagate<c6, sw, L.cl, L.ps, L.compact, np>, p, (const float4 *)h->d_atom,
+                                         (const StateDev *)h->d_states, (const int *)h->d_perm, h->d_pos, h->d_vel, h->k0, key,
+                                         it32, h->d_pot, h->d_kin, h->d_nan, d_only, (const MoveDev *)h->d_moves, h->d_box,
+                                         h->d_baro, (const double2 *)h->d_npt, min_edge);
+                });
+            });
+        });
+    });
+    if (!found) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_propagate: no kernel for the launch plan");
+    if (rc) return rc;
     RX_CHECK_CUDA(h, cudaGetLastError());
     (*launches)++;
     return RX_OK;
@@ -1142,46 +1147,34 @@ int rxi_snapshot_state(rx_engine *h) {
     return RX_OK;
 }
 
-// NPT: the box and barostat state of the failed replicas go back to the snapshot as well.
-__global__ void k_restore_failed_npt(const int *__restrict__ nan_flag, int k0, int kloc, const double4 *__restrict__ box_snap,
-                                     const rx_barostat_state *__restrict__ baro_snap, double4 *__restrict__ box,
-                                     rx_barostat_state *__restrict__ baro) {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= kloc || !nan_flag[k0 + r]) return;
-    box[r] = box_snap[r];
-    baro[r] = baro_snap[r];
-}
-
-__global__ void k_restore_failed(const int *__restrict__ nan_flag, int *__restrict__ retry, int k0, int N,
-                                 const float4 *__restrict__ pos_snap, const float4 *__restrict__ vel_snap,
-                                 float4 *__restrict__ pos, float4 *__restrict__ vel) {
+// retry[k] = the NaN flag of replica k; a failed replica's rows of positions and velocities (`words` 8-byte words each)
+// and, under NPT (box != nullptr), its box and barostat state go back to the snapshot.
+__global__ void k_restore_failed(const int *__restrict__ nan_flag, int *__restrict__ retry, int k0, int words,
+                                 const unsigned long long *__restrict__ pos_snap, const unsigned long long *__restrict__ vel_snap,
+                                 unsigned long long *__restrict__ pos, unsigned long long *__restrict__ vel,
+                                 const double4 *__restrict__ box_snap, const rx_barostat_state *__restrict__ baro_snap,
+                                 double4 *__restrict__ box, rx_barostat_state *__restrict__ baro) {
     const int r = blockIdx.x, k = k0 + r;
     const int failed = nan_flag[k];
     if (threadIdx.x == 0) retry[k] = failed;
     if (!failed) return;
-    for (int t = threadIdx.x; t < N; t += blockDim.x) {
-        pos[(size_t)r * N + t] = pos_snap[(size_t)r * N + t];
-        vel[(size_t)r * N + t] = vel_snap[(size_t)r * N + t];
+    for (int q = threadIdx.x; q < words; q += blockDim.x) {
+        pos[(size_t)r * words + q] = pos_snap[(size_t)r * words + q];
+        vel[(size_t)r * words + q] = vel_snap[(size_t)r * words + q];
     }
+    if (box && threadIdx.x == 0) { box[r] = box_snap[r]; baro[r] = baro_snap[r]; }
 }
 
 int rxi_restore_failed(rx_engine *h) {
     if (h->kloc == 0) return RX_OK;
     if (!h->have_snapshot) RX_FAIL(h, RX_ERR_INVALID, "rx_propagate_retry: no start-of-iteration snapshot (call rx_propagate first)");
-    if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
-        k_restore_failed_mol<<<h->kloc, 32, 0, h->stream>>>(h->d_nan, h->d_retry, h->k0, h->cfg.n_atoms, (const double *)h->d_pos_snap,
-                                                           (const double *)h->d_vel_snap, (double *)h->d_pos, (double *)h->d_vel);
-        RX_CHECK_CUDA(h, cudaGetLastError());
-        return RX_OK;
-    }
-    k_restore_failed<<<h->kloc, 256, 0, h->stream>>>(h->d_nan, h->d_retry, h->k0, h->cfg.n_atoms, h->d_pos_snap, h->d_vel_snap,
-                                                    h->d_pos, h->d_vel);
+    // a molecule's rows are double[N][3], an LJ replica's float4[N]
+    const int words = (h->cfg.system_kind == RX_SYSTEM_MOLECULE ? 3 : 2) * h->cfg.n_atoms;
+    using W = unsigned long long;
+    k_restore_failed<<<h->kloc, 256, 0, h->stream>>>(h->d_nan, h->d_retry, h->k0, words, (const W *)h->d_pos_snap,
+                                                    (const W *)h->d_vel_snap, (W *)h->d_pos, (W *)h->d_vel, h->d_box_snap,
+                                                    h->d_baro_snap, h->npt ? h->d_box : nullptr, h->d_baro);
     RX_CHECK_CUDA(h, cudaGetLastError());
-    if (h->npt) {
-        k_restore_failed_npt<<<(h->kloc + 127) / 128, 128, 0, h->stream>>>(h->d_nan, h->k0, h->kloc, h->d_box_snap, h->d_baro_snap,
-                                                                          h->d_box, h->d_baro);
-        RX_CHECK_CUDA(h, cudaGetLastError());
-    }
     return RX_OK;
 }
 
@@ -1205,11 +1198,8 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
                                                    double *__restrict__ rms_out, int *__restrict__ iters_out,
                                                    const double4 *__restrict__ box) {
     extern __shared__ float4 s_dyn[];
-    if constexpr (NPT) {
-        const double4 b = box[blockIdx.x];
-        p.Lx = (float)b.x; p.Ly = (float)b.y; p.Lz = (float)b.z;
-        p.iLx = (float)(1.0 / b.x); p.iLy = (float)(1.0 / b.y); p.iLz = (float)(1.0 / b.z);
-    }
+    BoxF bf = p.box;
+    if constexpr (NPT) { const double4 b = box[blockIdx.x]; bf = box_f(b.x, b.y, b.z); }
     const int stride = APT == 1 ? RX_MAX_ATOMS : p.N;
     float4 *s_pos = s_dyn, *s_par = s_dyn + stride;
     __shared__ float s_part[32][3];
@@ -1229,7 +1219,7 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
     }
     __syncthreads();
     PairCtx pc;
-    pc.Lx = p.Lx; pc.Ly = p.Ly; pc.Lz = p.Lz; pc.iLx = p.iLx; pc.iLy = p.iLy; pc.iLz = p.iLz; pc.rc2 = p.rc2;
+    pc.box = bf; pc.rc2 = p.rc2;
     pc.lam = {(float)st.la, (float)st.ob};
     const unsigned pos_base = (unsigned)__cvta_generic_to_shared(s_dyn);
     const float hx0 = (float)st.ho_x0[0], hx1 = (float)st.ho_x0[1], hx2 = (float)st.ho_x0[2], hK = (float)st.ho_K;
@@ -1307,7 +1297,7 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
         if (a < p.N) {
             const float4 xa = s_pos[a];
             float x = xa.x, y = xa.y, z = xa.z;
-            if (p.kind != RX_SYSTEM_HARMONIC) { x -= p.Lx * floorf(x * p.iLx); y -= p.Ly * floorf(y * p.iLy); z -= p.Lz * floorf(z * p.iLz); }
+            if (p.kind != RX_SYSTEM_HARMONIC) wrap_into(bf, x, y, z);
             pos[(size_t)r * p.N + a] = make_float4(x, y, z, 0.f);
         }
     }
@@ -1328,7 +1318,7 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
         return RX_OK;
     }
     DynParams p;
-    fill_dyn(h, p);
+    fill_dyn(h, p, 0);
     const int N = h->cfg.n_atoms;
     if (h->cfg.system_kind == RX_SYSTEM_HARMONIC && N > RX_MAX_ATOMS)
         RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_minimize: more than 1024 atoms per replica of a harmonic system is not supported");
@@ -1338,23 +1328,23 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
     const bool wide = N > RX_MAX_ATOMS;
     const int threads = wide ? ((N + 4 * 32 - 1) / (4 * 32)) * 32 : ((N + 31) / 32) * 32;
     const size_t smem = (size_t)2 * (wide ? N : RX_MAX_ATOMS) * sizeof(float4);
-#define RX_LAUNCH_MINIMIZE_NPT(C6, SW, NP)                                                                                 \
-    do {                                                                                                                   \
-        if (wide) {                                                                                                        \
-            RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_minimize<C6, SW, 4, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            k_minimize<C6, SW, 4, NP><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
-                                                                             (float)tolerance, max_iterations, d_rms, d_iters, h->d_box); \
-        } else {                                                                                                           \
-            k_minimize<C6, SW, 1, NP><<<h->kloc, threads, smem, h->stream>>>(p, h->d_atom, h->d_states, h->d_perm, h->d_pos, h->k0, \
-                                                                             (float)tolerance, max_iterations, d_rms, d_iters, h->d_box); \
-        }                                                                                                                  \
-    } while (0)
-#define RX_LAUNCH_MINIMIZE(C6, SW)                                                                                         \
-    do { if (h->npt) RX_LAUNCH_MINIMIZE_NPT(C6, SW, true); else RX_LAUNCH_MINIMIZE_NPT(C6, SW, false); } while (0)
-    if (p.c_is_6) { if (p.use_switch) RX_LAUNCH_MINIMIZE(true, true); else RX_LAUNCH_MINIMIZE(true, false); }
-    else { if (p.use_switch) RX_LAUNCH_MINIMIZE(false, true); else RX_LAUNCH_MINIMIZE(false, false); }
-#undef RX_LAUNCH_MINIMIZE
-#undef RX_LAUNCH_MINIMIZE_NPT
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = dim3((unsigned)h->kloc);
+    lc.blockDim = dim3((unsigned)threads);
+    lc.dynamicSmemBytes = smem;
+    lc.stream = h->stream;
+    const int rc = with_flag(p.c_is_6, [&](auto c6) {
+        return with_flag(p.use_switch, [&](auto sw) {
+            return with_flag(h->npt, [&](auto np) {
+                return with_flag(wide, [&](auto w) {
+                    return launch_kernel(h, lc, wide, k_minimize<c6, sw, w ? 4 : 1, np>, p, (const float4 *)h->d_atom,
+                                         (const StateDev *)h->d_states, (const int *)h->d_perm, h->d_pos, h->k0,
+                                         (float)tolerance, max_iterations, d_rms, d_iters, (const double4 *)h->d_box);
+                });
+            });
+        });
+    });
+    if (rc) return rc;
     RX_CHECK_CUDA(h, cudaGetLastError());
     return RX_OK;
 }

@@ -166,19 +166,6 @@ __device__ __forceinline__ void mol_cross(const double *a, const double *b, doub
 }
 __device__ __forceinline__ double mol_dot(const double *a, const double *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
-template <typename R> __device__ __forceinline__ R mol_sqrt(R x);
-template <> __device__ __forceinline__ float mol_sqrt<float>(float x) { return sqrtf(x); }
-template <> __device__ __forceinline__ double mol_sqrt<double>(double x) { return sqrt(x); }
-template <typename R> __device__ __forceinline__ R mol_acos(R x);
-template <> __device__ __forceinline__ float mol_acos<float>(float x) { return acosf(x); }
-template <> __device__ __forceinline__ double mol_acos<double>(double x) { return acos(x); }
-template <typename R> __device__ __forceinline__ R mol_atan2(R y, R x);
-template <> __device__ __forceinline__ float mol_atan2<float>(float y, float x) { return atan2f(y, x); }
-template <> __device__ __forceinline__ double mol_atan2<double>(double y, double x) { return atan2(y, x); }
-template <typename R> __device__ __forceinline__ void mol_sincos(R x, R *s, R *c);
-template <> __device__ __forceinline__ void mol_sincos<float>(float x, float *s, float *c) { sincosf(x, s, c); }
-template <> __device__ __forceinline__ void mol_sincos<double>(double x, double *s, double *c) { sincos(x, s, c); }
-
 // The term tables of one molecule in shared memory (a few KB: read every step by every lane).
 struct MolShared {
     const MolBond *bonds; const MolAngle *angles; const MolTorsion *torsions; const MolExc *exc;
@@ -189,38 +176,37 @@ struct MolShared {
 };
 
 // Force on atom a (ENERGY: instead the energy of the terms this atom owns: bonds/exceptions/pairs with the larger partner
-// index, angles and torsions in which it has role 0).  X: positions of all atoms in shared memory.  R: the arithmetic type --
-// float for the forces of the dynamics (as in k_propagate: f32 forces on f64-stored positions, differences taken in f64),
-// double for energies.
-template <bool ENERGY, typename R>
+// index, angles and torsions in which it has role 0).  X: positions of all atoms in shared memory.  In f64 (the dynamics'
+// forces are mol_forces_terms).
+template <bool ENERGY>
 __device__ double mol_atom(const MolShared &m, const double (*X)[3], int a, double *f) {
     double e = 0.0;
-    R fx = 0, fy = 0, fz = 0;
+    double fx = 0, fy = 0, fz = 0;
     const double xa[3] = {X[a][0], X[a][1], X[a][2]};
     for (int q = m.b_off[a]; q < m.b_off[a + 1]; q++) {
         const MolBond b = m.bonds[q];
-        const R d[3] = {(R)(xa[0] - X[b.j][0]), (R)(xa[1] - X[b.j][1]), (R)(xa[2] - X[b.j][2])};
-        const R r = mol_sqrt<R>(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), dr = r - (R)b.r0;
-        if (ENERGY) { if (b.j > a) e += 0.5 * b.K * (double)dr * (double)dr; }
-        else { const R c = -(R)b.K * dr / r; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
+        const double d[3] = {xa[0] - X[b.j][0], xa[1] - X[b.j][1], xa[2] - X[b.j][2]};
+        const double r = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), dr = r - b.r0;
+        if (ENERGY) { if (b.j > a) e += 0.5 * b.K * dr * dr; }
+        else { const double c = -b.K * dr / r; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
     }
     for (int q = m.a_off[a]; q < m.a_off[a + 1]; q++) {
         const MolAngle g = m.angles[q];
-        R u[3], v[3];
-        for (int c = 0; c < 3; c++) { u[c] = (R)(X[g.i][c] - X[g.j][c]); v[c] = (R)(X[g.k][c] - X[g.j][c]); }
-        const R ru2 = u[0] * u[0] + u[1] * u[1] + u[2] * u[2], rv2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
-        const R iruv = (R)1 / mol_sqrt<R>(ru2 * rv2);
-        R cs = (u[0] * v[0] + u[1] * v[1] + u[2] * v[2]) * iruv;
-        cs = cs > (R)1 ? (R)1 : (cs < (R)-1 ? (R)-1 : cs);
-        const R dt = mol_acos<R>(cs) - (R)g.t0;
-        if (ENERGY) { if (g.role == 0) e += 0.5 * g.K * (double)dt * (double)dt; }
+        double u[3], v[3];
+        for (int c = 0; c < 3; c++) { u[c] = X[g.i][c] - X[g.j][c]; v[c] = X[g.k][c] - X[g.j][c]; }
+        const double ru2 = u[0] * u[0] + u[1] * u[1] + u[2] * u[2], rv2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
+        const double iruv = 1.0 / sqrt(ru2 * rv2);
+        double cs = (u[0] * v[0] + u[1] * v[1] + u[2] * v[2]) * iruv;
+        cs = cs > 1.0 ? 1.0 : (cs < -1.0 ? -1.0 : cs);
+        const double dt = acos(cs) - g.t0;
+        if (ENERGY) { if (g.role == 0) e += 0.5 * g.K * dt * dt; }
         else {
-            const R sn = mol_sqrt<R>((R)1 - cs * cs);
-            const R gg = (sn > (R)1e-6) ? (R)g.K * dt / sn : (R)0;
-            R o[3];
+            const double sn = sqrt(1.0 - cs * cs);
+            const double gg = (sn > 1e-6) ? g.K * dt / sn : 0.0;
+            double o[3];
             for (int c = 0; c < 3; c++) {
-                const R fi = gg * (v[c] * iruv - cs * u[c] / ru2);
-                const R fk = gg * (u[c] * iruv - cs * v[c] / rv2);
+                const double fi = gg * (v[c] * iruv - cs * u[c] / ru2);
+                const double fk = gg * (u[c] * iruv - cs * v[c] / rv2);
                 o[c] = g.role == 0 ? fi : (g.role == 2 ? fk : -(fi + fk));
             }
             fx += o[0]; fy += o[1]; fz += o[2];
@@ -228,52 +214,52 @@ __device__ double mol_atom(const MolShared &m, const double (*X)[3], int a, doub
     }
     for (int q = m.t_off[a]; q < m.t_off[a + 1]; q++) {
         const MolTorsion t = m.torsions[q];
-        R rij[3], rkj[3], rkl[3], mm[3], nn[3];
-        for (int c = 0; c < 3; c++) { rij[c] = (R)(X[t.i][c] - X[t.j][c]); rkj[c] = (R)(X[t.k][c] - X[t.j][c]); rkl[c] = (R)(X[t.k][c] - X[t.l][c]); }
+        double rij[3], rkj[3], rkl[3], mm[3], nn[3];
+        for (int c = 0; c < 3; c++) { rij[c] = X[t.i][c] - X[t.j][c]; rkj[c] = X[t.k][c] - X[t.j][c]; rkl[c] = X[t.k][c] - X[t.l][c]; }
         mm[0] = rij[1] * rkj[2] - rij[2] * rkj[1]; mm[1] = rij[2] * rkj[0] - rij[0] * rkj[2]; mm[2] = rij[0] * rkj[1] - rij[1] * rkj[0];
         nn[0] = rkj[1] * rkl[2] - rkj[2] * rkl[1]; nn[1] = rkj[2] * rkl[0] - rkj[0] * rkl[2]; nn[2] = rkj[0] * rkl[1] - rkj[1] * rkl[0];
-        const R rkj2 = rkj[0] * rkj[0] + rkj[1] * rkj[1] + rkj[2] * rkj[2], nrkj = mol_sqrt<R>(rkj2);
-        const R phi = mol_atan2<R>(nrkj * (rij[0] * nn[0] + rij[1] * nn[1] + rij[2] * nn[2]), mm[0] * nn[0] + mm[1] * nn[1] + mm[2] * nn[2]);
-        R sn, cs;
-        mol_sincos<R>((R)t.n * phi - (R)t.phase, &sn, &cs);
-        if (ENERGY) { if (t.role == 0) e += t.kk * (1.0 + (double)cs); }
+        const double rkj2 = rkj[0] * rkj[0] + rkj[1] * rkj[1] + rkj[2] * rkj[2], nrkj = sqrt(rkj2);
+        const double phi = atan2(nrkj * (rij[0] * nn[0] + rij[1] * nn[1] + rij[2] * nn[2]), mm[0] * nn[0] + mm[1] * nn[1] + mm[2] * nn[2]);
+        double sn, cs;
+        sincos(t.n * phi - t.phase, &sn, &cs);
+        if (ENERGY) { if (t.role == 0) e += t.kk * (1.0 + cs); }
         else {
-            const R dU = -(R)t.kk * (R)t.n * sn;
-            const R m2 = mm[0] * mm[0] + mm[1] * mm[1] + mm[2] * mm[2], n2 = nn[0] * nn[0] + nn[1] * nn[1] + nn[2] * nn[2];
-            const R pp = (rij[0] * rkj[0] + rij[1] * rkj[1] + rij[2] * rkj[2]) / rkj2, qq = (rkl[0] * rkj[0] + rkl[1] * rkj[1] + rkl[2] * rkj[2]) / rkj2;
-            const R ci = -dU * nrkj / m2, cl = dU * nrkj / n2;
-            R o[3];
+            const double dU = -t.kk * t.n * sn;
+            const double m2 = mm[0] * mm[0] + mm[1] * mm[1] + mm[2] * mm[2], n2 = nn[0] * nn[0] + nn[1] * nn[1] + nn[2] * nn[2];
+            const double pp = (rij[0] * rkj[0] + rij[1] * rkj[1] + rij[2] * rkj[2]) / rkj2, qq = (rkl[0] * rkj[0] + rkl[1] * rkj[1] + rkl[2] * rkj[2]) / rkj2;
+            const double ci = -dU * nrkj / m2, cl = dU * nrkj / n2;
+            double o[3];
             for (int c = 0; c < 3; c++) {
-                const R fi = ci * mm[c], fl = cl * nn[c];
-                const R sv = pp * fi - qq * fl;
+                const double fi = ci * mm[c], fl = cl * nn[c];
+                const double sv = pp * fi - qq * fl;
                 o[c] = t.role == 0 ? fi : (t.role == 1 ? sv - fi : (t.role == 2 ? -sv - fl : fl));
             }
             fx += o[0]; fy += o[1]; fz += o[2];
         }
     }
     const unsigned mask = m.nb_mask[a];
-    const R qa = (R)(MOL_ONE_4PI_EPS0 * m.charge[a]), sa = (R)m.sigma[a], ea = (R)m.seps[a];
+    const double qa = MOL_ONE_4PI_EPS0 * m.charge[a], sa = m.sigma[a], ea = m.seps[a];
     for (int b = 0; b < m.n; b++) {
         if (!((mask >> b) & 1u)) continue;
         if (ENERGY && b < a) continue;
-        const R d[3] = {(R)(xa[0] - X[b][0]), (R)(xa[1] - X[b][1]), (R)(xa[2] - X[b][2])};
-        const R ir2 = (R)1 / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = mol_sqrt<R>(ir2);
-        const R qq = qa * (R)m.charge[b], s = (R)0.5 * (sa + (R)m.sigma[b]), ee = ea * (R)m.seps[b];
-        const R s2 = s * s * ir2, s6 = s2 * s2 * s2;
-        if (ENERGY) e += (double)(qq * ir + (R)4 * ee * (s6 * s6 - s6));
-        else { const R c = (qq * ir + (R)24 * ee * ((R)2 * s6 * s6 - s6)) * ir2; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
+        const double d[3] = {xa[0] - X[b][0], xa[1] - X[b][1], xa[2] - X[b][2]};
+        const double ir2 = 1.0 / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = sqrt(ir2);
+        const double qq = qa * m.charge[b], s = 0.5 * (sa + m.sigma[b]), ee = ea * m.seps[b];
+        const double s2 = s * s * ir2, s6 = s2 * s2 * s2;
+        if (ENERGY) e += qq * ir + 4.0 * ee * (s6 * s6 - s6);
+        else { const double c = (qq * ir + 24.0 * ee * (2.0 * s6 * s6 - s6)) * ir2; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
     }
     for (int q = m.x_off[a]; q < m.x_off[a + 1]; q++) {
         const MolExc x = m.exc[q];
         if (ENERGY && x.j < a) continue;
-        const R d[3] = {(R)(xa[0] - X[x.j][0]), (R)(xa[1] - X[x.j][1]), (R)(xa[2] - X[x.j][2])};
-        const R ir2 = (R)1 / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = mol_sqrt<R>(ir2);
-        const R qq = (R)(MOL_ONE_4PI_EPS0 * x.qq);
-        const R s2 = (R)(x.sig * x.sig) * ir2, s6 = s2 * s2 * s2;
-        if (ENERGY) e += (double)(qq * ir + (R)4 * (R)x.eps * (s6 * s6 - s6));
-        else { const R c = (qq * ir + (R)24 * (R)x.eps * ((R)2 * s6 * s6 - s6)) * ir2; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
+        const double d[3] = {xa[0] - X[x.j][0], xa[1] - X[x.j][1], xa[2] - X[x.j][2]};
+        const double ir2 = 1.0 / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = sqrt(ir2);
+        const double qq = MOL_ONE_4PI_EPS0 * x.qq;
+        const double s2 = (x.sig * x.sig) * ir2, s6 = s2 * s2 * s2;
+        if (ENERGY) e += qq * ir + 4.0 * x.eps * (s6 * s6 - s6);
+        else { const double c = (qq * ir + 24.0 * x.eps * (2.0 * s6 * s6 - s6)) * ir2; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
     }
-    if (!ENERGY) { f[0] = (double)fx; f[1] = (double)fy; f[2] = (double)fz; }
+    if (!ENERGY) { f[0] = fx; f[1] = fy; f[2] = fz; }
     return e;
 }
 
@@ -766,7 +752,7 @@ __device__ __forceinline__ double mol_energy_gb(const MolDev &m, const MolGB &g,
                                                 double *Cs) {
     const int a = threadIdx.x;
     const double e_gb = mol_gb_lane<false>(g, X, ms.charge, a, m.n, Bs, Cs, nullptr);
-    return mol_warp_sum(a < m.n ? mol_atom<true, double>(ms, X, a, nullptr) + e_gb : 0.0);
+    return mol_warp_sum(a < m.n ? mol_atom<true>(ms, X, a, nullptr) + e_gb : 0.0);
 }
 
 // the GB force on atom a (warp 0, after mol_gb_radii_pairs)
@@ -789,8 +775,10 @@ __device__ __forceinline__ void mol_gb_force(const double (*X)[3], int a, int n,
 // STAR: every constraint cluster has at most three constraints (MolDev::max_cluster): the MolStar path.
 // GB: OBC implicit solvent (g), three phases per force evaluation: the descreening integrals with the other terms, then
 // (a block barrier) Born radii, (barrier) pair terms, (barrier) chain-rule factors, then each atom's sum.
+// mv: the move, __grid_constant__ so that the program is indexed in the parameter bank (a plain by-value struct of this
+// size is copied to local memory).  `reassign` stays an argument: read from mv, it costs this kernel 40-250 instructions.
 template <bool STAR, bool GB>
-__global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynParams p, const StateDev *__restrict__ states,
+__global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, const __grid_constant__ MoveDev mv, const StateDev *__restrict__ states,
                                                       const int *__restrict__ perm, double *__restrict__ pos,
                                                       double *__restrict__ vel, int k0, uint2 key, uint32_t iteration,
                                                       int reassign, double *__restrict__ pot, double *__restrict__ kin,
@@ -830,19 +818,19 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
     __syncwarp();
     const double inv_mass = 1.0 / mass;
     // (the program is interpreted, so the compiler does not hoist these out of the step loop: two f64 divisions per R)
-    const double hm = (double)p.dt_d / p.nV * inv_mass, h = (double)p.dt_d / p.nR, inv_h = 1.0 / h;
+    const double hm = mv.dt_d / mv.nV * inv_mass, h = mv.dt_d / mv.nR, inv_h = 1.0 / h;
     double f[3] = {0, 0, 0};
     bool f_valid = false;
     uint32_t ocount = 0;
-    for (int s = 0; s < p.n_steps; s++) {
+    for (int s = 0; s < mv.n_steps; s++) {
         if (m.remove_cm) {
             double px = mol_warp_sum(active ? mass * V[a][0] : 0.0), py = mol_warp_sum(active ? mass * V[a][1] : 0.0),
                    pz = mol_warp_sum(active ? mass * V[a][2] : 0.0);
             if (active) { V[a][0] -= px * inv_mt; V[a][1] -= py * inv_mt; V[a][2] -= pz * inv_mt; }
             __syncwarp();
         }
-        for (int q = 0; q < p.n_prog; q++) {
-            const char op = p.prog[q];
+        for (int q = 0; q < mv.n_prog; q++) {
+            const char op = mv.prog[q];
             if (op == 'V') {
                 if (!f_valid) {
                     __syncthreads();   // warp 0's positions are in shared memory
@@ -879,9 +867,9 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
             } else {   // 'O'
                 if (active) {
                     const float3 g = philox_normal3(philox4x32_10(make_uint4(a, ocount, k, iteration), key));
-                    V[a][0] = p.a_d * V[a][0] + p.b_d * sg * (double)g.x;
-                    V[a][1] = p.a_d * V[a][1] + p.b_d * sg * (double)g.y;
-                    V[a][2] = p.a_d * V[a][2] + p.b_d * sg * (double)g.z;
+                    V[a][0] = mv.a_d * V[a][0] + mv.b_d * sg * (double)g.x;
+                    V[a][1] = mv.a_d * V[a][1] + mv.b_d * sg * (double)g.y;
+                    V[a][2] = mv.a_d * V[a][2] + mv.b_d * sg * (double)g.z;
                 }
                 ocount++;
                 __syncwarp();
@@ -890,7 +878,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, DynP
             }
         }
     }
-    const double U = GB ? mol_energy_gb(m, g, ms, X, gs.B, gs.C) : mol_warp_sum(active ? mol_atom<true, double>(ms, X, a, nullptr) : 0.0);
+    const double U = GB ? mol_energy_gb(m, g, ms, X, gs.B, gs.C) : mol_warp_sum(active ? mol_atom<true>(ms, X, a, nullptr) : 0.0);
     const double KE = mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
     const bool bad = active && !(isfinite(X[a][0]) && isfinite(X[a][1]) && isfinite(X[a][2]) && isfinite(V[a][0]) &&
                                  isfinite(V[a][1]) && isfinite(V[a][2]));
@@ -941,7 +929,7 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
     int n_pos = 0, it = 0;
     for (;; it++) {
         double f[3] = {0, 0, 0};
-        if (active) mol_atom<false, double>(ms, X, a, f);
+        if (active) mol_atom<false>(ms, X, a, f);
         if (GB) {
             double *gbs = (double *)((unsigned char *)mol_tab + m.shared_bytes);
             mol_gb_lane<true>(g, X, ms.charge, a, n, gbs, gbs + MOL_MAX_ATOMS, f);
@@ -999,7 +987,7 @@ __global__ void __launch_bounds__(32) k_energy_mol(MolDev m, const StateDev *__r
     __syncwarp();
     double *gbs = (double *)((unsigned char *)mol_tab + m.shared_bytes);
     const double U = GB ? mol_energy_gb(m, g, ms, X, gbs, gbs + MOL_MAX_ATOMS)
-                        : mol_warp_sum(active ? mol_atom<true, double>(ms, X, a, nullptr) : 0.0);
+                        : mol_warp_sum(active ? mol_atom<true>(ms, X, a, nullptr) : 0.0);
     for (int l = a; l < n_states; l += 32) u_out[(size_t)k * n_states + l] = states[l].beta * (U + states[l].offset);
 }
 
@@ -1013,18 +1001,5 @@ __global__ void k_randomize_velocities_mol(MolDev m, const StateDev *__restrict_
     vel[((size_t)r * m.n + a) * 3 + 0] = sv * g.x;
     vel[((size_t)r * m.n + a) * 3 + 1] = sv * g.y;
     vel[((size_t)r * m.n + a) * 3 + 2] = sv * g.z;
-}
-
-__global__ void k_restore_failed_mol(const int *__restrict__ nan_flag, int *__restrict__ retry, int k0, int N,
-                                     const double *__restrict__ pos_snap, const double *__restrict__ vel_snap,
-                                     double *__restrict__ pos, double *__restrict__ vel) {
-    const int r = blockIdx.x, k = k0 + r;
-    const int failed = nan_flag[k];
-    if (threadIdx.x == 0) retry[k] = failed;
-    if (!failed) return;
-    for (int q = threadIdx.x; q < 3 * N; q += blockDim.x) {
-        pos[(size_t)r * N * 3 + q] = pos_snap[(size_t)r * N * 3 + q];
-        vel[(size_t)r * N * 3 + q] = vel_snap[(size_t)r * N * 3 + q];
-    }
 }
 
