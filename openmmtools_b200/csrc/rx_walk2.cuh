@@ -332,22 +332,27 @@ __device__ __forceinline__ void w2_walk(const SlotRec2 *__restrict__ rec, const 
         uint4 qB = w2_lds128(ring_base + (ridxB << 4));
         ahead(qB);
         uint2 ei = w2_lds64(repiA), ej = w2_lds64(repjA);   // {state, diag} of both replicas
-        // what the round resolved last leaves to the next block: the committed window positions, the positions that leave
-        // the window, all-ones if this lane's attempt changes the permutation, its log entry
-        unsigned p_cm = 0, p_below = 0, p_chg = 0, p_entry = 0;
+        // what the round resolved last leaves to the next block: the stops (window order; the positions below the lowest one
+        // leave the window, 0: all of them), the visited positions, all-ones if this lane's position is visited / is visited
+        // and its attempt changes the permutation, its log entry
+        unsigned p_stop = 1, p_vis = 0, p_mv = 0, p_sw = 0, p_entry = 0;
+        unsigned lem = (2u << w) - 1u;   // the lane's prefix mask: window positions 0 .. w (w = 31: all)
         float f_ij = 0.f, f_ji = 0.f;
         unsigned K1w = 0, K2w = 0;   // candidates: window-order masks of the positions with k == 1 / k == 2 (state independent)
         // Commit the round described by the p_* values, slide the window and fetch the states of the next round:
         // permutation stores, at once the next round's loads, then the lane state.
         auto commit = [&]() {
-            // the window advances by the number of positions that leave it (computed here rather than where `below` appears,
-            // at the end of the previous block: a population count is a long-latency operation whose scoreboard slot would
-            // otherwise be waited for at the loop's back edge)
+            // A lane's record leaves the window iff no stop lies at or before its position: one test of the stops against
+            // the lane's own prefix mask, so that the predicates of the stores are one test away from the stop mask.  The
+            // committed prefix itself (`below`) is only needed for the counts, off that chain; the
+            // window advances by its population count (computed here rather than at the end of the previous block: a
+            // population count is a long-latency operation whose scoreboard slot would otherwise be waited for at the
+            // loop's back edge).
+            const bool p_promoted = (p_stop & lem) == 0u;
+            const bool p_mine = p_promoted && p_mv != 0u;
+            const bool p_swaps = p_promoted && p_sw != 0u;
+            const unsigned p_below = (p_stop & (0u - p_stop)) - 1u;
             const unsigned p_advance = (unsigned)__popc(p_below);
-            const unsigned bit = 1u << w;
-            const bool p_mine = (p_cm & bit) != 0u;
-            const bool p_swaps = (p_cm & bit & p_chg) != 0u;
-            const bool p_promoted = (p_below & bit) != 0u;
             if (p_swaps) {   // replica i takes state sj: its new diagonal value is the off-diagonal one just read
                 w2_sts64(repiA, ej.x, __float_as_uint(f_ij));
                 w2_sts64(repjA, ei.x, __float_as_uint(f_ji));
@@ -373,10 +378,11 @@ __device__ __forceinline__ void w2_walk(const SlotRec2 *__restrict__ rec, const 
             qB = w2_lds128(ring_base + (ridxB << 4));
             h += p_advance;
             r = (r + p_advance) & 31u;
-            rem -= __popc(p_cm);
+            rem -= __popc(p_vis & p_below);
             ei = ein;
             ej = ejn;
             w = (w - p_advance) & 31u;
+            lem = (2u << w) - 1u;
             if constexpr (CAND) {   // the hop classes of the new window (off the chain: they only depend on the promotions)
                 const unsigned b1 = __ballot_sync(0xffffffffu, kA == 1u), b2 = __ballot_sync(0xffffffffu, kA == 2u);
                 K1w = __funnelshift_r(b1, b1, r); K2w = __funnelshift_r(b2, b2, r);
@@ -426,9 +432,9 @@ __device__ __forceinline__ void w2_walk(const SlotRec2 *__restrict__ rec, const 
                 // at the forced stops of the chain.
                 const unsigned C = __ballot_sync(0xffffffffu, ((earlier & bmA) | und) != 0u);
                 Cw = (__funnelshift_r(C, C, r) | Cf) & V;   // empty: the whole window commits
-                const unsigned low = Cw & (0u - Cw);
-                const unsigned below = low - 1u;       // low == 0 -> all lanes
-                p_cm = V & below; p_below = below; p_chg = changes ? 0xffffffffu : 0u;
+                p_stop = Cw; p_vis = V;
+                p_mv = ((V >> w) & 1u) != 0u ? 0xffffffffu : 0u;
+                p_sw = changes ? p_mv : 0u;
                 p_entry = (sj * (1u << LOG_STATE_BITS) + si) | (acc ? (1u << 31) | (1u << LOG_ACC_BIT) : (1u << 31));
                 // (position 0 is always visited: nothing commits iff it is itself the lane that ends the round)
             } while (--quota != 0u && (Cw & 1u) == 0u);
@@ -478,19 +484,20 @@ __device__ __forceinline__ void w2_walk(const SlotRec2 *__restrict__ rec, const 
                 __syncwarp();
                 const bool first_ge0 = __ballot_sync(0xffffffffu, (d & 1u) != 0u) != 0u;
                 const bool acc = (d & 2u) != 0u;
-                p_cm = 1u;
+                p_vis = 1u;
                 if constexpr (CAND) {
                     const unsigned k0 = (K1w & 1u) + 2u * (K2w & 1u);   // hop class of window position 0
-                    p_below = first_ge0 ? 3u : (4u << k0) - 1u;         // 2 or 2 + k positions leave the window
+                    p_stop = first_ge0 ? 4u : 4u << k0;                 // 2 or 2 + k positions leave the window
                 } else {
-                    p_below = first_ge0 ? 1u : 3u;                      // 1 or 2
+                    p_stop = first_ge0 ? 2u : 4u;                       // 1 or 2
                 }
-                p_chg = (acc && neqA != 0u) ? 0xffffffffu : 0u;
+                p_mv = w == 0u ? 0xffffffffu : 0u;
+                p_sw = (acc && neqA != 0u) ? p_mv : 0u;
                 p_entry = (sj * (1u << LOG_STATE_BITS) + si) | (acc ? (1u << 31) | (1u << LOG_ACC_BIT) : (1u << 31));
                 commit();
                 w2_cp_async_wait<8>();
                 ahead(qB);
-                p_cm = p_below = 0;
+                p_stop = 1u; p_vis = 0u;
             }
         }
         commit();   // the round resolved last, if one is pending

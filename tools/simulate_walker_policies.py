@@ -7,6 +7,16 @@ permutation.  Rounds are then counted for:
            state-changing swap of the same round (window of W slots);
   P1       first-order forwarding: such a slot may stay in the round when exactly ONE earlier swap of the round touched it
            and that swap was itself evaluated normally (its new state could be forwarded by a shuffle);
+  P2, P3   one-level forwarding without iteration.  The partner of slot p = (i, j), i != j, is the most recent of the 31
+           slots before it that shares a replica with it (state independent).  Every slot is evaluated under the round's
+           starting states (branch 0) and under the states its partner's swap would leave (branch 1); it takes branch 1
+           if its partner lies in the window, changes the permutation under the starting states and is guessed visited:
+           P2 guesses visited unless slot q-1 (in the window, evaluated under the starting states) draws a uniform, P3
+           takes q's bit of the visited chain of the branch-0 decisions.  A visited slot is stale if a visited changing
+           swap other than its partner shares a replica with it, if its guess was wrong, or if its partner is a visited
+           slot that took branch 1; the round ends at the first stale slot or at a slot-31 attempt that draws a uniform.
+           (Measured on an H100 with P3 in k_mix_walk2: the headline's rounds fell 1.44x, but a round took 275 instead of
+           128 SASS instructions and 2.3x as long, so the walker was 1.52x slower; DESIGN.md section 9.)
   levels   the dependency depth of the true DAG (attempt waits for the last accepted swap that touched its replicas, and
            for its predecessor in the stream): the floor for any scheme without value prediction.
 Usage: python tools/simulate_walker_policies.py [K] [nswap] [model]"""
@@ -86,6 +96,92 @@ for W in (32, 64):
     r0 = rounds(W, False); r1 = rounds(W, True)
     print('window %2d slots: P0 %7d rounds (%.2f attempts/round)   P1 %7d rounds (%.2f attempts/round, x%.2f fewer)' % (
         W, r0, nswap / r0, r1, nswap / r1, r0 / r1))
+
+
+def rounds_forward(guess, limit):
+    """P2 (guess = 'prev') and P3 (guess = 'v0') over a 32-slot window: (rounds, attempts), the first `limit` attempts."""
+    IJ = [(int(words[2 * s]) & mask, int(words[2 * s + 1]) & mask) for s in range(len(words) // 2 - 2)]
+
+    def decide(s, si, sj):   # (log_p >= 0, accepted) of an attempt at slot s with replica states si, sj
+        i, j = IJ[s]
+        lp = -(ul[i][sj] + ul[j][si]) + ul[i][si] + ul[j][sj]
+        if lp >= 0.0:
+            return True, True
+        a, b = int(words[2 * s + 2]) >> 5, int(words[2 * s + 3]) >> 6
+        return False, (a * 67108864.0 + b) / 9007199254740992.0 < math.exp(lp)
+
+    def partner(s):          # (d, r, b) or None
+        i, j = IJ[s]
+        if i == j:
+            return None
+        for d in range(1, min(32, s + 1)):
+            oi, oj = IJ[s - d]
+            if oi in (i, j) or oj in (i, j):
+                if i != j and {oi, oj} == {i, j}:
+                    return d, i, j
+                r = i if i in (oi, oj) else j
+                return d, r, (oj if oi == r else oi)
+        return None
+
+    perm = list(range(K)); h = 0; n_rounds = 0; att = 0
+    while att < limit:
+        n_rounds += 1
+        start = perm[:]
+        b0 = [decide(h + w, start[IJ[h + w][0]], start[IJ[h + w][1]]) for w in range(32)]
+        v0 = set(); w = 0
+        while w < 32:
+            v0.add(w); w += 1 if b0[w][0] else 2
+        fw = [False] * 32; alt = [None] * 32; part = [None] * 32
+        for w in range(1, 32):
+            pq = partner(h + w)
+            if pq is None or pq[0] > w:
+                continue
+            d, r, b = pq; q = w - d; part[w] = q
+            i, j = IJ[h + w]
+            st = {i: start[i], j: start[j]}
+            if {i, j} == {r, b} and r != b:
+                st = {i: start[j], j: start[i]}
+            else:
+                st[r] = start[b]
+            alt[w] = decide(h + w, st[i], st[j])
+            qchg = b0[q][1] and r != b
+            if guess == 'v0':
+                seen = q in v0
+            elif guess == 'prev':
+                seen = not (q - 1 >= 0 and not b0[q - 1][0])
+            else:   # P0: never forward
+                seen = False
+            fw[w] = qchg and seen
+        committed = {}   # window position -> (changed, took branch 1)
+        w = 0
+        while w < 32 and att < limit:
+            i, j = IJ[h + w]
+            q = part[w]
+            stale = any(c[0] and e != q and set(IJ[h + e]) & {i, j} for e, c in committed.items())
+            if q is not None:
+                q_va = q in committed and committed[q][0]
+                stale = stale or fw[w] != q_va or (q in committed and committed[q][1])
+            if stale:
+                break
+            ge, acc = alt[w] if fw[w] else b0[w]
+            assert (ge, acc) == decide(h + w, perm[i], perm[j])   # the rules commit only decisions under the right states
+            if w == 31 and not ge:
+                break
+            committed[w] = (acc and i != j, fw[w])
+            if acc:
+                perm[i], perm[j] = perm[j], perm[i]
+            att += 1
+            w += 1 if ge else 2
+        h += max(w, 1)
+    return n_rounds, att
+
+
+n_fwd = min(nswap, 60000)
+rp0 = rounds_forward('none', n_fwd)
+for name, g in (('P2', 'prev'), ('P3', 'v0')):
+    rf = rounds_forward(g, n_fwd)
+    print('window 32 slots, first %d attempts: P0 %d rounds (%.2f attempts/round)   %s %d rounds (x%.2f fewer)' % (
+        n_fwd, rp0[0], rp0[1] / rp0[0], name, rf[0], rp0[0] / rf[0]))
 # dependency levels
 last = [0] * K
 F = 0
