@@ -109,7 +109,7 @@ struct rx_engine {
     uint32_t *d_log = nullptr;   // commit log of the walker: packed (si, sj, accepted)
     size_t log_cap = 0;
     uint32_t *d_slotlog = nullptr;   // sparse commit log of k_mix_walk2: one word per slot
-    uint32_t *d_cpos = nullptr;      // k_mix_walk2c: word position of every candidate of the pass
+    uint32_t *d_cpos = nullptr;      // k_mix_walk2c / k_mix_walk_cand: word position of every candidate of the pass
     uint32_t *d_ctile = nullptr;     // ... candidates per tile / their exclusive scan, then [last] = number of candidates
     size_t ctile_cap = 0;
     unsigned char *d_filt = nullptr;   // 24-bit row image of u for the K=256 walker

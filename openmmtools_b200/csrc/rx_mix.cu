@@ -2,7 +2,7 @@
 //
 // Replaces ReplicaExchangeSampler._mix_replicas (openmmtools/multistate/replicaexchange.py:255-292):
 //   swap-all       _mix_all_replicas_numba  (replicaexchange.py:294-349)  -> k_mix_walk2 / k_mix_walk_pow2 (K a power of two),
-//                                                                            k_mix_walk2c / k_mix_walk_any (any other K), k_mix_walk_serial
+//                                                                            k_mix_walk2c / k_mix_walk_cand (any other K), k_mix_walk_serial
 //   swap-neighbors _mix_neighboring_replicas (replicaexchange.py:366-406) -> k_mix_neighbors
 // The results are bit-identical to the reference for the same MT19937 state: the random stream is numba's
 // (numba/_random.c:37-73; randint = low bit_length(K-1) bits of one word with rejection, rand = 53-bit double
@@ -13,9 +13,10 @@
 // even word ("slot"), so a parallel pre-pass turns the stream into slot records (i, j, log U, overlap mask)
 // and ONE warp then walks the chain speculatively: 32 lanes evaluate 32 consecutive slots under the current
 // permutation, the visited-slot chain is resolved with a carry-propagation bit trick, and the longest prefix
-// in which no visited slot touches a replica swapped earlier in the same window is committed.  The filter walkers
-// (rx_walk2.cuh, rx_walk2c.cuh) take the bulk of a pass for K <= 256; the exact walker (rx_walk_exact.cuh) finishes
-// their passes over slots and walks every pass of larger K.
+// in which no visited slot touches a replica swapped earlier in the same window is committed.  Any other K is walked the
+// same way in candidate coordinates (the words randint accepts, rx_walk2c.cuh).  The filter walkers (rx_walk2.cuh) take
+// the bulk of a pass for K <= 256; the exact walker (rx_walk_exact.cuh) finishes their passes over slots and walks every
+// pass of larger K (and of any K with RX_NO_FILTER=1) in either coordinate system.
 #include "rx_internal.cuh"
 #include <type_traits>
 #include <math.h>
@@ -173,15 +174,16 @@ int rxi_selftest_exp(rx_engine *h, const double *x, double *y, int n) {
 
 // ------------------------------------------------------------------------------------------------------
 // The speculative chain walkers: the filter walkers (rx_walk2.cuh, rx_walk2c.cuh) and the exact walker
-// (rx_walk_exact.cuh).  Their state-independent records (slot records: k_slots_build, rx_walk2.cuh) are built in
-// parallel; each logs the attempts it commits as packed (si, sj, accepted) entries, bit 31 set.
+// (rx_walk_exact.cuh).  Their state-independent records (slot records: k_slots_build, rx_walk2.cuh; candidate records:
+// k_cand_*, rx_walk2c.cuh) are built in parallel; each logs the attempts it commits as packed (si, sj, accepted) entries,
+// bit 31 set.
 // ------------------------------------------------------------------------------------------------------
 #define LOGU_ZERO (-745.5)  /* stands in for log(0): exp(x) == 0 <=> x < -745.13 */
 #define LOG_ACC_BIT 28
 #define LOG_STATE_BITS 14
 #include "rx_walk2.cuh"
-#include "rx_walk_exact.cuh"
 #include "rx_walk2c.cuh"
+#include "rx_walk_exact.cuh"
 
 // 24-bit row image of the energy matrix for the filter walkers: delta = u[k,l] - min_l u[k,l] as a float32 truncated to
 // its top 24 bits (sign, 8 exponent, 15 mantissa bits), stored as a uint16 plane followed by a uint8 plane.  Relative
@@ -449,7 +451,11 @@ static inline unsigned count_blocks(const rx_engine *h, long long n) {
     return (unsigned)(nb < h->n_sm * 16 ? nb : h->n_sm * 16);
 }
 
-enum { REC_NONE = 0, REC_SLOT = 1, REC_SLOT2 = 2, REC_WORD = 3, REC_CAND = 4 };   // what prepare_pass builds from the stream
+// what prepare_pass builds from the stream: slot or candidate records, for the exact walker or (2: SlotRec2) the filter walkers
+enum { REC_NONE = 0, REC_SLOT = 1, REC_SLOT2 = 2, REC_CAND = 3, REC_CAND2 = 4 };
+
+// number of candidates of the pass, behind the tile counts and their scan
+static inline uint32_t *cand_total(const rx_engine *h) { return h->d_ctile + (h->ctile_cap / CAND_TILE + 4); }
 
 static inline size_t pass_need(long long remaining, bool fast, bool anyk = false) {
     const size_t chunk_words = anyk ? (size_t)1 << 25 : (size_t)1 << 26;  // words per pass (any K: 16 bytes of records per word)
@@ -463,14 +469,14 @@ static inline size_t pass_need(long long remaining, bool fast, bool anyk = false
 // on stream `st`.  Both are state independent, so for the NEXT mixing call this runs on the side stream while the
 // replicas are being propagated.
 static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, bool fast, int kind, int K, cudaStream_t st, int *launches) {
-    const bool rec2 = kind == REC_SLOT2, candk = kind == REC_CAND, anyk = kind == REC_WORD || candk;
+    const bool rec2 = kind == REC_SLOT2, anyk = kind == REC_CAND || kind == REC_CAND2;
     const size_t need = pass_need(remaining, fast, anyk);
     int rc = stream_reserve(h, S, 2 * need + 1024);   // room for the words generated ahead while the walker runs
     if (rc) return rc;
     rc = stream_fill(h, S, need, launches, st);
     if (rc) return rc;
     if (fast || anyk) {
-        const long long nslots = anyk ? (long long)S.avail : (long long)(S.avail / 2);   // records: per slot, or per word
+        const long long nslots = anyk ? (long long)S.avail : (long long)(S.avail / 2);   // records: per slot, or <= 1 per word
         if ((size_t)nslots > h->slots_cap) {
             // size for the largest stream the buffer can ever hold (2 * need + 1024 words), so that the slightly different
             // `avail` of every iteration never triggers another cudaFree/cudaMalloc (tens of ms each, device-synchronising)
@@ -488,7 +494,7 @@ static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, bool fas
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_slotlog, want * sizeof(uint32_t)));
             h->slots_cap = want;
         }
-        if (candk && (!h->d_cpos || h->ctile_cap < h->slots_cap)) {
+        if (anyk && (!h->d_cpos || h->ctile_cap < h->slots_cap)) {
             RX_CHECK_CUDA(h, cudaDeviceSynchronize());
             cudaFree(h->d_cpos); cudaFree(h->d_ctile);
             h->d_cpos = nullptr; h->d_ctile = nullptr;
@@ -496,23 +502,22 @@ static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, bool fas
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_ctile, (h->slots_cap / CAND_TILE + 8) * sizeof(uint32_t)));
             h->ctile_cap = h->slots_cap;
         }
-        if (candk) {
+        if (anyk) {
             // candidate coordinates (rx_walk2c.cuh): flag + count per tile, scan, scatter, one record per candidate index
+            static_assert(sizeof(CandRec) == sizeof(SlotRec), "all record formats share the d_slots buffer");
             int nbits = 0;
             for (unsigned m = (unsigned)(K - 1); m; m >>= 1) nbits++;
             const uint32_t mask = 0xffffffffu >> (32 - nbits);
             const int ntiles = (int)((nslots + CAND_TILE - 1) / CAND_TILE);
-            uint32_t *d_ncand = h->d_ctile + (h->ctile_cap / CAND_TILE + 4);
+            const unsigned nblk = (unsigned)((nslots + 255) / 256);
             k_cand_count<<<ntiles, 256, 0, st>>>(S.d_words, nslots, K, mask, h->d_ctile);
-            k_cand_scan<<<1, 1024, 0, st>>>(h->d_ctile, ntiles, d_ncand);
+            k_cand_scan<<<1, 1024, 0, st>>>(h->d_ctile, ntiles, cand_total(h));
             k_cand_scatter<<<ntiles, 256, 0, st>>>(S.d_words, nslots, K, mask, h->d_ctile, h->d_cpos);
-            k_cand_records<<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, h->d_cpos, d_ncand, mask, (SlotRec2 *)h->d_slots);
+            if (kind == REC_CAND2)
+                k_cand_records<false><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (SlotRec2 *)h->d_slots);
+            else
+                k_cand_records<true><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (CandRec *)h->d_slots);
             *launches += 3;
-        } else if (anyk) {
-            static_assert(sizeof(WordRec) == sizeof(SlotRec), "all record formats share the d_slots buffer");
-            int nbits = 0;
-            for (unsigned m = (unsigned)(K - 1); m; m >>= 1) nbits++;
-            k_words_build<<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, K, 0xffffffffu >> (32 - nbits), (WordRec *)h->d_slots);
         } else if (rec2)
             k_slots_build<true><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec2 *)h->d_slots);
         else
@@ -543,7 +548,7 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         return RX_OK;
     }
     const bool fast = is_pow2(K) && K <= (1 << LOG_STATE_BITS);
-    // any other K up to 4095: the speculative walker over word positions (rx_walk_exact.cuh); RX_WALK_SERIAL=1: the plain loop
+    // any other K up to 4095: the speculative walkers in candidate coordinates (rx_walk2c.cuh); RX_WALK_SERIAL=1: the plain loop
     const bool anyk = !fast && K >= 3 && K <= ANY_MAX_K && !getenv("RX_WALK_SERIAL");
     int logK = 0;
     while ((1 << logK) < K) logK++;
@@ -554,26 +559,26 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
     // smaller K the filter is still faster than f64 comparisons): 16-byte SlotRec2 records, k_mix_walk2 for the bulk of a pass
     // and k_mix_walk_pow2<true> for its tail.  Otherwise (RX_NO_FILTER=1: every K) exact f64 values from L2.
     const bool rec2 = fast && smem_f24 <= 224 * 1024 && !getenv("RX_NO_FILTER");
-    // any K <= 256 whose row image fits: the walker of k_mix_walk2 in candidate coordinates (k_mix_walk2c, rx_walk2c.cuh);
-    // RX_WALK_ANY_V1=1 keeps the word-position walker (cross-check)
+    // any K <= 256 whose row image fits: the walker of k_mix_walk2 in candidate coordinates (k_mix_walk2c); otherwise (and
+    // with RX_NO_FILTER=1) the exact walker k_mix_walk_cand
     const size_t smem_w2 = (size_t)W2_RING * 16 + (size_t)K * 8 + (size_t)((3 * K + 1) & ~1) * K;   // ring, replicas, image
-    const bool candk = anyk && K <= 256 && smem_w2 <= 224 * 1024 && !getenv("RX_WALK_ANY_V1") && !getenv("RX_NO_FILTER");
-    const int kind = candk ? REC_CAND : (anyk ? REC_WORD : (!fast ? REC_NONE : (rec2 ? REC_SLOT2 : REC_SLOT)));
+    const bool cand2 = anyk && K <= 256 && smem_w2 <= 224 * 1024 && !getenv("RX_NO_FILTER");
+    const int kind = anyk ? (cand2 ? REC_CAND2 : REC_CAND) : (!fast ? REC_NONE : (rec2 ? REC_SLOT2 : REC_SLOT));
     // The walkers are one latency-bound CTA each: they claim (almost) a whole SM's shared memory so that no other CTA -- in
     // particular the stream generator that runs concurrently on the side stream -- is scheduled onto the same SM and steals
     // issue slots.  226 KB + the kernel's static shared memory + the generator's 8 KB exceed the SM's 228 KB.
     const int smem_walk = 226 * 1024;
     if (!fast) {
         if (smem_small > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_serial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_small));
-        if (candk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2c, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
-        if (anyk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_any, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
+        if (cand2) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2c, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
+        else if (anyk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_cand, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
     } else {
         RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
         RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
         RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
     }
     tr.mark("func attributes");
-    if (rec2 || candk) {
+    if (rec2 || cand2) {
         if (!h->d_filt) {
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt, (size_t)3 * K * K + 16));
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt_scale, sizeof(double) * 2 * K));
@@ -592,10 +597,10 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         static_assert(sizeof(SlotRec2) == sizeof(SlotRec), "both record formats share the d_slots buffer");
         if (smem_w2 > (size_t)smem_walk) RX_FAIL(h, RX_ERR_INVALID, "internal: filter walker shared memory");
         RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, nrec * sizeof(uint32_t), h->stream));
-        if (candk)
-            k_mix_walk2c<<<1, W2_THREADS, smem_walk, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos,
-                                                                    h->d_ctile + (h->ctile_cap / CAND_TILE + 4), h->d_u, K, h->d_perm,
-                                                                    h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
+        if (cand2)
+            k_mix_walk2c<<<1, W2_THREADS, smem_walk, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos, cand_total(h),
+                                                                    h->d_u, K, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale,
+                                                                    h->d_ctl);
         else
             k_mix_walk2<<<1, W2_THREADS, smem_walk, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K,
                                                                    logK, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
@@ -659,19 +664,19 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
                 S.avail += ahead;
             }
         } else {
-            if (candk) {
-                // bulk of the pass: the filter walker over candidate indices; the plain loop below finishes the pass
+            if (anyk) {
+                // bulk of the pass: a walker over candidate indices (the filter walker, or the exact one, which claims the SM
+                // like the others); the plain loop below finishes the pass
                 RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
-                if ((rc = filter_walk(S.avail))) return rc;
+                if (cand2) {
+                    if ((rc = filter_walk(S.avail))) return rc;
+                } else {
+                    k_mix_walk_cand<<<1, 64, smem_walk, h->stream>>>((const CandRec *)h->d_slots, S.d_words, h->d_cpos, cand_total(h),
+                                                                       h->d_u, K, h->d_perm, h->d_log, h->d_ctl);
+                    RX_CHECK_CUDA(h, cudaGetLastError());
+                    *launches += 1;
+                }
                 RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
-            } else if (anyk) {
-                // bulk of the pass: speculative walker over word positions (claims the SM like the power-of-two walkers);
-                // what it leaves -- the last words of the pass -- is finished by the plain loop below
-                RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
-                k_mix_walk_any<<<1, 64, smem_walk, h->stream>>>((const WordRec *)h->d_slots, S.d_words, (unsigned)S.avail, h->d_u, K, h->d_perm, h->d_log, h->d_ctl);
-                RX_CHECK_CUDA(h, cudaGetLastError());
-                RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
-                *launches += 1;
             }
             k_mix_walk_serial<<<1, 32, smem_small, h->stream>>>(S.d_words, (long long)S.avail, h->d_u, K, M, h->d_perm, h->d_nacc,
                                                         h->d_nprop, h->d_ctl);
@@ -691,7 +696,7 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
             RX_CHECK_CUDA(h, cudaGetLastError());
             *launches += 1;
         }
-        if (ctl.log_count > 0) {   // the dense log of k_mix_walk_pow2 / k_mix_walk_any
+        if (ctl.log_count > 0) {   // the dense log of k_mix_walk_pow2 / k_mix_walk_cand
             k_mix_count<<<count_blocks(h, ctl.log_count), 256, 0, h->stream>>>(h->d_log, ctl.log_count, M, h->d_nacc, h->d_nprop);
             RX_CHECK_CUDA(h, cudaGetLastError());
             *launches += 1;

@@ -1,5 +1,5 @@
-// rx_walk2c.cuh -- candidate coordinates for the filter walker k_mix_walk2c (rx_walk2.cuh) at ANY K <= 256 (included by
-// rx_mix.cu after rx_walk2.cuh).
+// rx_walk2c.cuh -- candidate coordinates for the filter walker k_mix_walk2c (rx_walk2.cuh) at any K <= 256 and the exact
+// walker k_mix_walk_cand (rx_walk_exact.cuh) at any K <= ANY_MAX_K (included by rx_mix.cu after rx_walk2.cuh).
 //
 // For K that is not a power of two numba's randint rejects words (numba/_random.c: low bit_length(K-1) bits of one word,
 // retried while >= K), so attempts have no fixed length in the word stream.  In CANDIDATE coordinates they do: let the
@@ -10,10 +10,18 @@
 // words -- a property of the stream alone.  So a state-independent pre-pass (flag, scan, scatter, records) gives one
 // 16-byte record per candidate index {i | j << 16, back-mask, f32 log-uniform of this attempt, k}, and the walker is
 // the one of k_mix_walk2 with a window of 32 candidate indices and hops of 2, 3 or 4 instead of 1 or 2 (its visited chain:
-// w2_chain_cand; replicaexchange.py:321-349 bit for bit, like every other walker here).
+// w2_chain_cand; replicaexchange.py:321-349 bit for bit, like every other walker here).  The exact walker takes a CandRec
+// per candidate index instead, with the f64 log-uniform and 12-bit indices.
 #pragma once
 
 #define CAND_TILE 2048    // words per block of the flag/scan/scatter pre-pass
+#define ANY_MAX_K 4095    // 12-bit indices in a CandRec
+
+struct CandRec {          // 16 bytes, one per candidate index c: the attempt that would start there (exact walker)
+    uint32_t ijk;         // i | j << 12 | k << 24; k = hop class as in SlotRec2
+    uint32_t backmask;    // bit 31-b: the attempt at c-1-b shares a replica index with this one
+    double logU;          // log of the uniform this attempt draws if log_p < 0
+};
 
 // (1) candidates per tile of CAND_TILE words
 __global__ void __launch_bounds__(256) k_cand_count(const uint32_t *__restrict__ words, long long nwords, int K, uint32_t mask,
@@ -80,9 +88,12 @@ __global__ void __launch_bounds__(256) k_cand_scatter(const uint32_t *__restrict
         if ((flags >> q) & 1u) cpos[c++] = (uint32_t)(p0 + 8 * t + q);
 }
 
-// (4) one record per candidate index c < ncand - 3 (the attempt that would start there)
+// (4) one record per candidate index c < ncand - 3 (the attempt that would start there): SlotRec2 for the filter walker,
+// CandRec (EXACT) for the exact walker
+template <bool EXACT>
 __global__ void __launch_bounds__(256) k_cand_records(const uint32_t *__restrict__ words, const uint32_t *__restrict__ cpos,
-                                                      const uint32_t *__restrict__ ncand_p, uint32_t mask, SlotRec2 *__restrict__ rec) {
+                                                      const uint32_t *__restrict__ ncand_p, uint32_t mask,
+                                                      std::conditional_t<EXACT, CandRec, SlotRec2> *__restrict__ rec) {
     __shared__ uint32_t s_v[256 + 31 + 1];   // values of candidates c0-31 .. c0+256
     const uint32_t ncand = *ncand_p;
     const long long c0 = (long long)blockIdx.x * 256;
@@ -107,10 +118,18 @@ __global__ void __launch_bounds__(256) k_cand_records(const uint32_t *__restrict
     const uint32_t a = cpos[c + 1] + 1u;   // the uniform's words: a, a + 1 (cpos[c+3] >= a + 1: inside the stream)
     const uint32_t k = (cpos[c + 2] <= a + 1u ? 1u : 0u) + (cpos[c + 3] <= a + 1u ? 1u : 0u);
     const double U = mt_double(words[a], words[a + 1]);
-    SlotRec2 r;
-    r.ij = i | (j << 16);
-    r.backmask = bm;
-    r.lu_next = __float_as_uint((float)((U == 0.0) ? LOGU_ZERO : log(U)));
-    r.k = k;
-    rec[c] = r;
+    if constexpr (EXACT) {
+        CandRec r;
+        r.ijk = i | (j << 12) | (k << 24);
+        r.backmask = bm;
+        r.logU = (U == 0.0) ? LOGU_ZERO : log(U);
+        rec[c] = r;
+    } else {
+        SlotRec2 r;
+        r.ij = i | (j << 16);
+        r.backmask = bm;
+        r.lu_next = __float_as_uint((float)((U == 0.0) ? LOGU_ZERO : log(U)));
+        r.k = k;
+        rec[c] = r;
+    }
 }

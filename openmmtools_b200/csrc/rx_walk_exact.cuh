@@ -1,6 +1,6 @@
-// rx_walk_exact.cuh -- the exact speculative swap-all walker (included by rx_mix.cu after rx_walk2.cuh).  One body, two
+// rx_walk_exact.cuh -- the exact speculative swap-all walker (included by rx_mix.cu after rx_walk2c.cuh).  One body, two
 // coordinate systems: k_mix_walk_pow2 walks SLOTS (K a power of two <= 16384: every attempt starts on an even word),
-// k_mix_walk_any walks WORD positions (any other K <= 4095).
+// k_mix_walk_cand walks CANDIDATE indices (any other K <= ANY_MAX_K, rx_walk2c.cuh).
 //
 // One warp walks (a second one only helps with the prologue).  The records come from DRAM (written once by the pre-pass,
 // read once) into a 1024-entry shared-memory ring by cp.async that the walker issues itself, 640 records ahead.  Per round
@@ -12,15 +12,11 @@
 //
 // Slots (SlotRec, or SlotRec2 in filter mode): the visited chain from slot s goes on at s+1 if log_p >= 0 (no uniform
 // drawn) else at s+2, resolved with a carry-propagation bit trick.
-// Words: for K that is not a power of two numba's randint rejects words (numba/_random.c: low bit_length(K-1) bits of one
-// word, retried while >= K), so an attempt has no fixed length and no slot grid exists.  What stays true is that the words an
-// attempt STARTING at word position p would consume for its two indices depend on the stream alone: a parallel pre-pass
-// turns every position into a WordRec {i, j, len, back-mask, log of the uniform at p + len}, the window is 32 consecutive
-// positions evaluated as if an attempt started at each of them, and the chain
-//     next(p) = p + len(p) + (log_p(p) < 0 ? 2 : 0)
-// is followed by pointer jumping over the lanes (four doublings: a hop is at least two words, so at most 16 positions of
-// a window are visited).  The last < 80 words of a pass and the (astronomically rare) attempt whose indices need more than
-// ANY_SCAN words are left to k_mix_walk_serial.
+// Candidates (CandRec {i | j << 12 | k << 24, back-mask, f64 log U of the attempt}, k_cand_records<true>): the chain goes on
+// at c+2 if log_p >= 0, else at c+2+k, resolved by w2_chain_cand; a visited position whose hop would leave the window is a
+// forced stop that opens the next round, so a round advances by at most 32 records.  The pass starts at candidate 0; the
+// last < 35 candidates of a pass are left to k_mix_walk_serial, which continues from the word position reported in
+// ctl->head: the next attempt's first candidate, or the word after the last attempt if the budget ended in the walker.
 //
 // Where the energies live (FILTER):
 //   true    slots only, the tail of every pass of k_mix_walk2 (K <= 256, on its SlotRec2 records): shared memory holds a
@@ -29,7 +25,7 @@
 //           taken from the image, in f32, whenever it is more than eps away from both thresholds (log_p = 0 and
 //           log_p = log U); a round whose committed prefix contains an undecided lane is redone with the exact f64 values
 //           from L2.  The result is therefore still bit-identical.
-//   false   exact f64 values from L2 every round (K > 256, or any K with RX_NO_FILTER=1).
+//   false   exact f64 values from L2 every round (slots: K > 256, or any K with RX_NO_FILTER=1; every candidate walk).
 //
 // The walker's round is one dependent chain (~105 instructions); what shortens it: no f64 on the chain, no
 // data-dependent branch besides the loop's (one loop condition, predicated commit), no sub-word shared stores (a
@@ -38,75 +34,16 @@
 #pragma once
 
 #define RING 1024         // records in the shared-memory ring
-#define ANY_SCAN 40       // words scanned for the two indices of an attempt; P(more) < (1/2)^38 per attempt
-#define ANY_MAX_K 4095    // 12-bit indices in the record
 
-struct WordRec {          // 16 bytes, one per WORD position p: the attempt that would start there
-    uint32_t ijl;         // i | j << 12 | len << 24; len = words that hold the two indices (0: unknown, see ANY_SCAN)
-    uint32_t backmask;    // bit 31-b: the attempt at p-1-b shares a replica index with this one (or is unknown)
-    double logU;          // log of the uniform made of words p+len, p+len+1: this attempt's draw if log_p < 0
-};
-
-__global__ void __launch_bounds__(256) k_words_build(const uint32_t *__restrict__ words, long long nwords, int K, uint32_t mask,
-                                                     WordRec *__restrict__ rec) {
-    __shared__ uint32_t s_w[256 + 31 + ANY_SCAN + 2];   // words of positions p0-31 .. p0+255+ANY_SCAN+1
-    __shared__ uint32_t s_ijl[256 + 31];                 // records' first word for positions p0-31 .. p0+255
-    const long long p0 = (long long)blockIdx.x * 256;
-    const int t = threadIdx.x;
-    for (int q = t; q < 256 + 31 + ANY_SCAN + 2; q += 256) {
-        const long long p = p0 - 31 + q;
-        s_w[q] = (p >= 0 && p < nwords) ? words[p] : 0u;
-    }
-    __syncthreads();
-    for (int q = t; q < 256 + 31; q += 256) {
-        const long long p = p0 - 31 + q;
-        uint32_t ijl = 0;
-        if (p >= 0 && p < nwords) {
-            int found = 0;
-            uint32_t i = 0;
-            for (int k = 0; k < ANY_SCAN && p + k < nwords; k++) {
-                const uint32_t r = s_w[q + k] & mask;
-                if (r < (uint32_t)K) {
-                    if (found == 0) { i = r; found = 1; }
-                    else { ijl = i | (r << 12) | ((uint32_t)(k + 1) << 24); break; }
-                }
-            }
-        }
-        s_ijl[q] = ijl;
-    }
-    __syncthreads();
-    const long long p = p0 + t;
-    if (p >= nwords) return;
-    const int q = t + 31;
-    const uint32_t ijl = s_ijl[q];
-    const uint32_t i = ijl & 0xfffu, j = (ijl >> 12) & 0xfffu, len = ijl >> 24;
-    uint32_t bm = 0;
-#pragma unroll 4
-    for (int b = 0; b < 31; b++) {
-        const uint32_t o = s_ijl[q - 1 - b];
-        const uint32_t oi = o & 0xfffu, oj = (o >> 12) & 0xfffu;
-        const bool hit = (o >> 24) == 0u || oi == i || oi == j || oj == i || oj == j;
-        bm |= (hit ? 1u : 0u) << (31 - b);
-    }
-    WordRec r;
-    r.ijl = ijl;
-    r.backmask = bm;
-    double lu = 0.0;
-    if (len != 0u && p + len + 1 < nwords) {
-        const double U = mt_double(s_w[q + len], s_w[q + len + 1]);
-        lu = (U == 0.0) ? LOGU_ZERO : log(U);
-    }
-    r.logU = lu;
-    rec[p] = r;
-}
-
-// The walker.  WORDS = false: records [ctl->head, nrec) are slots; WORDS = true: word positions (ctl->head counts words).
-template <bool WORDS, bool FILTER>
-__device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const uint32_t *__restrict__ words, unsigned nrec,
-                                        const double *__restrict__ u, int K, int logK, int *__restrict__ perm_g,
-                                        uint32_t *__restrict__ commit_log, const unsigned char *__restrict__ filt,
-                                        const double *__restrict__ filt_rowabs, MixCtl *ctl) {
-    static_assert(!(WORDS && FILTER), "the row-image filter exists for slots only");
+// The walker.  CAND = false: records [ctl->head, nrec) are slots; CAND = true: candidate indices [0, nrec), cpos gives the
+// word position of every candidate (ctl->head counts words).
+template <bool CAND, bool FILTER>
+__device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const uint32_t *__restrict__ words,
+                                        const uint32_t *__restrict__ cpos, unsigned nrec, const double *__restrict__ u, int K,
+                                        int logK, int *__restrict__ perm_g, uint32_t *__restrict__ commit_log,
+                                        const unsigned char *__restrict__ filt, const double *__restrict__ filt_rowabs,
+                                        MixCtl *ctl) {
+    static_assert(!(CAND && FILTER), "the row-image filter of this walker exists for slots only");
     extern __shared__ double s_mix[];
     // layout: ring[RING] 16-byte records | diag[K] f64 | (rowabs[K]) | perm[K] i32 | (image: u16[K*K] + u8[K*K])
     uint4 *s_ring = (uint4 *)s_mix;
@@ -115,13 +52,13 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
     int *s_perm = (int *)(s_rowabs + (FILTER ? K : 0));
     unsigned char *s_q = (unsigned char *)(s_perm + K);   // 24-bit image: int16 high plane [K*K] then uint8 low plane [K*K]
     // row r, column c of the K x K matrices
-    auto at = [&](unsigned r, unsigned c) { return WORDS ? r * (unsigned)K + c : (r << logK) | c; };
+    auto at = [&](unsigned r, unsigned c) { return CAND ? r * (unsigned)K + c : (r << logK) | c; };
     // (the warp index through a shuffle: warp-uniform for the compiler, see k_mix_walk2)
     const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     for (int q = tid; q < K; q += 64) {
         const int st = perm_g[q];
         s_perm[q] = st;
-        s_diag[q] = u[WORDS ? (size_t)q * K + st : ((size_t)q << logK) + st];
+        s_diag[q] = u[CAND ? (size_t)q * K + st : ((size_t)q << logK) + st];
         // per-row share of the f64-rounding bound, f32 rounded up: 1.6e-14 (|row minimum| + 1/2)
         if (FILTER) ((float *)s_rowabs)[q] = __fmul_ru(1.6e-14f, __fadd_ru(__double2float_ru(filt_rowabs[q]), 0.5f));
     }
@@ -130,13 +67,14 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
         uint32_t *dst = (uint32_t *)s_q;
         for (int q = tid; q < (3 * K * K) / 4; q += 64) dst[q] = src[q];
     }
-    const unsigned head0 = (unsigned)ctl->head;
+    // slots: the pass continues at slot ctl->head; candidates: a pass starts at candidate 0 (word position ctl->head == 0)
+    const unsigned head0 = CAND ? 0u : (unsigned)ctl->head;
     __syncthreads();
     if (warp != 0) return;   // (the second warp only helps with the prologue)
 
-    // The records come into the ring by cp.async issued by the walker itself, 640 records ahead, topped up every 8 rounds
-    // (slots) or 4 rounds (words); completion is tracked by the hardware (cp.async.wait_group), the warp barrier at the end
-    // of a round makes the data visible to all lanes.  No second warp, no flags, no fences: nothing for racecheck to find.
+    // The records come into the ring by cp.async issued by the walker itself, 640 records ahead, topped up every 8 rounds;
+    // completion is tracked by the hardware (cp.async.wait_group), the warp barrier at the end of a round makes the data
+    // visible to all lanes.  No second warp, no flags, no fences: nothing for racecheck to find.
     // (32-bit shared address through a shuffle: it then lives in a register instead of being re-derived from SR_CgaCtaId
     // every round)
     const unsigned ring_addr = __shfl_sync(0xffffffffu, (unsigned)__cvta_generic_to_shared((const void *)s_ring), 0);
@@ -165,8 +103,9 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
     const unsigned short *s_qhi = (const unsigned short *)s_q;            // [K*K] sign, exponent, 7 mantissa bits
     const unsigned char *s_qlo = s_q + 2 * (size_t)K * K;                  // [K*K] next 8 mantissa bits
     unsigned wpos = (h + (unsigned)lane) & (RING - 1);   // this lane's ring entry
-    // words: the attempt at the window's first position has unknown indices -- k_mix_walk_serial takes over
-    bool give_up = false;
+    // candidates: the word after the last attempt, when the budget ends in the walker (the plain loop then has nothing to
+    // do, and the stream position must be the reference's)
+    [[maybe_unused]] unsigned end_word = 0;
     // One round.  TAIL = the launch's attempt budget may end inside the window (checked only in the last rounds).
     auto round = [&](auto tail_tag) {
         constexpr bool TAIL = decltype(tail_tag)::value;
@@ -174,15 +113,20 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
         const unsigned w = wpos;   // (h + lane) & (RING - 1), carried from round to round
         const uint4 rq = w2_lds128(ring_addr + (w << 4));
         const uint32_t backmask = rq.y;
-        unsigned i, j, len = 0;
-        if constexpr (WORDS) { i = rq.x & 0xfffu; j = (rq.x >> 12) & 0xfffu; len = rq.x >> 24; }
-        else { i = rq.x & 0xffffu; j = rq.x >> 16; }
-        const bool unknown = WORDS && len == 0u;
+        unsigned i, j;
+        [[maybe_unused]] unsigned K1 = 0, K2 = 0;   // candidates: ballots of the hop classes k == 1, k == 2 (state independent)
+        if constexpr (CAND) {
+            i = rq.x & 0xfffu; j = (rq.x >> 12) & 0xfffu;
+            K1 = __ballot_sync(0xffffffffu, (rq.x >> 24) == 1u);
+            K2 = __ballot_sync(0xffffffffu, (rq.x >> 24) == 2u);
+        } else {
+            i = rq.x & 0xffffu; j = rq.x >> 16;
+        }
         // f64 log of the uniform an attempt here would draw: for a slot it belongs to the NEXT slot (words z, w of its
-        // SlotRec), for a word position it is the record's own
+        // SlotRec), for a candidate index it is the record's own
         double logU = 0.0;
         if (!FILTER) {
-            const uint2 lw = WORDS ? make_uint2(rq.z, rq.w) : w2_lds64(ring_addr + (((w + 1) & (RING - 1)) << 4) + 8u);
+            const uint2 lw = CAND ? make_uint2(rq.z, rq.w) : w2_lds64(ring_addr + (((w + 1) & (RING - 1)) << 4) + 8u);
             logU = __hiloint2double((int)lw.y, (int)lw.x);
         }
         const int si = s_perm[i], sj = s_perm[j];
@@ -225,10 +169,10 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
             const double d = logp - logU;
             ge0 = logp >= 0.0;
             acc = ge0 || d > 1e-9;
-            const bool ambiguous = !ge0 && fabs(d) <= 1e-9 && !unknown;   // NaN compares false: rejected, like the reference
+            const bool ambiguous = !ge0 && fabs(d) <= 1e-9;   // NaN compares false: rejected, like the reference
             if (__any_sync(0xffffffffu, ambiguous)) {
                 if (ambiguous) {  // too close to call in the log domain: do exactly what the reference does
-                    const size_t a = WORDS ? (size_t)h + lane + len : 2 * (size_t)(h + lane + 1);   // the uniform's words
+                    const size_t a = CAND ? (size_t)cpos[h + lane + 1] + 1 : 2 * (size_t)(h + lane + 1);   // the uniform's words
                     acc = mt_double(words[a], words[a + 1]) < rx_exp_cr(logp);
                     slow++;
                 }
@@ -237,21 +181,12 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
         unsigned V, C, low, cm, n, advance;
         auto resolve = [&]() {
             unsigned full;   // how far the window advances if all of it commits
-            [[maybe_unused]] const unsigned G = WORDS ? 0u : __ballot_sync(0xffffffffu, ge0);   // (slots)
-            const unsigned A = __ballot_sync(0xffffffffu, acc && i != j && !unknown);   // accepted and really changing the permutation
-            if constexpr (WORDS) {
-                // Pointer jumping over the lanes: N = window position of the attempt after this one (>= 32: beyond the
-                // window), R = set of positions the chain from here visits; lane 0 holds the chain from h.
-                unsigned N = unknown ? 64u : (unsigned)lane + len + (ge0 ? 0u : 2u);
-                unsigned R = 1u << lane;
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    const unsigned src = N & 31u;
-                    const unsigned Rn = __shfl_sync(0xffffffffu, R, src), Nn = __shfl_sync(0xffffffffu, N, src);
-                    if (N < 32u) { R |= Rn; N = Nn; }
-                }
-                V = __shfl_sync(0xffffffffu, R, 0);
-                full = __shfl_sync(0xffffffffu, N, 0);
+            unsigned Cf = 0;   // candidates: forced stops, visited positions whose hop would leave the window
+            const unsigned G = __ballot_sync(0xffffffffu, ge0);
+            const unsigned A = __ballot_sync(0xffffffffu, acc && i != j);   // accepted and really changing the permutation
+            if constexpr (CAND) {
+                w2_chain_cand(G, K1, K2, V, Cf);
+                full = 32u;
             } else {
                 // Visited chain: from a visited slot s the next attempt starts at s+1 if log_p >= 0 (no uniform drawn) else
                 // at s+2.  skip[s+1] = NG[s] & ~skip[s]: inside a run of NG ones the skip flag alternates, so skip[s] =
@@ -270,7 +205,8 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
             // lane t is stale if an earlier visited state-changing swap in this window shares a replica with it
             unsigned earlier;   // bit 31-b: lane t-1-b is a visited state-changing swap (shl by 32 gives 0 for lane 0)
             asm("shl.b32 %0, %1, %2;" : "=r"(earlier) : "r"(VA), "r"(sh_amt));
-            C = __ballot_sync(0xffffffffu, (earlier & backmask) != 0u || unknown) & V;
+            // the stops: stale visited lanes and forced stops (never position 0)
+            C = (__ballot_sync(0xffffffffu, (earlier & backmask) != 0u) | Cf) & V;
             low = C & (0u - C);
             cm = V & (low - 1u);           // low == 0 -> all lanes
             n = __popc(cm);
@@ -295,7 +231,6 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
         } else {
             resolve();
         }
-        if (WORDS && (C & 1u)) { give_up = true; return; }   // (only an unknown position can stop the window's first attempt)
         if (TAIL && n > rem) {
             unsigned pos = 0;  // the first visited lane we must NOT run: the (rem+1)-th set bit of cm
             for (unsigned cnt = 0; pos < 32; pos++)
@@ -303,6 +238,12 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
             cm &= (1u << pos) - 1u;
             n = rem;
             advance = pos;
+        }
+        if constexpr (CAND) {
+            if (TAIL && n == rem) {   // the budget ends in this round: the word after its last attempt (i, j, uniform?)
+                const unsigned last = 31u - __clz(cm);
+                end_word = __shfl_sync(0xffffffffu, cpos[h + lane + 1] + (ge0 ? 1u : 3u), last);
+            }
         }
         // commit: everything is computed by every lane, only the stores are predicated (no divergent block); bit 31 marks
         // a logged attempt (the count kernel also reads the filter walkers' sparse log)
@@ -318,20 +259,18 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
         wpos = (wpos + advance) & (RING - 1);
         rem -= n;
         // Every R rounds top the ring up to 640 records ahead and wait for all copies but the ones just issued.  A round
-        // advances by at most 33 slots, or 31 + ANY_SCAN + 2 = 73 words.  The next R rounds read below h + 33 R + 32
-        // (slots) / h + 73 R + 32 (words); the copies already waited for were issued at the previous top-up, at most R
-        // rounds back, and reach h - 33 R + 640 / h - 73 R + 640.  So 2 R 33 + 32 <= 640 and 2 R 73 + 32 <= 640: R = 8 for
-        // slots (the next 8 rounds read below h + 296, the copies reach h + 376), R = 4 for words (below h + 324, h + 348).
-        if ((rounds & (WORDS ? 3u : 7u)) == 0u) { refill(h); w2_cp_async_wait<1>(); }
+        // advances by at most 33 slots or 32 candidates.  The next R rounds read below h + 33 R + 32; the copies already
+        // waited for were issued at the previous top-up, at most R rounds back, and reach h - 33 R + 640.  So
+        // 2 R 33 + 32 <= 640: R = 8 (the next 8 rounds read below h + 296, the copies reach h + 376).
+        if ((rounds & 7u) == 0u) { refill(h); w2_cp_async_wait<1>(); }
         __syncwarp();
     };
-    // a round may start while every attempt of its window has its records (slots: and the next slot's uniform), words: its
-    // index words and its uniform inside the pass
-    const unsigned span = WORDS ? 32u + ANY_SCAN + 2u : 33u;
-    while (rem > 0 && h + span <= nrec && !give_up) {
+    // a round may start while every attempt of its window has its record (slots: and the next slot's uniform)
+    const unsigned span = CAND ? 32u : 33u;
+    while (rem > 0 && h + span <= nrec) {
         if (rem >= 33) {
             // main loop: a round commits at most 32 attempts, so the budget cannot end inside it
-            do { round(std::false_type()); } while (rem >= 33u && h + span <= nrec && !give_up);
+            do { round(std::false_type()); } while (rem >= 33u && h + span <= nrec);
         } else {
             round(std::true_type());
         }
@@ -341,7 +280,8 @@ __device__ __forceinline__ void ex_walk(const uint4 *__restrict__ recs, const ui
     slow = __reduce_add_sync(0xffffffffu, slow);
     if (lane == 0) {
         const long long remaining = remaining0 - (long long)(rem0 - rem);
-        ctl->head = h;
+        if constexpr (!CAND) ctl->head = h;
+        else if (h > 0) ctl->head = rem ? (long long)cpos[h] : (long long)end_word;   // word position for the plain loop
         ctl->remaining = remaining;
         ctl->status = remaining > 0 ? 1 : 0;
         ctl->rounds += (int)rounds;
@@ -357,11 +297,14 @@ __global__ void __launch_bounds__(64) k_mix_walk_pow2(const SlotRec *__restrict_
                                                       int *__restrict__ perm_g, uint32_t *__restrict__ commit_log,
                                                       const unsigned char *__restrict__ filt,
                                                       const double *__restrict__ filt_rowabs, MixCtl *ctl) {
-    ex_walk<false, FILTER>((const uint4 *)rec, words, nslots, u, K, logK, perm_g, commit_log, filt, filt_rowabs, ctl);
+    ex_walk<false, FILTER>((const uint4 *)rec, words, nullptr, nslots, u, K, logK, perm_g, commit_log, filt, filt_rowabs, ctl);
 }
 
-__global__ void __launch_bounds__(64) k_mix_walk_any(const WordRec *__restrict__ rec, const uint32_t *__restrict__ words,
-                                                     unsigned nwords, const double *__restrict__ u, int K,
-                                                     int *__restrict__ perm_g, uint32_t *__restrict__ commit_log, MixCtl *ctl) {
-    ex_walk<true, false>((const uint4 *)rec, words, nwords, u, K, 0, perm_g, commit_log, nullptr, nullptr, ctl);
+__global__ void __launch_bounds__(64) k_mix_walk_cand(const CandRec *__restrict__ rec, const uint32_t *__restrict__ words,
+                                                      const uint32_t *__restrict__ cpos, const uint32_t *__restrict__ ncand_p,
+                                                      const double *__restrict__ u, int K, int *__restrict__ perm_g,
+                                                      uint32_t *__restrict__ commit_log, MixCtl *ctl) {
+    const unsigned ncand = *ncand_p;   // records exist for c < ncand - 3
+    ex_walk<true, false>((const uint4 *)rec, words, cpos, ncand >= 3u ? ncand - 3u : 0u, u, K, 0, perm_g, commit_log, nullptr,
+                         nullptr, ctl);
 }

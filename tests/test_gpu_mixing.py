@@ -89,19 +89,18 @@ def test_swap_all_full_size_vs_oracle(K, model, seed):
                                                 (65, 'flat', 65 ** 3, 34), (100, 'normal', 100 ** 3, 35),
                                                 (127, 'ladder', 500_000, 36), (129, 'normal', 500_000, 37),
                                                 (200, 'normal', 2_000_000, 38), (1000, 'flat', 1_000_000, 39)])
-@pytest.mark.parametrize('path', ['default', 'serial', 'words'])
+@pytest.mark.parametrize('path', ['default', 'serial', 'exact'])
 def test_swap_all_any_k_vs_oracle(monkeypatch, K, model, nswap, seed, path):
-    """K that is not a power of two.  default: the walk2 organisation in candidate coordinates (k_mix_walk2c, K <= 256) or the
-    walker over word positions (k_mix_walk_any: above 256, or everywhere with RX_WALK_ANY_V1=1 -- exact f64 values from
-    L2); with RX_WALK_SERIAL=1 the plain loop; three iterations each."""
+    """K that is not a power of two, walked in candidate coordinates.  default: the walk2 organisation (k_mix_walk2c, K <= 256)
+    or the exact walker (k_mix_walk_cand, exact f64 values from L2: above 256); exact: the exact walker at every K
+    (RX_NO_FILTER=1); serial: the plain loop (RX_WALK_SERIAL=1); three iterations each."""
     from oracle import oracle
     serial = path == 'serial'
     if serial:
         if nswap > 300_000: pytest.skip('the plain loop takes 0.6 us per attempt')
         monkeypatch.setenv('RX_WALK_SERIAL', '1')
-    if path == 'words':
-        if K > 256: pytest.skip('already the default above K = 256')
-        monkeypatch.setenv('RX_WALK_ANY_V1', '1')
+    if path == 'exact':
+        monkeypatch.setenv('RX_NO_FILTER', '1')
     u = energies(model, K, 777 + K)
     e = gpu_engine(0, K, K)
     e.set_energies(u)
@@ -131,10 +130,11 @@ def test_swap_all_any_k_vs_oracle(monkeypatch, K, model, nswap, seed, path):
     e.close()
 
 
-@pytest.mark.parametrize('K,kind', [(100, 'equal_rows'), (100, 'nonfinite'), (37, 'equal_rows')])
+@pytest.mark.parametrize('K,kind', [(100, 'equal_rows'), (100, 'nonfinite'), (37, 'equal_rows'), (300, 'equal_rows'),
+                                    (300, 'nonfinite')])
 def test_swap_all_any_k_hard_matrices(K, kind):
     """Identical rows (iteration 0 of a run whose replicas start from one configuration: every log_p is a rounding error
-    around 0) and non-finite entries."""
+    around 0) and non-finite entries; K = 300 puts them on the exact walker's guard band and NaN path."""
     from oracle import oracle
     rng = np.random.default_rng(5)
     if kind == 'equal_rows':

@@ -2,7 +2,7 @@
   python tools/ab_walk.py libA.so libB.so ...     each library runs in its own process (RX_B200_LIB, 'default' = the
   library of this tree), alternated AB_ROUNDS times (default 3).  Cases: K = 256 on the real alchemical-LJ energy matrix
   tools/data/u_lj_256.npy (K^3 attempts: k_mix_walk2 + k_mix_walk_pow2<true>), and the 'ladder' and 'flat' matrices of
-  tests/golden/energy_models.py with AB_NSWAP attempts (default 2 000 000) at K = 300, 500, 1000 (k_mix_walk_any),
+  tests/golden/energy_models.py with AB_NSWAP attempts (default 2 000 000) at K = 300, 500, 1000 (k_mix_walk_cand),
   512, 1024 (k_mix_walk_pow2<false>) and, with RX_NO_FILTER=1, K = 64 and 256 (k_mix_walk_pow2<false>).  AB_CASES
   (e.g. 'lj:256,ladder:300,flat:64:nofilter') selects cases.  Every case makes AB_REPS (default 3) calls in one engine and
   prints walker ms per call, the mix_stats of the last call and a permutation / count-matrix digest of every call: all

@@ -8,7 +8,7 @@ from openmmtools_b200 import testsystems, alchemy, states, mcmc, multistate, uni
 from openmmtools_b200._engine import Engine
 
 # mixing kernels: pow2 small, K=256 (row image, k_mix_walk2 + k_mix_walk_pow2<true> tail), K not a power of two (k_cand_* + k_mix_walk2c + plain tail;
-# above 256 k_words_build + k_mix_walk_any), neighbours
+# above 256 k_cand_records<true> + k_mix_walk_cand), neighbours
 for K, n in ((16, 4096), (256, 60000), (12, 1728), (100, 30000), (255, 20000), (300, 20000)):
     e = Engine(0, K, K)
     e.set_energies(energies('flat', K, 7)); e.set_replica_states(np.arange(K)); e.mix_seed(3, 0); e.mix_seed(4, 1)
