@@ -116,6 +116,20 @@ typedef struct {
 RX_API int rx_set_particles(rx_engine *h, const double *sigma, const double *epsilon, const double *mass,
                      const uint8_t *alchemical_mask);
 RX_API int rx_set_states(rx_engine *h, const rx_state_params *states /* [n_states] */);
+/* Two alchemical regions (RX_SYSTEM_LJ_ALCH).  Replaces AbsoluteAlchemicalFactory.create_alchemical_system with a list
+ * of two AlchemicalRegions and no alchemical_regions_interactions (alchemy.py:637-754, 1539-2038): region[i] is 0 for the
+ * environment, 1 or 2 for the atoms of the first or second region (their epsilons are zeroed in the NonbondedForce,
+ * :1903-1909); environment x region r pairs are soft-core sterics driven by region r's lambda_sterics<suffix>
+ * (:1774-1775, 1915), r x r pairs the same expression with lambda 1 unless annihilate_r (:1776-1777, 1919), and pairs
+ * across the two regions have no interaction (no force covers them, :1684-1685).  Both regions use the soft-core
+ * constants of rx_config (OpenMM keeps one value per global parameter name, :2009-2017); annihilate_1/annihilate_2
+ * replace rx_config.annihilate_sterics.  Call after rx_set_particles (which returns the engine to one region); the
+ * engine then runs the two-region kernel instantiations.
+ * rx_set_states_region2  lambda_sterics of the second region [n_states] (GlobalParameterState with a
+ *                        parameters_name_suffix, states.py:3276-3280, 3830-3898); rx_set_states resets it to 1, so call
+ *                        it after every rx_set_states.  rx_state_params.lambda_sterics is the first region's lambda. */
+RX_API int rx_set_alchemical_regions(rx_engine *h, const uint8_t *region /*[N]*/, int32_t annihilate_1, int32_t annihilate_2);
+RX_API int rx_set_states_region2(rx_engine *h, const double *lambda_sterics_2 /*[n_states]*/);
 /* RX_SYSTEM_MOLECULE: the particles and the force field at once (instead of rx_set_particles).
  * Replaces: the System built by AmberPrmtopFile.createSystem for AlanineDipeptideVacuum, testsystems.py:3375-3388.
  * RX_ERR_UNSUPPORTED (and no molecule set) when the term tables need more shared memory than a block of the device can
@@ -329,6 +343,10 @@ RX_API int rx_set_barostat(rx_engine *h, int32_t first, int32_t count, const rx_
 RX_API int rx_get_barostat(rx_engine *h, int32_t first, int32_t count, rx_barostat_state *state);
 RX_API int rx_compute_energies_at_npt(rx_engine *h, const rx_state_params *states, const double *pressure,
                                       const double *dispersion, int32_t n, double *u_out);
+/* rx_compute_energies_at (pressure = dispersion = NULL) or rx_compute_energies_at_npt with the second alchemical region's
+ * lambda_sterics [n] of those states (rx_set_alchemical_regions, rx_set_states_region2). */
+RX_API int rx_compute_energies_at_region2(rx_engine *h, const rx_state_params *states, const double *lambda_sterics_2,
+                                          const double *pressure, const double *dispersion, int32_t n, double *u_out);
 
 /* ---- multi-GPU ------------------------------------------------------------------------------------ */
 /* NCCL is loaded with dlopen(nccl_library_path).  Rank 0 creates an id (rx_comm_unique_id), the host code

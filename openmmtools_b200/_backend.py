@@ -68,15 +68,26 @@ def _softcore(r, sig, eps, lam, alpha, a, b, c):
     return lam ** a * 4.0 * eps * x * (x - 1.0)
 
 
-def alchemical_dispersion_correction(system, lambda_sterics):
+def alchemical_dispersion_correction(system, lambda_sterics, lambda_sterics_2=1.0):
     """CustomNonbondedForce long-range correction of the two soft-core forces (SURVEY.md Appendix A): for each
     class pair, count(pairs in the interaction group) * [int_rc^inf r^2 U dr + int_rs^rc r^2 U (1-S) dr], summed,
     divided by N(N+1)/2 and multiplied by 2 pi N^2 / V.  Depends on lambda (the cost the reference warns about,
-    alchemy.py:535-540)."""
+    alchemy.py:535-540).  With two alchemical regions the two forces of each region (environment = the atoms of
+    neither region, lambda_sterics of region 1, lambda_sterics_2 of region 2) are summed; no force covers the pairs
+    across the regions."""
     if system.kind != LJ or not system.is_alchemical or not system.alchemical_dispersion_correction:
         return 0.0
+    if getattr(system, 'alchemical_regions', None) is None:
+        return _region_dispersion_correction(system, system.alchemical_mask().astype(bool),
+                                             ~system.alchemical_mask().astype(bool), lambda_sterics, system.annihilate_sterics)
+    ids = system.alchemical_region_ids()
+    return sum(_region_dispersion_correction(system, ids == r + 1, ids == 0, lam, annihilate)
+               for r, (lam, (_, _, annihilate)) in enumerate(zip((lambda_sterics, lambda_sterics_2), system.alchemical_regions)))
+
+
+def _region_dispersion_correction(system, mask, env, lambda_sterics, annihilate_sterics):
+    """The corrections of one region's environment x region (`mask` x `env`) and region x region forces."""
     N = system.n_particles
-    mask = system.alchemical_mask().astype(bool)
     sig, eps = np.asarray(system.sigma), np.asarray(system.epsilon)
     rc, rs = system.cutoff, system.switching_distance
     alpha, a, b, c = system.softcore_alpha, system.softcore_a, system.softcore_b, system.softcore_c
@@ -92,13 +103,13 @@ def alchemical_dispersion_correction(system, lambda_sterics):
         return tail + sw
 
     total = 0.0
-    ca, ce = _classes(sig[mask], eps[mask]), _classes(sig[~mask], eps[~mask])
+    ca, ce = _classes(sig[mask], eps[mask]), _classes(sig[env], eps[env])
     # na_sterics: environment x alchemical (alchemy.py:1915)
     for (sa, ea), na in ca:
         for (se, ee), ne in ce:
             total += na * ne * integral(0.5 * (sa + se), np.sqrt(ea * ee), lambda_sterics)
     # aa_sterics: alchemical x alchemical, each unordered pair once, lambda fixed to 1 unless annihilating (:1919)
-    lam_aa = lambda_sterics if system.annihilate_sterics else 1.0
+    lam_aa = lambda_sterics if annihilate_sterics else 1.0
     for i in range(len(ca)):
         for j in range(i, len(ca)):
             (si, ei), ni = ca[i]
@@ -132,12 +143,19 @@ def engine_tables(thermodynamic_states):
     sys0 = check_compatible(thermodynamic_states)
     M = len(thermodynamic_states)
     T = np.zeros(M); lam = np.ones(M); off = np.zeros(M); hoK = np.zeros(M); hox0 = np.zeros((M, 3))
+    two = sys0.kind == LJ and sys0.alchemical_regions is not None
+    lam2 = np.ones(M) if two else None
     base_lrc = lj_dispersion_correction(sys0) if sys0.kind == LJ else 0.0
     cache = {}
     for l, s in enumerate(thermodynamic_states):
         p = s._engine_parameters()
         T[l] = p['temperature']
-        if sys0.kind == LJ:
+        if two:
+            lam[l], lam2[l] = region_lambdas(sys0, p)
+            if (lam[l], lam2[l]) not in cache:
+                cache[lam[l], lam2[l]] = alchemical_dispersion_correction(sys0, lam[l], lam2[l])
+            off[l] = base_lrc + cache[lam[l], lam2[l]]
+        elif sys0.kind == LJ:
             lam[l] = p['lambda_sterics'] if sys0.is_alchemical else 1.0
             if lam[l] not in cache:
                 cache[lam[l]] = alchemical_dispersion_correction(sys0, lam[l])
@@ -149,7 +167,15 @@ def engine_tables(thermodynamic_states):
             hoK[l] = so.ho_K
             hox0[l] = so.ho_x0
             off[l] = so.ho_U0
-    return sys0, dict(temperature=T, lambda_sterics=lam, energy_offset=off, ho_K=hoK, ho_x0=hox0)
+    tab = dict(temperature=T, lambda_sterics=lam, energy_offset=off, ho_K=hoK, ho_x0=hox0)
+    if two:
+        tab['lambda_sterics_2'] = lam2
+    return sys0, tab
+
+
+def region_lambdas(system, parameters):
+    """(lambda of region 1, lambda of region 2) of a two-region system from a state's _engine_parameters()."""
+    return tuple(float(parameters.get(n, system.global_parameters.get(n, 1.0))) for n in system.lambda_sterics_names())
 
 
 def pressure_tables(thermodynamic_states):
@@ -166,9 +192,12 @@ def pressure_tables(thermodynamic_states):
     cache = {}
     c = np.zeros(len(thermodynamic_states))
     for l, s in enumerate(thermodynamic_states):
-        lam = s._engine_parameters()['lambda_sterics'] if sys0.is_alchemical else 1.0
+        if sys0.alchemical_regions is not None:
+            lam = region_lambdas(sys0, s._engine_parameters())
+        else:
+            lam = (s._engine_parameters()['lambda_sterics'] if sys0.is_alchemical else 1.0,)
         if lam not in cache:
-            cache[lam] = (base + alchemical_dispersion_correction(sys0, lam)) * V0
+            cache[lam] = (base + alchemical_dispersion_correction(sys0, *lam)) * V0
         c[l] = cache[lam]
     return p, c
 
@@ -203,6 +232,8 @@ def build_engine(thermodynamic_states, n_replicas, device=0, rank=0, world_size=
                      softcore_alpha=sys0.softcore_alpha, softcore_a=sys0.softcore_a, softcore_b=sys0.softcore_b,
                      softcore_c=sys0.softcore_c)
         eng.set_particles(sys0.sigma, sys0.epsilon, sys0.masses, sys0.alchemical_mask())
+        if sys0.alchemical_regions is not None:
+            eng.set_alchemical_regions(sys0.alchemical_region_ids(), *[a for _, _, a in sys0.alchemical_regions])
     elif sys0.kind == MOLECULE:
         if N > 32:
             raise NotImplementedError('molecules above 32 atoms are not provided (one lane per atom): %d atoms' % N)

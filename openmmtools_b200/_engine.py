@@ -72,6 +72,7 @@ class Engine:
         epsilon = None if epsilon is None else _c64(epsilon, (self.N,))
         mask = None if alchemical_mask is None else np.ascontiguousarray(alchemical_mask, dtype=np.uint8)
         self._check(self._lib.rx_set_particles(self._h, _ptr(sigma), _ptr(epsilon), _ptr(mass), _ptr(mask)))
+        self._two_regions = False
 
     @staticmethod
     def _state_table(temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None):
@@ -87,20 +88,48 @@ class Engine:
                 arr[l].ho_x0[q] = float(x0[q])
         return arr
 
-    def set_states(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None):
+    def set_states(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None, lambda_sterics_2=None):
+        """lambda_sterics_2: the second alchemical region's lambda of every state (rx_set_states_region2)."""
         if len(temperature) != self.M:
             raise ValueError('expected %d states' % self.M)
+        self._check_region2(lambda_sterics_2)
         arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0)
         self._check(self._lib.rx_set_states(self._h, C.cast(arr, C.c_void_p)))
+        if lambda_sterics_2 is not None:
+            self._check(self._lib.rx_set_states_region2(self._h, _ptr(_c64(lambda_sterics_2, (self.M,)))))
+
+    def _check_region2(self, lambda_sterics_2):
+        # a two-region engine takes the second region's lambdas with every state table (the C layer would take 1)
+        two = getattr(self, '_two_regions', False)
+        if two and lambda_sterics_2 is None:
+            raise ValueError('a two-region engine needs lambda_sterics_2 with every state table')
+        if not two and lambda_sterics_2 is not None:
+            raise ValueError('lambda_sterics_2 needs an engine with two alchemical regions (set_alchemical_regions)')
+
+    def set_alchemical_regions(self, region, annihilate_1, annihilate_2):
+        """Two alchemical regions: region[i] = 0 (environment), 1 or 2, and each region's annihilate_sterics
+        (rx_set_alchemical_regions; after set_particles)."""
+        r = np.ascontiguousarray(region, dtype=np.uint8)
+        if r.shape != (self.N,):
+            raise ValueError('expected %d region ids' % self.N)
+        self._check(self._lib.rx_set_alchemical_regions(self._h, _ptr(r), int(bool(annihilate_1)), int(bool(annihilate_2))))
+        self._two_regions = True
 
     def compute_energies_at(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None, pressure=None,
-                            dispersion=None):
+                            dispersion=None, lambda_sterics_2=None):
         """u[K][n] of every replica at n other states (unsampled states); the resident matrix is untouched.  An NPT engine
-        takes those states' pressures (kJ/mol/nm^3) and dispersion coefficients (kJ/mol nm^3) as well."""
+        takes those states' pressures (kJ/mol/nm^3) and dispersion coefficients (kJ/mol nm^3) as well; a two-region engine
+        their second-region lambdas."""
+        self._check_region2(lambda_sterics_2)
         arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0)
         n = len(temperature)
         out = np.zeros((self.K, n))
-        if pressure is None:
+        if lambda_sterics_2 is not None:
+            l2 = _c64(lambda_sterics_2, (n,))
+            p, c = (None, None) if pressure is None else (_c64(pressure, (n,)), _c64(dispersion, (n,)))
+            self._check(self._lib.rx_compute_energies_at_region2(self._h, C.cast(arr, C.c_void_p), _ptr(l2), _ptr(p), _ptr(c), n,
+                                                                 _ptr(out)))
+        elif pressure is None:
             self._check(self._lib.rx_compute_energies_at(self._h, C.cast(arr, C.c_void_p), n, _ptr(out)))
         else:
             p, c = _c64(pressure, (n,)), _c64(dispersion, (n,))

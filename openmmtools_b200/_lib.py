@@ -23,6 +23,7 @@ SYMBOLS = [
     'rx_mix_skip', 'rx_mix_swap_all', 'rx_mix_swap_neighbors', 'rx_get_mix_counts', 'rx_mix_stream_position',
     'rx_run_iterations', 'rx_sams_set', 'rx_sams_step', 'rx_sams_get', 'rx_sams_run_iterations', 'rx_get_phase_times', 'rx_timer_mark', 'rx_timer_elapsed', 'rx_get_mix_stats', 'rx_selftest_exp', 'rx_plan_propagate', 'rx_comm_unique_id', 'rx_comm_init',
     'rx_set_pressures', 'rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat', 'rx_compute_energies_at_npt',
+    'rx_set_alchemical_regions', 'rx_set_states_region2', 'rx_compute_energies_at_region2',
 ]
 
 
@@ -138,6 +139,9 @@ def load():
     lib.rx_comm_init.argtypes = [vp, C.c_char_p, vp]
     lib.rx_set_pressures.argtypes = [vp, vp, vp]
     lib.rx_compute_energies_at_npt.argtypes = [vp, vp, vp, vp, i32, vp]
+    lib.rx_set_alchemical_regions.argtypes = [vp, vp, i32, i32]
+    lib.rx_set_states_region2.argtypes = [vp, vp]
+    lib.rx_compute_energies_at_region2.argtypes = [vp, vp, vp, vp, vp, i32, vp]
     for name in ('rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat'):
         getattr(lib, name).argtypes = [vp, i32, i32, vp]
     if lib.rx_abi_version() != RX_ABI_VERSION:

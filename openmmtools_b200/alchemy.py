@@ -7,7 +7,23 @@ fluid (:1539-2038) is restated as parameters of the CUDA energy function: non-al
 (NonbondedForce with the alchemical epsilons zeroed, :1903-1909), alchemical/non-alchemical pairs use soft-core
 sterics controlled by ``lambda_sterics`` (:1383-1388, interaction group :1915), alchemical/alchemical pairs use
 the same expression with lambda fixed to 1 unless ``annihilate_sterics`` (:1776-1777, group :1919).  Bonded,
-electrostatic, GB and multi-region branches need a molecular force field and are out of scope.
+electrostatic and GB branches need a molecular force field and are out of scope.
+
+Two alchemical regions (a list of two ``AlchemicalRegion``, e.g. ``name=None`` or ``'A'`` plus ``'B'``) are the
+dual-topology / separated-topology set-up: the epsilons of both regions are zeroed in the NonbondedForce, each region r
+gets its own environment x r and r x r groups driven by ``lambda_sterics<suffix_r>`` (suffix ``'_' + name``, or none for
+``name=None``; :1695-1700, 1752-1777), and pairs across the two regions have no interaction (no
+``alchemical_regions_interactions``, :1684-1685).  Control them with one ``AlchemicalState`` per region, built with
+``parameters_name_suffix``::
+
+    regions = [AlchemicalRegion(alchemical_atoms=range(5), name='A'),
+               AlchemicalRegion(alchemical_atoms=range(5, 10), name='B', annihilate_sterics=True)]
+    system = AbsoluteAlchemicalFactory().create_alchemical_system(fluid.system, regions)
+    state_a = AlchemicalState.from_system(system, parameters_name_suffix='A')
+    state_b = AlchemicalState.from_system(system, parameters_name_suffix='B')
+
+Up to two regions; both must use the same soft-core constants (OpenMM keeps one value per global parameter name,
+:2009-2017), their ``annihilate_sterics`` may differ.
 """
 import collections
 from . import unit
@@ -54,6 +70,8 @@ _AR_FIELDS = ['alchemical_atoms', 'alchemical_bonds', 'alchemical_angles', 'alch
 AlchemicalRegion = collections.namedtuple('AlchemicalRegion', _AR_FIELDS)
 # defaults as alchemy.py:417-427
 AlchemicalRegion.__new__.__defaults__ = (None, None, None, None, True, False, 0.5, 1, 1, 6, 0.0, 1, 1, 2, None)
+_SOFTCORE_FIELDS = ('softcore_alpha', 'softcore_a', 'softcore_b', 'softcore_c', 'softcore_beta', 'softcore_d',
+                    'softcore_e', 'softcore_f')
 
 
 class AbsoluteAlchemicalFactory:
@@ -70,27 +88,46 @@ class AbsoluteAlchemicalFactory:
         self.split_alchemical_forces = split_alchemical_forces
 
     def create_alchemical_system(self, reference_system, alchemical_regions, alchemical_regions_interactions=frozenset()):
+        if alchemical_regions_interactions != frozenset():       # alchemy.py:661-662
+            raise NotImplementedError('Interactions between alchemical regions is untested')
         if not isinstance(reference_system, System) or reference_system.kind != LJ:
             raise NotImplementedError('only the Lennard-Jones test system can be alchemically modified on this path')
-        if isinstance(alchemical_regions, (list, tuple)) and not isinstance(alchemical_regions, AlchemicalRegion):
-            if len(alchemical_regions) != 1:
-                raise NotImplementedError('multiple alchemical regions are not provided')
-            alchemical_regions = alchemical_regions[0]
-        region = alchemical_regions
-        if region.alchemical_atoms is None or len(list(region.alchemical_atoms)) == 0:
-            raise ValueError('alchemical_atoms must be specified')     # alchemy.py:835
-        atoms = sorted(set(int(a) for a in region.alchemical_atoms))
+        if isinstance(alchemical_regions, AlchemicalRegion):
+            alchemical_regions = [alchemical_regions]
+        regions = list(alchemical_regions)
+        if len(regions) == 0:
+            raise ValueError('alchemical_atoms must be specified')
+        if len(regions) > 2:
+            raise NotImplementedError('more than two alchemical regions are not provided')
         n = reference_system.n_particles
-        if atoms[0] < 0 or atoms[-1] >= n:
-            raise ValueError('alchemical atom index out of range')
-        if any(x for x in (region.alchemical_bonds, region.alchemical_angles, region.alchemical_torsions)
-               if x not in (None, False, [], ())):
-            raise NotImplementedError('bonded alchemical terms are outside the hot path (the LJ fluid has none)')
+        region_atoms = []
+        for region in regions:
+            if region.alchemical_atoms is None or len(list(region.alchemical_atoms)) == 0:
+                raise ValueError('alchemical_atoms must be specified')     # alchemy.py:835
+            atoms = sorted(set(int(a) for a in region.alchemical_atoms))
+            if atoms[0] < 0 or atoms[-1] >= n:
+                raise ValueError('alchemical atom index out of range')
+            if any(x for x in (region.alchemical_bonds, region.alchemical_angles, region.alchemical_torsions)
+                   if x not in (None, False, [], ())):
+                raise NotImplementedError('bonded alchemical terms are outside the hot path (the LJ fluid has none)')
+            region_atoms.append(atoms)
+        if len(regions) == 2:
+            if set(region_atoms[0]) & set(region_atoms[1]):                 # alchemy.py:674-689
+                raise ValueError('Two regions have duplicate atoms.')
+            if regions[0].name == regions[1].name:                          # alchemy.py:691-694
+                raise ValueError('Two alchemical regions have the same name')
+            if any(getattr(regions[0], f) != getattr(regions[1], f) for f in _SOFTCORE_FIELDS):
+                raise NotImplementedError('the alchemical regions must share their soft-core constants (one value per '
+                                          'global parameter name, alchemy.py:2009-2017)')
+        region = regions[0]
         if reference_system.is_alchemical:
             raise ValueError('the system is already alchemically modified')
         system = reference_system.copy()
-        system.alchemical_atoms = tuple(atoms)
+        system.alchemical_atoms = tuple(sorted(a for atoms in region_atoms for a in atoms))
         system.annihilate_sterics = bool(region.annihilate_sterics)
+        if len(regions) == 2:
+            system.alchemical_regions = tuple((r.name, tuple(atoms), bool(r.annihilate_sterics))
+                                              for r, atoms in zip(regions, region_atoms))
         system.softcore_alpha = float(region.softcore_alpha)
         system.softcore_a = float(region.softcore_a)
         system.softcore_b = float(region.softcore_b)
@@ -101,8 +138,10 @@ class AbsoluteAlchemicalFactory:
         # lambda_electrostatics is defined by the factory even for zero charges (the electrostatic forces exist but
         # are identically zero), so AlchemicalState.from_system finds both parameters
         system.global_parameters = dict(reference_system.global_parameters)
-        system.global_parameters['lambda_sterics'] = 1.0
-        system.global_parameters['lambda_electrostatics'] = 1.0
+        for r in regions:
+            suffix = '' if r.name is None else '_' + r.name                  # alchemy.py:1695-1700
+            system.global_parameters['lambda_sterics' + suffix] = 1.0
+            system.global_parameters['lambda_electrostatics' + suffix] = 1.0
         return system
 
     @staticmethod

@@ -11,7 +11,9 @@ that holds a zero-charge Lennard-Jones ``NonbondedForce`` (``testsystems.Lennard
     :1915, controlled by the global ``lambda_sterics``) and alchemical x alchemical (:1919; its expression has
     ``lambda_sterics = 1`` baked in unless ``annihilate_sterics``, :1776-1777).  Per-particle parameters are (sigma,
     epsilon); the globals ``softcore_alpha/a/b/c`` are the region's soft-core constants (:1383-1388);
-  * electrostatic forces exist but are identically zero for the LJ fluid and are ignored (non-zero charges are refused).
+  * electrostatic forces exist but are identically zero for the LJ fluid and are ignored (non-zero charges are refused);
+  * with two alchemical regions each region has its own pair of soft-core forces, driven by ``lambda_sterics<suffix>``
+    (:1695-1777), and no force covers the pairs across the regions; the record then carries ``alchemical_regions``.
 
 and returns the :class:`openmmtools_b200.system.System` record the engine consumes.  ``create_engine_from_openmm`` goes
 on to a configured :class:`Engine`; ``B200ReplicaExchangeSampler`` is the drop-in sampler fed with reference-side
@@ -123,7 +125,18 @@ def system_from_openmm(system, forces=None):
     if not steric:
         out.sigma, out.epsilon = sigma, eps
         return out
-    atoms, annihilate, soft = None, None, None
+    # One environment x region force and one region x region force per region (alchemy.py:1752-1777, 1915-1919), in the
+    # order of the regions; a region's lambda is the global lambda_sterics<suffix> of its environment x region force.
+    regions, soft = [], None      # regions: [atoms, lambda name or None, annihilate]
+    def region_of(atoms):
+        for r in regions:
+            if r[0] == atoms:
+                return r
+        if any(r[0] & atoms for r in regions):
+            raise NotImplementedError('the soft-core forces disagree on the alchemical atoms')
+        regions.append([atoms, None, None])
+        return regions[-1]
+    lambdas = lambda g: [k for k in g if re.fullmatch(r'lambda_sterics(_.+)?', k)]
     for f in steric:
         groups = _interaction_groups(f)
         if len(groups) != 1:
@@ -134,38 +147,67 @@ def system_from_openmm(system, forces=None):
         if soft is not None and sc != soft:
             raise NotImplementedError('the soft-core forces disagree on the soft-core constants')
         soft = sc
-        if a == b:          # alchemical x alchemical (alchemy.py:1919): lambda is a free global only when annihilating
-            atoms_aa = a
-            annihilate = 'lambda_sterics' in g and not re.search(r'lambda_sterics\s*=\s*1(\.0*)?\s*;', _expression(f))
-            atoms = atoms_aa if atoms is None else atoms
-            if atoms != atoms_aa:
-                raise NotImplementedError('the soft-core forces disagree on the alchemical atoms')
-        else:               # alchemical x environment (alchemy.py:1915)
-            alch = a if len(a) <= len(b) and not (a & b) else b
+        if a == b:          # region x region (alchemy.py:1919): lambda is a free global only when annihilating
+            r = region_of(a)
+            names = lambdas(g)
+            r[2] = bool(names) and not re.search(re.escape(names[0]) + r'\s*=\s*1(\.0*)?\s*;', _expression(f))
+        else:               # region x environment (alchemy.py:1915)
             if a & b:
                 raise NotImplementedError('overlapping interaction groups')
-            atoms = alch if atoms is None else atoms
-            if atoms != alch:
-                raise NotImplementedError('the soft-core forces disagree on the alchemical atoms')
+            r = region_of(a if len(a) <= len(b) else b)
+            names = lambdas(g)
+            if len(names) != 1:
+                raise NotImplementedError('an environment x region soft-core force needs one lambda_sterics parameter')
+            r[1] = names[0]
         # the original sigma / epsilon of the alchemical atoms live in the custom force (zeroed in the NonbondedForce)
-        for i in sorted(atoms):
+        for i in sorted(r[0]):
             p = _particle_parameters(f, i)
             sigma[i], eps[i] = float(_md(p[0])), float(_md(p[1]))
+    if len(regions) > 2:
+        raise NotImplementedError('more than two alchemical regions are not provided')
+    names = [r[1] or 'lambda_sterics' for r in regions]
+    if len(set(names)) != len(names):
+        raise NotImplementedError('two alchemical regions with the same lambda_sterics parameter')
     out.sigma, out.epsilon = sigma, eps
-    out.alchemical_atoms = tuple(sorted(int(i) for i in atoms))
-    out.annihilate_sterics = bool(annihilate) if annihilate is not None else False
+    out.alchemical_atoms = tuple(sorted(int(i) for r in regions for i in r[0]))
+    out.annihilate_sterics = bool(regions[0][2])
     out.softcore_alpha, out.softcore_a, out.softcore_b, out.softcore_c = soft
     lrc = [bool(f.getUseLongRangeCorrection()) if hasattr(f, 'getUseLongRangeCorrection') else bool(getattr(f, 'lrc', False)) for f in steric]
     out.alchemical_dispersion_correction = any(lrc)
-    out.global_parameters = {'lambda_sterics': 1.0, 'lambda_electrostatics': 1.0}
+    if len(regions) == 1:
+        out.global_parameters = {'lambda_sterics': 1.0, 'lambda_electrostatics': 1.0}
+        return out
+    out.alchemical_regions = tuple((None if n == 'lambda_sterics' else n[len('lambda_sterics_'):],
+                                    tuple(sorted(int(i) for i in r[0])), bool(r[2])) for n, r in zip(names, regions))
+    out.global_parameters = {}
+    for n in names:
+        out.global_parameters[n] = 1.0
+        out.global_parameters[n.replace('sterics', 'electrostatics')] = 1.0
     return out
 
 
-def thermodynamic_states_from_openmm(system_record, temperatures, lambda_sterics=None):
+def thermodynamic_states_from_openmm(system_record, temperatures, lambda_sterics=None, lambda_sterics_2=None):
     """Our ThermodynamicState objects (one per state) for the record: temperatures in kelvin (numbers or quantities), and
-    for an alchemical record the lambda_sterics of every state."""
+    for an alchemical record the lambda_sterics of every state (with two regions: of the first region, and
+    ``lambda_sterics_2`` of the second)."""
     from .. import states, alchemy
     temps = [float(_md(t)) for t in temperatures]
+    if system_record.alchemical_regions is not None:
+        if lambda_sterics is None or lambda_sterics_2 is None or not (len(lambda_sterics) == len(lambda_sterics_2) == len(temps)):
+            raise ValueError('one lambda_sterics and one lambda_sterics_2 per state are needed for two alchemical regions')
+        out = []
+        for T, lams in zip(temps, zip(lambda_sterics, lambda_sterics_2)):
+            comp = []
+            for (name, _, _), lam in zip(system_record.alchemical_regions, lams):
+                a = alchemy.AlchemicalState.from_system(system_record, parameters_name_suffix=name)
+                sfx = '' if name is None else '_' + name
+                setattr(a, 'lambda_sterics' + sfx, float(lam))
+                setattr(a, 'lambda_electrostatics' + sfx, float(lam))
+                comp.append(a)
+            out.append(states.CompoundThermodynamicState(states.ThermodynamicState(system_record, T * unit.kelvin), comp))
+        return out
+    if lambda_sterics_2 is not None:
+        raise ValueError('lambda_sterics_2 needs a system with two alchemical regions')
     if system_record.is_alchemical:
         if lambda_sterics is None or len(lambda_sterics) != len(temps):
             raise ValueError('one lambda_sterics per state is needed for an alchemical system')
@@ -180,11 +222,12 @@ def thermodynamic_states_from_openmm(system_record, temperatures, lambda_sterics
 
 
 def create_engine_from_openmm(system, temperatures, lambda_sterics=None, n_replicas=None, forces=None, device=0,
-                              rank=0, world_size=1):
+                              rank=0, world_size=1, lambda_sterics_2=None):
     """``rx_create`` + ``rx_set_particles`` + ``rx_set_states`` from OpenMM objects (INTEGRATION.md section 2): returns
-    ``(engine, system_record, thermodynamic_states)``; positions, integrator and the mixing seed are the caller's."""
+    ``(engine, system_record, thermodynamic_states)``; positions, integrator and the mixing seed are the caller's.
+    Two alchemical regions take the second region's lambdas as ``lambda_sterics_2``."""
     rec = system_from_openmm(system, forces)
-    tstates = thermodynamic_states_from_openmm(rec, temperatures, lambda_sterics)
+    tstates = thermodynamic_states_from_openmm(rec, temperatures, lambda_sterics, lambda_sterics_2)
     eng = _backend.build_engine(tstates, n_replicas or len(tstates), device=device, rank=rank, world_size=world_size)
     return eng, rec, tstates
 

@@ -145,6 +145,8 @@ extern "C" void rx_destroy(rx_engine *h) {
     (h)->err.clear();                             \
     RX_CHECK_CUDA(h, cudaSetDevice((h)->cfg.device))
 
+static int upload_atoms(rx_engine *h, const std::vector<int> &al);
+
 extern "C" int rx_set_particles(rx_engine *h, const double *sigma, const double *epsilon, const double *mass,
                                 const uint8_t *alch) {
     ENTER(h);
@@ -166,9 +168,20 @@ extern "C" int rx_set_particles(rx_engine *h, const double *sigma, const double 
         ad[i] = make_double4(s, e, m, isal ? 1.0 : 0.0);
         if (isal) al.push_back(i);
     }
+    h->have_particles = false;
+    h->two_regions = false;
+    h->annihilate_mask = 0;
+    h->h_atom = a;
+    h->h_atom_d = ad;
+    return upload_atoms(h, al);
+}
+
+// The atom tables of h_atom / h_atom_d, the list `al` of alchemical atoms and the pair scratch sized for it.
+static int upload_atoms(rx_engine *h, const std::vector<int> &al) {
+    const int N = h->cfg.n_atoms;
     h->n_alch = (int)al.size();
-    RX_CHECK_CUDA(h, cudaMemcpy(h->d_atom, a.data(), sizeof(float4) * N, cudaMemcpyHostToDevice));
-    RX_CHECK_CUDA(h, cudaMemcpy(h->d_atom_d, ad.data(), sizeof(double4) * N, cudaMemcpyHostToDevice));
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_atom, h->h_atom.data(), sizeof(float4) * N, cudaMemcpyHostToDevice));
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_atom_d, h->h_atom_d.data(), sizeof(double4) * N, cudaMemcpyHostToDevice));
     if (h->n_alch) RX_CHECK_CUDA(h, cudaMemcpy(h->d_alch_list, al.data(), sizeof(int) * h->n_alch, cudaMemcpyHostToDevice));
     // scratch for the lambda-controlled pair list of each owned replica
     long long cap = (long long)h->n_alch * (N - 1);
@@ -180,6 +193,27 @@ extern "C" int rx_set_particles(rx_engine *h, const double *sigma, const double 
     RX_CHECK_CUDA(h, cudaMalloc(&h->d_pairs, sizeof(double2) * (size_t)cap * (h->kloc > 0 ? h->kloc : 1)));
     h->have_particles = true;
     return RX_OK;
+}
+
+extern "C" int rx_set_alchemical_regions(rx_engine *h, const uint8_t *region, int32_t annihilate_1, int32_t annihilate_2) {
+    ENTER(h);
+    if (h->cfg.system_kind != RX_SYSTEM_LJ_ALCH) RX_FAIL(h, RX_ERR_INVALID, "rx_set_alchemical_regions: RX_SYSTEM_LJ_ALCH engines only");
+    if (!region) RX_FAIL(h, RX_ERR_INVALID, "rx_set_alchemical_regions: null");
+    if (h->h_atom.empty()) RX_FAIL(h, RX_ERR_INVALID, "rx_set_alchemical_regions: call rx_set_particles first");
+    const int N = h->cfg.n_atoms;
+    for (int i = 0; i < N; i++)
+        if (region[i] > 2) RX_FAIL(h, RX_ERR_INVALID, "rx_set_alchemical_regions: region ids are 0 (environment), 1 or 2");
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    std::vector<int> al;
+    for (int i = 0; i < N; i++) {
+        h->h_atom[i].w = (float)region[i];
+        h->h_atom_d[i].w = (double)region[i];
+        if (region[i]) al.push_back(i);
+    }
+    h->have_particles = false;
+    h->two_regions = true;
+    h->annihilate_mask = (annihilate_1 ? 1 : 0) | (annihilate_2 ? 2 : 0);
+    return upload_atoms(h, al);
 }
 
 extern "C" int rx_set_molecule(rx_engine *h, const rx_molecule *molecule) {
@@ -216,7 +250,36 @@ static int convert_states(rx_engine *h, const rx_state_params *s, int n, std::ve
         d.offset = s[l].energy_offset;
         d.ho_K = s[l].ho_K;
         for (int q = 0; q < 3; q++) d.ho_x0[q] = s[l].ho_x0[q];
+        d.lambda2 = 1.0; d.la2 = 1.0; d.ob2 = 0.0;
     }
+    return RX_OK;
+}
+
+// The second region's lambda_sterics of n converted states (`lambda2` may be NULL: 1 everywhere).
+static int convert_states_region2(rx_engine *h, const double *lambda2, int n, std::vector<StateDev> &out, const char *who) {
+    if (!lambda2) return RX_OK;
+    if (h->cfg.system_kind != RX_SYSTEM_LJ_ALCH) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": RX_SYSTEM_LJ_ALCH engines only");
+    for (int l = 0; l < n; l++) {
+        if (!(lambda2[l] >= 0.0 && lambda2[l] <= 1.0)) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": lambda_sterics must be in [0, 1]");
+        StateDev &d = out[l];
+        d.lambda2 = lambda2[l];
+        d.la2 = pow(lambda2[l], h->cfg.softcore_a);
+        d.ob2 = h->cfg.softcore_alpha * pow(1.0 - lambda2[l], h->cfg.softcore_b);
+    }
+    return RX_OK;
+}
+
+extern "C" int rx_set_states_region2(rx_engine *h, const double *lambda2) {
+    ENTER(h);
+    if (!lambda2) RX_FAIL(h, RX_ERR_INVALID, "rx_set_states_region2: null");
+    if (!h->have_states) RX_FAIL(h, RX_ERR_INVALID, "rx_set_states_region2: call rx_set_states first");
+    const int M = h->cfg.n_states;
+    std::vector<StateDev> tab = h->h_states;
+    int rc = convert_states_region2(h, lambda2, M, tab, "rx_set_states_region2");
+    if (rc) return rc;
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_states, tab.data(), sizeof(StateDev) * M, cudaMemcpyHostToDevice));
+    h->h_states = tab;
     return RX_OK;
 }
 
@@ -607,13 +670,15 @@ extern "C" int rx_get_energies(rx_engine *h, double *u) {
 }
 
 // Energies at n other states; pressure / dispersion (NPT engines only, else NULL) are those states' (p, c) tables.
-static int energies_at(rx_engine *h, const rx_state_params *st, const double *pressure, const double *dispersion, int32_t n,
-                       double *u_out, const char *who) {
+// lambda2 (NULL: 1) is those states' lambda of the second alchemical region.
+static int energies_at(rx_engine *h, const rx_state_params *st, const double *lambda2, const double *pressure,
+                       const double *dispersion, int32_t n, double *u_out, const char *who) {
     int rc = check_ready(h, who);
     if (rc) return rc;
     if (!st || !u_out || n < 1) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": bad arguments");
     std::vector<StateDev> hs;
     rc = convert_states(h, st, n, hs, who);
+    if (!rc) rc = convert_states_region2(h, lambda2, n, hs, who);
     if (rc) return rc;
     std::vector<double2> tab;
     if (pressure) {
@@ -653,14 +718,21 @@ static int energies_at(rx_engine *h, const rx_state_params *st, const double *pr
 
 extern "C" int rx_compute_energies_at(rx_engine *h, const rx_state_params *st, int32_t n, double *u_out) {
     ENTER(h);
-    return energies_at(h, st, nullptr, nullptr, n, u_out, "rx_compute_energies_at");
+    return energies_at(h, st, nullptr, nullptr, nullptr, n, u_out, "rx_compute_energies_at");
 }
 
 extern "C" int rx_compute_energies_at_npt(rx_engine *h, const rx_state_params *st, const double *pressure,
                                           const double *dispersion, int32_t n, double *u_out) {
     ENTER(h);
     if (!pressure || !dispersion) RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at_npt: null argument");
-    return energies_at(h, st, pressure, dispersion, n, u_out, "rx_compute_energies_at_npt");
+    return energies_at(h, st, nullptr, pressure, dispersion, n, u_out, "rx_compute_energies_at_npt");
+}
+
+extern "C" int rx_compute_energies_at_region2(rx_engine *h, const rx_state_params *st, const double *lambda2,
+                                              const double *pressure, const double *dispersion, int32_t n, double *u_out) {
+    ENTER(h);
+    if (!lambda2 || (!pressure) != (!dispersion)) RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at_region2: null argument");
+    return energies_at(h, st, lambda2, pressure, dispersion, n, u_out, "rx_compute_energies_at_region2");
 }
 
 extern "C" int rx_mix_seed(rx_engine *h, int32_t stream, uint32_t seed) {

@@ -175,11 +175,24 @@ struct PairCtx {
     float x, y, z, sig_i, se_i;
     bool alch_i;
     PairLam lam;
+    int reg_i;      // REG: region of atom i (0 environment, 1, 2)
+    PairLam lam2;   // REG: the second region's lambda factors
 };
 
+// Pair rule of two alchemical regions (alchemy.py:1752-1777, 1903-1919 with two regions and no
+// alchemical_regions_interactions): an environment-region pair is soft with that region's lambda, a same-region pair is
+// soft only when that region annihilates (bit r-1 of `annihilate`), a pair across the regions has no interaction (`across`:
+// the caller discards its terms, which are then exactly zero at any separation).  One formula for every pair kind.
+__device__ __forceinline__ bool region_pair(int annihilate, int ri, int rj, PairLam lam2, PairLam &lam, bool &across) {
+    const int rr = ri | rj;   // 0 environment, 1 or 2 one region, 3 across
+    if (rr >= 2) lam = lam2;
+    across = rr == 3;
+    return ri != rj || (((annihilate << 1) >> ri) & 1);
+}
+
 // One candidate pair with atom j (position records at pos_base; parameter records par_off bytes further, or with P8
-// 8-byte parameter records (sqrt_eps, alch) starting at the shared address par_off).
-template <bool C6, bool SW, bool ENERGY, bool P8 = false>
+// 8-byte parameter records (sqrt_eps, alch) starting at the shared address par_off).  REG: the records carry region ids.
+template <bool C6, bool SW, bool ENERGY, bool P8 = false, bool REG = false>
 __device__ __forceinline__ void pair_term(const DynParams &p, const PairCtx &c, unsigned pos_base, int par_off, unsigned j,
                                           float &ax, float &ay, float &az, float &en) {
     const unsigned aj = pos_base + 16u * j;
@@ -188,17 +201,24 @@ __device__ __forceinline__ void pair_term(const DynParams &p, const PairCtx &c, 
     const float r2 = image_r2(c.box, dx, dy, dz);
     if (r2 < c.rc2) {
         const float2 qj = lds_f2(P8 ? (unsigned)par_off + 8u * j : aj + (unsigned)par_off);
-        const bool alch_j = qj.y != 0.f;
-        const bool soft = (c.alch_i != alch_j) || (c.alch_i && alch_j && p.annihilate);
+        bool soft, across = false;
+        PairLam lam = c.lam;
+        if constexpr (REG) {
+            soft = region_pair(p.annihilate, c.reg_i, (int)qj.y, c.lam2, lam, across);
+        } else {
+            const bool alch_j = qj.y != 0.f;
+            soft = (c.alch_i != alch_j) || (c.alch_i && alch_j && p.annihilate);
+        }
         float e;
-        const float fr = lj_pair_f<C6, SW, ENERGY>(p, r2, 0.5f * (c.sig_i + pj.w), c.se_i * qj.x, soft, c.lam, e);
+        float fr = lj_pair_f<C6, SW, ENERGY>(p, r2, 0.5f * (c.sig_i + pj.w), c.se_i * qj.x, soft, lam, e);
+        if (REG && across) { fr = 0.f; e = 0.f; }
         ax += fr * dx; ay += fr * dy; az += fr * dz;
         if (ENERGY) en += 0.5f * e;
     }
 }
 
 // Force on one atom from the inner part of its neighbour list or, in the fallback, from all other atoms.
-template <bool C6, bool SW, bool ENERGY, bool P8 = false>
+template <bool C6, bool SW, bool ENERGY, bool P8 = false, bool REG = false>
 __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, unsigned pos_base, int par_off,
                                           unsigned nb_t, int N, int ncol, int a, bool use_list, int n_inner,
                                           float &fx, float &fy, float &fz, float &en) {
@@ -207,10 +227,10 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
         const unsigned stride = 2u * (unsigned)ncol;
         unsigned q = nb_t;
         for (int n = 0; n < n_inner; n++, q += stride)
-            pair_term<C6, SW, ENERGY, P8>(p, c, pos_base, par_off, lds_u16(q), ax, ay, az, e);
+            pair_term<C6, SW, ENERGY, P8, REG>(p, c, pos_base, par_off, lds_u16(q), ax, ay, az, e);
     } else {
         for (int j = 0; j < N; j++)
-            if (j != a) pair_term<C6, SW, ENERGY, P8>(p, c, pos_base, par_off, (unsigned)j, ax, ay, az, e);
+            if (j != a) pair_term<C6, SW, ENERGY, P8, REG>(p, c, pos_base, par_off, (unsigned)j, ax, ay, az, e);
     }
     fx = ax; fy = ay; fz = az; en = e;
 }
@@ -246,7 +266,9 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
 // parameter records (sqrt_eps, alch) -- sigma rides in the position's w -- so that 4096 atoms leave room for a list.
 // NPT: the box is the replica's (box[r], kept in f64 there) and a Monte Carlo barostat attempt opens every 25th step
 // (rx_b200.h, rx_set_pressures); npt[state] = (pressure, dispersion coefficient), min_edge = twice the cutoff.
-template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false, bool NPT = false>
+// REG: two alchemical regions (rx_set_alchemical_regions): the parameter records carry each atom's region id instead of the
+// alchemical flag and the pair rule is region_pair's.
+template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false, bool NPT = false, bool REG = false>
 __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *__restrict__ atom,
                                                     const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                     float4 *__restrict__ pos, float4 *__restrict__ vel, int k0,
@@ -311,9 +333,11 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     const float h_V = mv.dt / (float)mv.nV, h_R = mv.dt / (float)mv.nR;
     float sig_i, se_i, inv_m, sigma_v;
     bool alch_i;
+    int reg_i = 0;
     auto load_atom = [&]() {
         const float4 a4 = active ? atom[a] : make_float4(1.f, 0.f, 1.f, 0.f);
         sig_i = a4.x; se_i = a4.y; inv_m = a4.z; alch_i = a4.w != 0.f;
+        if constexpr (REG) reg_i = (int)a4.w;
         sigma_v = sqrtf((float)st.kT * inv_m);  // sqrt(kT/m), integrators.py:1314
     };
     load_atom();
@@ -326,8 +350,9 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     }
     for (int j = t; j < p.N; j += nthr) {   // parameter records of ALL atoms (the pair loop reads those of its partners)
         const float4 a4 = atom[j];
-        if (COMPACT) s_par8[j] = make_float2(a4.y, a4.w != 0.f ? 1.f : 0.f);
-        else s_par[j] = make_float4(a4.y, a4.w != 0.f ? 1.f : 0.f, 0.f, 0.f);
+        const float tag = REG ? a4.w : (a4.w != 0.f ? 1.f : 0.f);
+        if (COMPACT) s_par8[j] = make_float2(a4.y, tag);
+        else s_par[j] = make_float4(a4.y, tag, 0.f, 0.f);
     }
     if (CL > 1) cg::this_cluster().sync();   // every block of the cluster is resident and has cleared its vote words
     float fx = 0, fy = 0, fz = 0;
@@ -445,6 +470,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
     // reaches the pair loop) most NPT instantiations spill more (DESIGN 4.2).
     PairCtx pc;
     pc.box = bf; pc.rc2 = p.rc2; pc.lam = lam;
+    if constexpr (REG) pc.lam2 = {(float)st.la2, (float)st.ob2};
     const int N = p.N;
     // Publish the current positions and make the neighbour list valid for them: one barrier unless a list is rebuilt.
     auto publish = [&]() {
@@ -472,11 +498,12 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         if (!f_valid) publish();
         if (active) {
             pc.x = x; pc.y = y; pc.z = z; pc.sig_i = sig_i; pc.se_i = se_i; pc.alch_i = alch_i;
+            if constexpr (REG) pc.reg_i = reg_i;
             const unsigned pos_base = dyn_base + (cur ? 16u * (unsigned)pos1 : 0u);
             // (COMPACT: the address of the 8-byte records; otherwise the offset from either buffer to the 16-byte records)
             const int par_off = COMPACT ? (int)(dyn_base + 32u * (unsigned)N) : (cur ? -16 * RX_MAX_ATOMS : 16 * RX_MAX_ATOMS);
-            if (want_energy) lj_forces<C6, SW, true, COMPACT>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
-            else lj_forces<C6, SW, false, COMPACT>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
+            if (want_energy) lj_forces<C6, SW, true, COMPACT, REG>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
+            else lj_forces<C6, SW, false, COMPACT, REG>(p, pc, pos_base, par_off, nb_t, N, nthr, a, use_list, n_inner, fx, fy, fz, e_out);
         } else {
             fx = fy = fz = 0.f; e_out = 0.f;
         }
@@ -653,7 +680,9 @@ __device__ __forceinline__ double switch_d(const EnParams &p, double r) {
 }
 
 // NPT: the replica's box from box[r], and u[k][l] gains beta_l (c_l / V_k + p_l V_k), npt[l] = (p_l, c_l).
-template <bool NPT = false>
+// REG: two alchemical regions (atom_d[i].w is the region id; the pair rule of region_pair).  A lambda-controlled pair record
+// carries its region in the sign of its first word (negative: region 2; the word, (r/sigma)^c, is > 0).
+template <bool NPT = false, bool REG = false>
 __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *__restrict__ atom_d,
                                                      const int *__restrict__ alch_list,
                                                      const StateDev *__restrict__ states,
@@ -697,7 +726,13 @@ __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *
             int j = i + d; if (j >= p.N) j -= p.N;
             const double4 aj = atom_d[j];
             const bool alch_j = aj.w != 0.0;
-            const bool soft = (alch_i != alch_j) || (alch_i && alch_j && p.annihilate);
+            bool soft;
+            if constexpr (REG) {   // lambda-controlled or across the regions: not here
+                const int ri = (int)ai.w, rj = (int)aj.w;
+                soft = ri != rj || (((p.annihilate << 1) >> ri) & 1);
+            } else {
+                soft = (alch_i != alch_j) || (alch_i && alch_j && p.annihilate);
+            }
             if (soft) continue;
             const double dx = min_image_d(sx[i] - sx[j], p.Lx), dy = min_image_d(sy[i] - sy[j], p.Ly),
                          dz = min_image_d(sz[i] - sz[j], p.Lz);
@@ -735,7 +770,11 @@ __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *
                 if (j == a) continue;
                 const double4 pj = atom_d[j];
                 const bool alch_j = pj.w != 0.0;
-                if (alch_j && (!p.annihilate || j < a)) continue;  // A-A: only when annihilating, counted once
+                if constexpr (REG) {   // same region: only when that region annihilates, counted once; across: never
+                    if (alch_j && (pj.w != pa.w || !(((p.annihilate << 1) >> (int)pa.w) & 1) || j < a)) continue;
+                } else {
+                    if (alch_j && (!p.annihilate || j < a)) continue;  // A-A: only when annihilating, counted once
+                }
                 const double dx = min_image_d(sx[a] - sx[j], p.Lx), dy = min_image_d(sy[a] - sy[j], p.Ly),
                              dz = min_image_d(sz[a] - sz[j], p.Lz);
                 const double r2 = dx * dx + dy * dy + dz * dz;
@@ -746,7 +785,7 @@ __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *
                         const double sig = 0.5 * (pa.x + pj.x), eps = sqrt(pa.y * pj.y);
                         const double q = r2 / (sig * sig);
                         const double rsc = p.c_is_6 ? q * q * q : pow(q, 0.5 * p.sc_c);
-                        my_pairs[slot] = make_double2(rsc, 4.0 * eps * switch_d(p, sqrt(r2)));
+                        my_pairs[slot] = make_double2(REG && pa.w == 2.0 ? -rsc : rsc, 4.0 * eps * switch_d(p, sqrt(r2)));
                     }
                 }
                 cnt++;
@@ -764,9 +803,16 @@ __global__ void __launch_bounds__(512) k_energy_rows(EnParams p, const double4 *
         double Ua = 0.0;
         for (int q = 0; q < npairs; q++) {
             const double2 pr = my_pairs[q];
-            const double D = st.ob + pr.x;
-            const double x = p.c_is_6 ? 1.0 / D : pow(D, -6.0 / p.sc_c);
-            Ua += st.la * pr.y * x * (x - 1.0);
+            if constexpr (REG) {
+                const bool second = pr.x < 0.0;
+                const double D = (second ? st.ob2 : st.ob) + fabs(pr.x);
+                const double x = p.c_is_6 ? 1.0 / D : pow(D, -6.0 / p.sc_c);
+                Ua += (second ? st.la2 : st.la) * pr.y * x * (x - 1.0);
+            } else {
+                const double D = st.ob + pr.x;
+                const double x = p.c_is_6 ? 1.0 / D : pow(D, -6.0 / p.sc_c);
+                Ua += st.la * pr.y * x * (x - 1.0);
+            }
         }
         if constexpr (NPT) {
             const double V = p.Lx * p.Ly * p.Lz;
@@ -870,7 +916,7 @@ static int fill_dyn(rx_engine *h, DynParams &p, int reassign) {
     p.box = box_f(c.box[0], c.box[1], c.box[2]);
     p.rc2 = (float)(c.r_cutoff * c.r_cutoff); p.rs2 = (float)(c.r_switch * c.r_switch); p.rs = (float)c.r_switch;
     p.inv_w = (float)(1.0 / (c.r_cutoff - c.r_switch));
-    p.use_switch = c.use_switch; p.annihilate = c.annihilate_sterics;
+    p.use_switch = c.use_switch; p.annihilate = h->two_regions ? h->annihilate_mask : c.annihilate_sterics;
     p.c_is_6 = (c.softcore_c == 6.0); p.sc_c = (float)c.softcore_c;
     p.maxnb = 0; p.sort_atoms = 0; p.rl2 = p.rin2 = p.rc2; p.half_in2 = p.half_out2 = 0.f;
     p.move = make_move(h->dt, h->gamma, h->n_steps, h->program, reassign);
@@ -1111,11 +1157,13 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
     const bool found = with_flag(p.c_is_6, [&](auto c6) {
         return with_flag(p.use_switch, [&](auto sw) {
             return with_flag(npt, [&](auto np) {
-                return with_layout(PropagateLayouts{}, plan, per_state, rc, [&](auto L) {
-                    return launch_kernel(h, lc, smem > 48 * 1024, k_propagate<c6, sw, L.cl, L.ps, L.compact, np>, p, (const float4 *)h->d_atom,
-                                         (const StateDev *)h->d_states, (const int *)h->d_perm, h->d_pos, h->d_vel, h->k0, key,
-                                         it32, h->d_pot, h->d_kin, h->d_nan, d_only, (const MoveDev *)h->d_moves, h->d_box,
-                                         h->d_baro, (const double2 *)h->d_npt, min_edge);
+                return with_flag(h->two_regions, [&](auto rg) {
+                    return with_layout(PropagateLayouts{}, plan, per_state, rc, [&](auto L) {
+                        return launch_kernel(h, lc, smem > 48 * 1024, k_propagate<c6, sw, L.cl, L.ps, L.compact, np, rg>, p,
+                                             (const float4 *)h->d_atom, (const StateDev *)h->d_states, (const int *)h->d_perm,
+                                             h->d_pos, h->d_vel, h->k0, key, it32, h->d_pot, h->d_kin, h->d_nan, d_only,
+                                             (const MoveDev *)h->d_moves, h->d_box, h->d_baro, (const double2 *)h->d_npt, min_edge);
+                    });
                 });
             });
         });
@@ -1190,8 +1238,8 @@ int rxi_restore_failed(rx_engine *h) {
 // sums are added in that order, so the result does not depend on scheduling.  Shared memory: [stride] positions, then
 // [stride] parameter records, stride = RX_MAX_ATOMS (APT = 1) or N.
 // ---------------------------------------------------------------------------------------------------
-// NPT: every replica at its own box (box[r]).
-template <bool C6, bool SW, int APT, bool NPT = false>
+// NPT: every replica at its own box (box[r]).  REG: two alchemical regions, as in k_propagate.
+template <bool C6, bool SW, int APT, bool NPT = false, bool REG = false>
 __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__restrict__ atom,
                                                    const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                    float4 *__restrict__ pos, int k0, float tol_rms, int max_iter,
@@ -1214,13 +1262,15 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
         if (a < p.N) {
             const float4 a4 = atom[a], x4 = pos[(size_t)r * p.N + a];
             s_pos[a] = make_float4(x4.x, x4.y, x4.z, a4.x);
-            s_par[a] = make_float4(a4.y, a4.w != 0.f ? 1.f : 0.f, 0.f, 0.f);
+            s_par[a] = make_float4(a4.y, REG ? a4.w : (a4.w != 0.f ? 1.f : 0.f), 0.f, 0.f);
         }
     }
     __syncthreads();
     PairCtx pc;
     pc.box = bf; pc.rc2 = p.rc2;
     pc.lam = {(float)st.la, (float)st.ob};
+    if constexpr (REG) pc.lam2 = {(float)st.la2, (float)st.ob2};
+
     const unsigned pos_base = (unsigned)__cvta_generic_to_shared(s_dyn);
     const float hx0 = (float)st.ho_x0[0], hx1 = (float)st.ho_x0[1], hx2 = (float)st.ho_x0[2], hK = (float)st.ho_K;
     const float dt0 = 0.001f, dt_max = 0.010f, alpha0 = 0.1f, max_move = 0.01f;  // ps, ps, -, nm per step
@@ -1239,7 +1289,8 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
             else if (active) {
                 const float4 a4 = atom[a];
                 pc.x = xa.x; pc.y = xa.y; pc.z = xa.z; pc.sig_i = a4.x; pc.se_i = a4.y; pc.alch_i = a4.w != 0.f;
-                lj_forces<C6, SW, false>(p, pc, pos_base, 16 * stride, 0u, p.N, p.N, a, false, 0, gx, gy, gz, e);
+                if constexpr (REG) pc.reg_i = (int)a4.w;
+                lj_forces<C6, SW, false, false, REG>(p, pc, pos_base, 16 * stride, 0u, p.N, p.N, a, false, 0, gx, gy, gz, e);
             }
             if (!active) { gx = gy = gz = 0.f; }
             fx[u] = gx; fy[u] = gy; fz[u] = gz;
@@ -1337,9 +1388,11 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
         return with_flag(p.use_switch, [&](auto sw) {
             return with_flag(h->npt, [&](auto np) {
                 return with_flag(wide, [&](auto w) {
-                    return launch_kernel(h, lc, wide, k_minimize<c6, sw, w ? 4 : 1, np>, p, (const float4 *)h->d_atom,
-                                         (const StateDev *)h->d_states, (const int *)h->d_perm, h->d_pos, h->k0,
-                                         (float)tolerance, max_iterations, d_rms, d_iters, (const double4 *)h->d_box);
+                    return with_flag(h->two_regions, [&](auto rg) {
+                        return launch_kernel(h, lc, wide, k_minimize<c6, sw, w ? 4 : 1, np, rg>, p, (const float4 *)h->d_atom,
+                                             (const StateDev *)h->d_states, (const int *)h->d_perm, h->d_pos, h->k0,
+                                             (float)tolerance, max_iterations, d_rms, d_iters, (const double4 *)h->d_box);
+                    });
                 });
             });
         });
@@ -1398,7 +1451,9 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
         RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at: a constant-pressure engine needs the states' pressures (rx_compute_energies_at_npt)");
     if (!h->npt && d_npt_tab)
         RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at_npt: the engine has no pressure (rx_set_pressures)");
-    auto kern = h->npt ? k_energy_rows<true> : k_energy_rows<false>;
+    if (h->two_regions) p.annihilate = h->annihilate_mask;
+    auto kern = h->two_regions ? (h->npt ? k_energy_rows<true, true> : k_energy_rows<false, true>)
+                               : (h->npt ? k_energy_rows<true> : k_energy_rows<false>);
     const int rco = smem_opt_in(h, (const void *)kern, (int)smem);
     if (rco) return rco;
     kern<<<h->kloc, 512, smem, h->stream>>>(p, h->d_atom_d, h->d_alch_list, d_states, h->d_pos, h->k0,

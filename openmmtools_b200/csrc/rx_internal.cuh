@@ -20,6 +20,9 @@ struct StateDev {
     double offset;   // kJ/mol
     double ho_K;
     double ho_x0[3];
+    // the second alchemical region's lambda_sterics<suffix> and its two soft-core factors (rx_set_states_region2);
+    // read only by the two-region kernels
+    double lambda2, la2, ob2;
 };
 
 // ---- MT19937 stream resident on the device (numba's / numpy's generator restated) ---------------------
@@ -67,10 +70,16 @@ struct rx_engine {
     long long mix_stats[6] = {0, 0, 0, 0, 0, 0};   // rounds, exact-exp, passes, words, walker us, prepare-wait us
     cudaEvent_t ev_walk[2] = {};
     // particles
-    float4 *d_atom = nullptr;     // (sigma, sqrt_eps, inv_mass, alch ? 1 : 0)
-    double4 *d_atom_d = nullptr;  // (sigma, eps, mass, alch)
+    float4 *d_atom = nullptr;     // (sigma, sqrt_eps, inv_mass, alch ? 1 : 0), or the region id (0, 1, 2) with two regions
+    double4 *d_atom_d = nullptr;  // (sigma, eps, mass, alch or region id)
+    std::vector<float4> h_atom;   // host copies of both (rx_set_alchemical_regions rewrites their w)
+    std::vector<double4> h_atom_d;
     int n_alch = 0;
-    int *d_alch_list = nullptr;   // indices of the alchemical atoms
+    int *d_alch_list = nullptr;   // indices of the alchemical atoms (of either region)
+    // two alchemical regions (rx_set_alchemical_regions): the two-region kernel instantiations run, and their pair rules
+    // read the annihilate flags as bit 0 (region 1) and bit 1 (region 2) of DynParams / EnParams::annihilate
+    bool two_regions = false;
+    int annihilate_mask = 0;
     bool have_particles = false, have_states = false, have_integrator = false;
     StateDev *d_states = nullptr;
     std::vector<StateDev> h_states;

@@ -213,8 +213,12 @@ class ThermodynamicState:
     # -- engine-facing view of this state (overridden/extended by CompoundThermodynamicState)
     def _engine_parameters(self):
         s = self._standard_system
-        return dict(temperature=self._temperature, lambda_sterics=s.global_parameters.get('lambda_sterics', 1.0),
-                    ho_K=s.ho_K, ho_x0=s.ho_x0, ho_U0=s.ho_U0, pressure=self._pressure_md)
+        p = dict(temperature=self._temperature, lambda_sterics=s.global_parameters.get('lambda_sterics', 1.0),
+                 ho_K=s.ho_K, ho_x0=s.ho_x0, ho_U0=s.ho_U0, pressure=self._pressure_md)
+        if getattr(s, 'alchemical_regions', None) is not None:   # each region's lambda_sterics<suffix>
+            for n in s.lambda_sterics_names():
+                p[n] = s.global_parameters.get(n, 1.0)
+        return p
 
     # -- copies share the (immutable) standard system like the reference (states.py:1235-1253)
     def __copy__(self):
@@ -473,9 +477,11 @@ class GlobalParameterState:
         def __get__(self, instance, owner=None):
             if instance is None:
                 return self
+            self._check_controlled(instance)
             return instance._parameters[self.variable_name]
 
         def __set__(self, instance, new_value):
+            self._check_controlled(instance)
             if self.variable_name not in instance._parameters or instance._parameters[self.variable_name] is None:
                 if new_value is not None or self.variable_name not in instance._parameters:
                     raise GlobalParameterError(GlobalParameterError.PARAMETER_NOT_DEFINED,
@@ -488,24 +494,33 @@ class GlobalParameterState:
             self.validator_func = validator
             return validator
 
+        def _check_controlled(self, instance):
+            # a state with a parameter name suffix controls only the suffixed names (states.py:3469-3479)
+            suffix = instance.__dict__.get('_parameters_name_suffix')
+            if suffix is not None:
+                raise AttributeError('This state does not control {} but {}.'.format(
+                    self.variable_name, self.variable_name + '_' + suffix))
+
     def __init__(self, parameters_name_suffix=None, **kwargs):
         self._initialize(parameters_name_suffix=parameters_name_suffix, **kwargs)
 
     @classmethod
     def _get_controlled_parameters(cls, parameters_name_suffix=None):
+        """name (with '_' + parameters_name_suffix appended, if given) -> descriptor (states.py:3698-3730)."""
+        suffix = '' if parameters_name_suffix is None else '_' + parameters_name_suffix
         out = {}
         for klass in reversed(cls.__mro__):
             for name, d in vars(klass).items():
                 if isinstance(d, GlobalParameterState.GlobalParameter):
-                    out[d.variable_name] = d
+                    out[d.variable_name + suffix] = d
         return out
 
     def _initialize(self, parameters_name_suffix=None, **kwargs):
-        if parameters_name_suffix is not None:
-            raise NotImplementedError('multiple alchemical regions (parameter suffixes) are not provided')
-        self._parameters_name_suffix = None
+        """kwargs by their unsuffixed names; stored under the suffixed ones (states.py:3932-3963)."""
+        self.__dict__['_parameters_name_suffix'] = None
         controlled = self._get_controlled_parameters()
-        self._parameters = {name: None for name in controlled}
+        suffixed = self._get_controlled_parameters(parameters_name_suffix)
+        self._parameters = {name: None for name in suffixed}
         for name, value in kwargs.items():
             if name not in controlled:
                 raise GlobalParameterError(GlobalParameterError.PARAMETER_NOT_DEFINED,
@@ -513,17 +528,46 @@ class GlobalParameterState:
             d = controlled[name]
             if d.validator_func is not None and value is not None:
                 value = d.validator_func(self, value)
-            self._parameters[name] = value
+            self._parameters[name if parameters_name_suffix is None else name + '_' + parameters_name_suffix] = value
+        self.__dict__['_parameters_name_suffix'] = parameters_name_suffix
+
+    def _suffixed_descriptor(self, key):
+        """The descriptor of a suffixed parameter name this state controls, or None."""
+        suffix = self.__dict__.get('_parameters_name_suffix')
+        if suffix is None or key not in self.__dict__.get('_parameters', {}):
+            return None
+        return self._get_controlled_parameters(suffix)[key]
+
+    def __getattr__(self, key):
+        # only called when normal lookup fails: the suffixed parameters (states.py:3830-3839)
+        if self._suffixed_descriptor(key) is not None:
+            return self._parameters[key]
+        raise AttributeError("{} object has no attribute '{}'".format(type(self).__name__, key))
+
+    def __setattr__(self, key, value):
+        d = self._suffixed_descriptor(key)
+        if d is None:
+            object.__setattr__(self, key, value)
+            return
+        if self._parameters[key] is None and value is not None:
+            raise GlobalParameterError(GlobalParameterError.PARAMETER_NOT_DEFINED,
+                                       'Cannot set the parameter {} in the system as it was not defined.'.format(key))
+        if d.validator_func is not None and value is not None:
+            value = d.validator_func(self, value)
+        self._parameters[key] = value
 
     @classmethod
     def from_system(cls, system, parameters_name_suffix=None):
-        """Read the parameters from the system's global-parameter defaults (alchemy.py:227-253)."""
+        """Read the parameters from the system's global-parameter defaults (alchemy.py:227-253); with a suffix, the
+        parameters named ``name + '_' + parameters_name_suffix`` (states.py:3281-3334)."""
+        suffix = '' if parameters_name_suffix is None else '_' + parameters_name_suffix
         controlled = cls._get_controlled_parameters()
-        found = {n: system.global_parameters[n] for n in controlled if n in system.global_parameters}
+        found = {n: system.global_parameters[n + suffix] for n in controlled if n + suffix in system.global_parameters}
         if not found:
             raise GlobalParameterError(GlobalParameterError.PARAMETER_NOT_DEFINED,
-                                       'System has no global parameters {}.'.format(set(controlled)))
-        return cls(**found)
+                                       'System has no global parameters {}.'.format(
+                                           set(cls._get_controlled_parameters(parameters_name_suffix))))
+        return cls(parameters_name_suffix=parameters_name_suffix, **found)
 
     def apply_to_system(self, system):
         for n, v in self._parameters.items():
@@ -558,11 +602,17 @@ class GlobalParameterState:
         return str(self._parameters)
 
     def __getstate__(self):
-        return dict(_parameters=dict(self._parameters), _parameters_name_suffix=None)
+        # unsuffixed names plus the suffix, as the reference serialises them (states.py:3879-3898)
+        suffix = self._parameters_name_suffix
+        cut = 0 if suffix is None else len(suffix) + 1
+        params = {n[:len(n) - cut]: v for n, v in self._parameters.items()}
+        return dict(_parameters=params, _parameters_name_suffix=suffix)
 
     def __setstate__(self, s):
-        self._parameters = dict(s['_parameters'])
-        self._parameters_name_suffix = None
+        suffix = s.get('_parameters_name_suffix')
+        self.__dict__['_parameters_name_suffix'] = None
+        self._parameters = {(n if suffix is None else n + '_' + suffix): v for n, v in s['_parameters'].items()}
+        self.__dict__['_parameters_name_suffix'] = suffix
 
 
 class CompoundThermodynamicState(ThermodynamicState):
@@ -632,7 +682,7 @@ class CompoundThermodynamicState(ThermodynamicState):
         p = super()._engine_parameters()
         for s in self._composable_states:
             for n, v in getattr(s, '_parameters', {}).items():
-                if v is not None and n in ('lambda_sterics',):
+                if v is not None and n.startswith('lambda_sterics'):   # (with a region's suffix, if any)
                     p[n] = v
         return p
 

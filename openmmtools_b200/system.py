@@ -37,6 +37,9 @@ class System:
         self.softcore_b = 1.0
         self.softcore_c = 6.0
         self.alchemical_dispersion_correction = False
+        # two alchemical regions: ((name, atoms, annihilate_sterics), (name, atoms, annihilate_sterics)), regions 1 and 2
+        # (alchemical_atoms is then their union); None: one region or none
+        self.alchemical_regions = None
         # -- harmonic oscillator (CustomExternalForce global parameters)
         self.ho_K = None
         self.ho_x0 = (0.0, 0.0, 0.0)
@@ -93,6 +96,19 @@ class System:
             m[list(self.alchemical_atoms)] = 1
         return m
 
+    def alchemical_region_ids(self):
+        """Per-atom region id: 0 environment, 1 and 2 the atoms of the two alchemical regions."""
+        ids = np.zeros(self.n_particles, np.uint8)
+        for r, (_, atoms, _) in enumerate(self.alchemical_regions or ()):
+            ids[list(atoms)] = r + 1
+        return ids
+
+    def lambda_sterics_names(self):
+        """The global parameter controlling each alchemical region's sterics (lambda_sterics<suffix>)."""
+        if self.alchemical_regions is None:
+            return ('lambda_sterics',)
+        return tuple('lambda_sterics' + ('' if name is None else '_' + name) for name, _, _ in self.alchemical_regions)
+
     def copy(self):
         return copy.deepcopy(self)
 
@@ -111,6 +127,8 @@ class System:
                            self.use_dispersion_correction, self.alchemical_atoms, self.annihilate_sterics,
                            self.softcore_alpha, self.softcore_a, self.softcore_b, self.softcore_c,
                            self.alchemical_dispersion_correction)).encode())
+            if getattr(self, 'alchemical_regions', None) is not None:   # (one-region systems keep their hash)
+                h.update(repr(self.alchemical_regions).encode())
         if self.kind == MOLECULE:
             for a in (self.sigma, self.epsilon, self.charge, self.bonds, self.angles, self.torsions, self.exclusions,
                       self.exceptions, self.constraints):
@@ -127,3 +145,4 @@ class System:
 
     def __setstate__(self, d):
         self.__dict__.update(d)
+        self.__dict__.setdefault('alchemical_regions', None)
