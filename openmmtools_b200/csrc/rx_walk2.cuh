@@ -394,6 +394,13 @@ __device__ __forceinline__ void w2_walk(const SlotRec2 *__restrict__ rec, const 
             return w2_exact_decision(u, K, rec[sA].ij, si, sj, words, a);
         };
         unsigned Cw = 0;
+        // The fast loop ends when nothing can commit, i.e. when window position 0 is itself a stop: bit 0 of Cw.  Position 0 is
+        // always visited, is never a forced stop and has no earlier position, so that bit is the `undecided` answer of the
+        // lane at position 0.  Slots take it from a vote straight into a predicate: read off Cw it goes from the uniform
+        // datapath's predicate to the branch (a 13-cycle fixed stall at the back edge of every round; 7 % of the round at
+        // K = 256, DESIGN.md 4.1).  Candidates keep the test on Cw: their longer chain resolver hides that stall, and the
+        // extra vote made their round 2.7 % slower.
+        bool stop0 = false;
         // Exact decisions injected into ONE fast round (see the rare path below): `bias` joins the lane's log_p, `luA` is
         // replaced, so that the filter reproduces the exact answer; both are restored when that round has been resolved.
         float bias = 0.f, lu_saved = 0.f;
@@ -432,18 +439,20 @@ __device__ __forceinline__ void w2_walk(const SlotRec2 *__restrict__ rec, const 
                 // at the forced stops of the chain.
                 const unsigned C = __ballot_sync(0xffffffffu, ((earlier & bmA) | und) != 0u);
                 Cw = (__funnelshift_r(C, C, r) | Cf) & V;   // empty: the whole window commits
+                if constexpr (CAND) stop0 = (Cw & 1u) != 0u;
+                else stop0 = __any_sync(0xffffffffu, undecided && w == 0u);
                 p_stop = Cw; p_vis = V;
                 p_mv = ((V >> w) & 1u) != 0u ? 0xffffffffu : 0u;
                 p_sw = changes ? p_mv : 0u;
                 p_entry = (sj * (1u << LOG_STATE_BITS) + si) | (acc ? (1u << 31) | (1u << LOG_ACC_BIT) : (1u << 31));
                 // (position 0 is always visited: nothing commits iff it is itself the lane that ends the round)
-            } while (--quota != 0u && (Cw & 1u) == 0u);
+            } while (--quota != 0u && !stop0);
             // (a no-op unless the round just resolved ran alone, with injected decisions: see below)
             const bool was_injected = injected;
             luA = was_injected ? lu_saved : luA;
             bias = 0.f;
             injected = false;
-            if ((Cw & 1u) == 0u) continue;
+            if (!stop0) continue;
             commit();   // (nothing to commit: positions the lanes on the round that could not start)
             w2_cp_async_wait<8>();
             ahead(qB);
