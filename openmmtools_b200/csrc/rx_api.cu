@@ -790,20 +790,17 @@ extern "C" int rx_mix_stream_position(rx_engine *h, int32_t stream, uint64_t *wo
     return RX_OK;
 }
 
-extern "C" int rx_run_iterations(rx_engine *h, int32_t n_iterations, int32_t mixing, uint64_t seed,
-                                 uint64_t first_iteration, int32_t reassign) {
-    ENTER(h);
-    int rc = check_ready(h, "rx_run_iterations");
-    if (rc) return rc;
-    if (!h->have_integrator) RX_FAIL(h, RX_ERR_INVALID, "rx_run_iterations: rx_set_integrator must be called first");
-    if (mixing < 0 || mixing > 2) RX_FAIL(h, RX_ERR_INVALID, "rx_run_iterations: mixing must be 0, 1 or 2");
-    const long long K = h->cfg.n_replicas;
+// The fused loop of rx_run_iterations and rx_sams_run_iterations, multistatesampler.py:776-782 without a host round trip:
+// mix (with the previous iteration's energies) -> propagate -> energies.  mix(iteration, &launches) is the mixing step; `who`
+// names the entry point in errors.
+template <class Mix>
+static int run_fused(rx_engine *h, const char *who, int32_t n_iterations, uint64_t seed, uint64_t first_iteration, int32_t reassign,
+                     Mix mix) {
+    int rc;
     for (int it = 0; it < n_iterations; it++) {
-        // multistatesampler.py:776-782: mix (with the previous iteration's energies) -> propagate -> energies
         int lm = 0, lp = 0, le = 0;
         PhaseTimer Tm(h, 0);
-        if (mixing == 1) rc = rxi_mix_swap_all(h, K * K * K, &lm);
-        else if (mixing == 2) rc = rxi_mix_swap_neighbors(h, &lm);
+        rc = mix(first_iteration + it, &lm);
         if (rc) return rc;
         Tm.stop(lm);
         PhaseTimer Tp(h, 1);
@@ -817,19 +814,30 @@ extern "C" int rx_run_iterations(rx_engine *h, int32_t n_iterations, int32_t mix
         if (rc) return rc;
         Te.stop(le);
         RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
-        const double m0 = h->phase_ms[0];
         Tm.accumulate(); Tp.accumulate(); Te.accumulate();
-        if (getenv("RX_TRACE_ITER"))
-            fprintf(stderr, "[iter %d] mix %.2f ms (walker %.2f ms, exact-path lanes %lld, rounds %lld)\n", it, h->phase_ms[0] - m0,
-                    h->mix_stats[4] / 1e3, h->mix_stats[1], h->mix_stats[0]);
     }
     rc = check_device_error(h);
     if (rc) return rc;
-    std::vector<int> f(K, 0);
-    RX_CHECK_CUDA(h, cudaMemcpy(f.data(), h->d_nan, sizeof(int) * K, cudaMemcpyDeviceToHost));
+    std::vector<int> f(h->cfg.n_replicas, 0);
+    RX_CHECK_CUDA(h, cudaMemcpy(f.data(), h->d_nan, sizeof(int) * f.size(), cudaMemcpyDeviceToHost));
     for (int k = h->k0; k < h->k0 + h->kloc; k++)
-        if (f[k]) RX_FAIL(h, RX_ERR_NAN, "rx_run_iterations: NaN encountered in a replica");
+        if (f[k]) RX_FAIL(h, RX_ERR_NAN, std::string(who) + ": NaN encountered in a replica");
     return RX_OK;
+}
+
+extern "C" int rx_run_iterations(rx_engine *h, int32_t n_iterations, int32_t mixing, uint64_t seed,
+                                 uint64_t first_iteration, int32_t reassign) {
+    ENTER(h);
+    int rc = check_ready(h, "rx_run_iterations");
+    if (rc) return rc;
+    if (!h->have_integrator) RX_FAIL(h, RX_ERR_INVALID, "rx_run_iterations: rx_set_integrator must be called first");
+    if (mixing < 0 || mixing > 2) RX_FAIL(h, RX_ERR_INVALID, "rx_run_iterations: mixing must be 0, 1 or 2");
+    const long long K = h->cfg.n_replicas;
+    return run_fused(h, "rx_run_iterations", n_iterations, seed, first_iteration, reassign, [&](uint64_t, int *lm) {
+        if (mixing == 1) return rxi_mix_swap_all(h, K * K * K, lm);
+        if (mixing == 2) return rxi_mix_swap_neighbors(h, lm);
+        return (int)RX_OK;
+    });
 }
 
 // ---- SAMS (rx_sams.cuh) ------------------------------------------------------------------------------------------------------
@@ -866,34 +874,10 @@ extern "C" int rx_sams_run_iterations(rx_engine *h, int32_t n_iterations, uint64
     int rc = check_ready(h, "rx_sams_run_iterations");
     if (rc) return rc;
     if (!h->have_integrator) RX_FAIL(h, RX_ERR_INVALID, "rx_sams_run_iterations: rx_set_integrator must be called first");
-    const long long K = h->cfg.n_replicas;
-    for (int it = 0; it < n_iterations; it++) {
-        // multistatesampler.py:776-782 with sams.py:395-437 as the mixing: jump + weight update -> propagate -> energies
-        int lm = 0, lp = 0, le = 0;
-        PhaseTimer Tm(h, 0);
-        rc = rxi_sams_step(h, (long long)(first_iteration + it), first_iteration + it > 0 ? 1 : 0, &lm);
-        if (rc) return rc;
-        Tm.stop(lm);
-        PhaseTimer Tp(h, 1);
-        rc = rxi_propagate(h, seed, first_iteration + it, reassign, &lp);
-        if (rc) return rc;
-        Tp.stop(lp);
-        PhaseTimer Te(h, 2);
-        rc = rxi_compute_energy_rows(h, &le);
-        if (rc) return rc;
-        rc = rxi_allgather_energies(h);
-        if (rc) return rc;
-        Te.stop(le);
-        RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
-        Tm.accumulate(); Tp.accumulate(); Te.accumulate();
-    }
-    rc = check_device_error(h);
-    if (rc) return rc;
-    std::vector<int> f(K, 0);
-    RX_CHECK_CUDA(h, cudaMemcpy(f.data(), h->d_nan, sizeof(int) * K, cudaMemcpyDeviceToHost));
-    for (int k = h->k0; k < h->k0 + h->kloc; k++)
-        if (f[k]) RX_FAIL(h, RX_ERR_NAN, "rx_sams_run_iterations: NaN encountered in a replica");
-    return RX_OK;
+    // sams.py:395-437 as the mixing: jump + weight update
+    return run_fused(h, "rx_sams_run_iterations", n_iterations, seed, first_iteration, reassign, [&](uint64_t iteration, int *lm) {
+        return rxi_sams_step(h, (long long)iteration, iteration > 0 ? 1 : 0, lm);
+    });
 }
 
 extern "C" int rx_get_phase_times(rx_engine *h, double ms[4], int64_t counts[4], int32_t reset) {

@@ -52,6 +52,18 @@ struct MixCtl {          // device-resident control block of the resumable mixin
     long long aux;       // k_mix_walk2 / k_mix_walk2c: record reached (extent of their sparse commit log)
 };
 
+// How a swap-all pass walks the chain (mix_plan in rx_mix.cu): coordinates and filter choose the records and the walkers.
+enum MixCoords { MIX_LOOP, MIX_SLOTS, MIX_CANDS };   // the plain loop alone, slots (power-of-two K), candidate indices
+struct MixPlan {
+    MixCoords coords;
+    bool filter;      // a filter walker takes the bulk of the pass, on SlotRec2 records (else SlotRec / CandRec)
+    int head_unit;    // stream words per unit of MixCtl::head
+    int smem_tail;    // dynamic shared memory of the kernel that finishes the pass (the bulk walkers take WALK_SMEM)
+    bool operator==(const MixPlan &o) const {
+        return coords == o.coords && filter == o.filter && head_unit == o.head_unit && smem_tail == o.smem_tail;
+    }
+};
+
 struct rx_state_move {
     double dt = 0, gamma = 0;
     int n_steps = 0, reassign = 0;
@@ -112,21 +124,22 @@ struct rx_engine {
     void *d_moves = nullptr;
     // mixing
     MTStream streams[2];
-    SlotRec *d_slots = nullptr;
+    uint4 *d_slots = nullptr;   // the 16-byte records of a pass: SlotRec, SlotRec2 or CandRec
     size_t slots_cap = 0;
     MixCtl *d_ctl = nullptr;
     uint32_t *d_log = nullptr;   // commit log of the walker: packed (si, sj, accepted)
-    size_t log_cap = 0;
     uint32_t *d_slotlog = nullptr;   // sparse commit log of k_mix_walk2: one word per slot
     uint32_t *d_cpos = nullptr;      // k_mix_walk2c / k_mix_walk_cand: word position of every candidate of the pass
     uint32_t *d_ctile = nullptr;     // ... candidates per tile / their exclusive scan, then [last] = number of candidates
     size_t ctile_cap = 0;
     unsigned char *d_filt = nullptr;   // 24-bit row image of u for the K=256 walker
     double *d_filt_scale = nullptr;    // [K] scales + [K] row abs-max
-    int prepared_kind = 0;        // ... with these records (REC_* of rx_mix.cu)
-    bool prepared = false;        // words + slot records for the next swap-all call were produced on stream_rng
+    struct {
+        bool valid = false;       // words + records for the next swap-all call were produced on stream_rng ...
+        MixPlan plan = {};        // ... for this plan
+        size_t avail = 0;         // ... over this many stream words
+    } prepared;
     size_t last_consumed = 0;     // words the previous swap-all call consumed (sizes the generate-ahead)
-    size_t slots_for_avail = 0;   // S.avail the slot records were built for
     cudaEvent_t ev_prepared = nullptr, ev_consumed = nullptr;
     void *sams = nullptr;         // SamsState (rx_sams.cuh): device-resident logZ / weights / histogram of a SAMSSampler
     // timing

@@ -14,9 +14,10 @@
 // and ONE warp then walks the chain speculatively: 32 lanes evaluate 32 consecutive slots under the current
 // permutation, the visited-slot chain is resolved with a carry-propagation bit trick, and the longest prefix
 // in which no visited slot touches a replica swapped earlier in the same window is committed.  Any other K is walked the
-// same way in candidate coordinates (the words randint accepts, rx_walk2c.cuh).  The filter walkers (rx_walk2.cuh) take
-// the bulk of a pass for K <= 256; the exact walker (rx_walk_exact.cuh) finishes their passes over slots and walks every
-// pass of larger K (and of any K with RX_NO_FILTER=1) in either coordinate system.
+// same way in candidate coordinates (the words randint accepts, rx_walk2c.cuh).  One plan per call (mix_plan) chooses the
+// walkers: the filter walkers (rx_walk2.cuh) take the bulk of a pass for K <= 256 unless RX_NO_FILTER=1; the exact walker
+// (rx_walk_exact.cuh) finishes their passes over slots and takes their place in either coordinate system for larger K; the
+// plain loop k_mix_walk_serial finishes every pass over candidates and walks every K that has no walker.
 #include "rx_internal.cuh"
 #include <type_traits>
 #include <math.h>
@@ -390,7 +391,7 @@ int rxi_mix_seed(rx_engine *h, int stream, uint32_t seed) {
     if (!S.d_window) RX_CHECK_CUDA(h, cudaMalloc(&S.d_window, 624 * sizeof(uint32_t)));
     RX_CHECK_CUDA(h, cudaMemcpy(S.d_window, mt, sizeof(mt), cudaMemcpyHostToDevice));
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream_rng));
-    if (stream == RX_STREAM_NUMBA) { h->prepared = false; h->last_consumed = 0; }
+    if (stream == RX_STREAM_NUMBA) { h->prepared.valid = false; h->last_consumed = 0; }
     S.avail = 0;
     S.consumed = 0;
     S.seeded = true;
@@ -403,23 +404,13 @@ int rxi_mix_skip(rx_engine *h, int stream, unsigned long long n) {
     if (!S.seeded) RX_FAIL(h, RX_ERR_INVALID, "rx_mix_skip: seed the stream first");
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream_rng));
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
-    if (stream == RX_STREAM_NUMBA) h->prepared = false;
+    if (stream == RX_STREAM_NUMBA) h->prepared.valid = false;
     // drop buffered words first, then advance the generator without storing
-    unsigned long long todo = n;
-    if (S.avail) {
-        const size_t c = (size_t)(todo < S.avail ? todo : S.avail);
-        {
-            size_t left = S.avail - c;
-            if (left && c) {
-                k_copy_words<<<1184, 1024, 0, h->stream>>>(S.d_words + c, S.d_words_alt, (long long)left);
-                RX_CHECK_CUDA(h, cudaGetLastError());
-                std::swap(S.d_words, S.d_words_alt);
-            }
-            S.avail = left;
-            S.consumed += c;
-        }
-        todo -= c;
-    }
+    const size_t c = (size_t)(n < S.avail ? n : S.avail);
+    int launches = 0;
+    int rc = stream_consume(h, S, c, &launches);
+    if (rc) return rc;
+    unsigned long long todo = n - c;
     while (todo > 0) {
         const long long chunk = todo > (1ull << 30) ? (1ll << 30) : (long long)todo;
         k_mt_generate<<<1, 256, 0, h->stream>>>(S.d_window, nullptr, chunk);
@@ -431,18 +422,6 @@ int rxi_mix_skip(rx_engine *h, int stream, unsigned long long n) {
     return RX_OK;
 }
 
-struct MixTrace {   // RX_TRACE_MIX=1: device-time breakdown of one swap-all call (development aid)
-    cudaEvent_t ev[10]; const char *name[10]; int n = 0; bool on = false; cudaStream_t st;
-    void init(cudaStream_t s_) { st = s_; on = getenv("RX_TRACE_MIX") != nullptr; }
-    void mark(const char *what) { if (!on || n >= 10) return; cudaEventCreate(&ev[n]); cudaEventRecord(ev[n], st); name[n++] = what; }
-    void dump() {
-        if (!on) return;
-        cudaStreamSynchronize(st);
-        for (int i = 1; i < n; i++) { float ms = 0; cudaEventElapsedTime(&ms, ev[i - 1], ev[i]); fprintf(stderr, "[mix trace] %-22s %9.3f ms\n", name[i], ms); }
-        for (int i = 0; i < n; i++) cudaEventDestroy(ev[i]);
-    }
-};
-
 static inline bool is_pow2(int k) { return k >= 2 && (k & (k - 1)) == 0; }
 
 // grid of the count kernels over n log entries: one thread per entry, at most 16 blocks per SM (grid-stride loop)
@@ -451,50 +430,77 @@ static inline unsigned count_blocks(const rx_engine *h, long long n) {
     return (unsigned)(nb < h->n_sm * 16 ? nb : h->n_sm * 16);
 }
 
-// what prepare_pass builds from the stream: slot or candidate records, for the exact walker or (2: SlotRec2) the filter walkers
-enum { REC_NONE = 0, REC_SLOT = 1, REC_SLOT2 = 2, REC_CAND = 3, REC_CAND2 = 4 };
-
 // number of candidates of the pass, behind the tile counts and their scan
 static inline uint32_t *cand_total(const rx_engine *h) { return h->d_ctile + (h->ctile_cap / CAND_TILE + 4); }
 
-static inline size_t pass_need(long long remaining, bool fast, bool anyk = false) {
-    const size_t chunk_words = anyk ? (size_t)1 << 25 : (size_t)1 << 26;  // words per pass (any K: 16 bytes of records per word)
-    size_t need = fast ? (size_t)(4 * remaining + 160) : (size_t)(8 * remaining + 512);
+// The speculative walkers are one latency-bound CTA each: they claim (almost) a whole SM's shared memory so that no other CTA --
+// in particular the stream generator that runs concurrently on the side stream -- is scheduled onto the same SM and steals
+// issue slots.  226 KB + the kernel's static shared memory + the generator's 8 KB exceed the SM's 228 KB.
+#define WALK_SMEM (226 * 1024)
+
+// The plan of a swap-all call: the records prepare_pass builds and the walkers of a pass.  A pass runs the bulk walker, if
+// the plan has one, then the tail kernel, which continues from ctl.head:
+//   coords      filter  K                              bulk              tail
+//   slots       yes     power of two, <= 256           k_mix_walk2       k_mix_walk_pow2<true>
+//   slots       no      power of two, <= 16384                           k_mix_walk_pow2<false>
+//   candidates  yes     any other K in [3, 256]        k_mix_walk2c      k_mix_walk_serial
+//   candidates  no      any other K in [3, ANY_MAX_K]  k_mix_walk_cand   k_mix_walk_serial
+//   loop        no      every other K                                    k_mix_walk_serial
+// RX_NO_FILTER=1 turns the filter off; RX_WALK_SERIAL=1 sends the K that would walk candidates to the plain loop.
+static MixPlan mix_plan(int K) {
+    MixPlan p = {MIX_LOOP, false, 1, (int)(K * sizeof(int))};
+    if (is_pow2(K) && K <= (1 << LOG_STATE_BITS)) p = {MIX_SLOTS, false, 2, WALK_SMEM};
+    else if (K >= 3 && K <= ANY_MAX_K && !getenv("RX_WALK_SERIAL")) p.coords = MIX_CANDS;
+    // The f32 row-image filter wherever its walkers' shared memory fits (K <= 256; at K = 256 the 512 KB of f64 would not fit in
+    // shared memory, and at smaller K the filter is still faster than f64 comparisons).  k_mix_walk2 / k_mix_walk2c hold ring,
+    // replicas and image; k_mix_walk_pow2<true> ring, diag, rowabs, perm and image.
+    const size_t smem_w2 = (size_t)W2_RING * 16 + (size_t)K * 8 + (size_t)((3 * K + 1) & ~1) * K;
+    const size_t smem_f24 = (size_t)RING * 16 + (size_t)K * (2 * sizeof(double) + sizeof(int)) + (size_t)3 * K * K;
+    p.filter = p.coords != MIX_LOOP && K <= 256 && smem_w2 <= 224 * 1024 && (p.coords == MIX_CANDS || smem_f24 <= 224 * 1024) &&
+               !getenv("RX_NO_FILTER");
+    return p;
+}
+
+static inline size_t pass_need(long long remaining, const MixPlan &p) {
+    // words per pass (candidates: 16 bytes of records per word)
+    const size_t chunk_words = p.coords == MIX_CANDS ? (size_t)1 << 25 : (size_t)1 << 26;
+    size_t need = p.coords == MIX_SLOTS ? (size_t)(4 * remaining + 160) : (size_t)(8 * remaining + 512);
     if (need > chunk_words) need = chunk_words;
     if (need < 512) need = 512;
     return need;
 }
 
-// Top the stream up to what a pass over `remaining` attempts may consume and (fast path) build its slot records,
-// on stream `st`.  Both are state independent, so for the NEXT mixing call this runs on the side stream while the
-// replicas are being propagated.
-static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, bool fast, int kind, int K, cudaStream_t st, int *launches) {
-    const bool rec2 = kind == REC_SLOT2, anyk = kind == REC_CAND || kind == REC_CAND2;
-    const size_t need = pass_need(remaining, fast, anyk);
+// Top the stream up to what a pass over `remaining` attempts may consume and build the plan's records, on stream `st`.
+// Both are state independent, so for the NEXT mixing call this runs on the side stream while the replicas are being
+// propagated.
+static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, const MixPlan &p, int K, cudaStream_t st, int *launches) {
+    static_assert(sizeof(SlotRec) == 16 && sizeof(SlotRec2) == 16 && sizeof(CandRec) == 16, "every record format fills one uint4");
+    const bool cand = p.coords == MIX_CANDS;
+    const size_t need = pass_need(remaining, p);
     int rc = stream_reserve(h, S, 2 * need + 1024);   // room for the words generated ahead while the walker runs
     if (rc) return rc;
     rc = stream_fill(h, S, need, launches, st);
     if (rc) return rc;
-    if (fast || anyk) {
-        const long long nslots = anyk ? (long long)S.avail : (long long)(S.avail / 2);   // records: per slot, or <= 1 per word
+    if (p.coords != MIX_LOOP) {
+        const long long nslots = cand ? (long long)S.avail : (long long)(S.avail / 2);   // records: per slot, or <= 1 per word
         if ((size_t)nslots > h->slots_cap) {
             // size for the largest stream the buffer can ever hold (2 * need + 1024 words), so that the slightly different
             // `avail` of every iteration never triggers another cudaFree/cudaMalloc (tens of ms each, device-synchronising)
-            size_t want = anyk ? S.cap : (S.cap + 1) / 2;
+            size_t want = cand ? S.cap : (S.cap + 1) / 2;
             if (want < (size_t)nslots) want = (size_t)nslots;
             RX_CHECK_CUDA(h, cudaDeviceSynchronize());
             cudaFree(h->d_slots);
             cudaFree(h->d_log);
             h->d_slots = nullptr; h->d_log = nullptr;
             h->slots_cap = 0;
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_slots, want * sizeof(SlotRec)));
+            RX_CHECK_CUDA(h, cudaMalloc(&h->d_slots, want * sizeof(uint4)));
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_log, want * sizeof(uint32_t)));
             cudaFree(h->d_slotlog);
             h->d_slotlog = nullptr;
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_slotlog, want * sizeof(uint32_t)));
             h->slots_cap = want;
         }
-        if (anyk && (!h->d_cpos || h->ctile_cap < h->slots_cap)) {
+        if (cand && (!h->d_cpos || h->ctile_cap < h->slots_cap)) {
             RX_CHECK_CUDA(h, cudaDeviceSynchronize());
             cudaFree(h->d_cpos); cudaFree(h->d_ctile);
             h->d_cpos = nullptr; h->d_ctile = nullptr;
@@ -502,9 +508,8 @@ static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, bool fas
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_ctile, (h->slots_cap / CAND_TILE + 8) * sizeof(uint32_t)));
             h->ctile_cap = h->slots_cap;
         }
-        if (anyk) {
+        if (cand) {
             // candidate coordinates (rx_walk2c.cuh): flag + count per tile, scan, scatter, one record per candidate index
-            static_assert(sizeof(CandRec) == sizeof(SlotRec), "all record formats share the d_slots buffer");
             int nbits = 0;
             for (unsigned m = (unsigned)(K - 1); m; m >>= 1) nbits++;
             const uint32_t mask = 0xffffffffu >> (32 - nbits);
@@ -513,19 +518,19 @@ static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, bool fas
             k_cand_count<<<ntiles, 256, 0, st>>>(S.d_words, nslots, K, mask, h->d_ctile);
             k_cand_scan<<<1, 1024, 0, st>>>(h->d_ctile, ntiles, cand_total(h));
             k_cand_scatter<<<ntiles, 256, 0, st>>>(S.d_words, nslots, K, mask, h->d_ctile, h->d_cpos);
-            if (kind == REC_CAND2)
+            if (p.filter)
                 k_cand_records<false><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (SlotRec2 *)h->d_slots);
             else
                 k_cand_records<true><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (CandRec *)h->d_slots);
             *launches += 3;
-        } else if (rec2)
+        } else if (p.filter)
             k_slots_build<true><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec2 *)h->d_slots);
         else
-            k_slots_build<false><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), h->d_slots);
+            k_slots_build<false><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec *)h->d_slots);
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
     }
-    h->slots_for_avail = S.avail;
+    h->prepared = {false, p, S.avail};
     return RX_OK;
 }
 
@@ -535,10 +540,8 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
     const int K = h->cfg.n_replicas, M = h->cfg.n_states;
     if (K != M) RX_FAIL(h, RX_ERR_INVALID, "rx_mix_swap_all: requires n_replicas == n_states");
     const size_t mm = (size_t)M * M * sizeof(unsigned long long);
-    MixTrace tr; tr.init(h->stream); tr.mark("enter");
     RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_nacc, 0, mm, h->stream));
     RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_nprop, 0, mm, h->stream));
-    tr.mark("memsets");
     if (nswap <= 0) return RX_OK;
     if (K == 1) {  // randint(1) draws nothing, log_p == 0: every attempt is an accepted no-op
         unsigned long long two_n = 2ull * (unsigned long long)nswap;
@@ -547,38 +550,17 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
         return RX_OK;
     }
-    const bool fast = is_pow2(K) && K <= (1 << LOG_STATE_BITS);
-    // any other K up to 4095: the speculative walkers in candidate coordinates (rx_walk2c.cuh); RX_WALK_SERIAL=1: the plain loop
-    const bool anyk = !fast && K >= 3 && K <= ANY_MAX_K && !getenv("RX_WALK_SERIAL");
+    const MixPlan p = mix_plan(K);
     int logK = 0;
     while ((1 << logK) < K) logK++;
-    const size_t smem_small = (size_t)K * sizeof(int);
-    // ring + diag + rowabs + perm + image
-    const size_t smem_f24 = (size_t)RING * 16 + (size_t)K * (2 * sizeof(double) + sizeof(int)) + (size_t)3 * K * K;
-    // The f32 row-image filter wherever it fits (K <= 256; at K = 256 the 512 KB of f64 would not fit in shared memory, and at
-    // smaller K the filter is still faster than f64 comparisons): 16-byte SlotRec2 records, k_mix_walk2 for the bulk of a pass
-    // and k_mix_walk_pow2<true> for its tail.  Otherwise (RX_NO_FILTER=1: every K) exact f64 values from L2.
-    const bool rec2 = fast && smem_f24 <= 224 * 1024 && !getenv("RX_NO_FILTER");
-    // any K <= 256 whose row image fits: the walker of k_mix_walk2 in candidate coordinates (k_mix_walk2c); otherwise (and
-    // with RX_NO_FILTER=1) the exact walker k_mix_walk_cand
-    const size_t smem_w2 = (size_t)W2_RING * 16 + (size_t)K * 8 + (size_t)((3 * K + 1) & ~1) * K;   // ring, replicas, image
-    const bool cand2 = anyk && K <= 256 && smem_w2 <= 224 * 1024 && !getenv("RX_NO_FILTER");
-    const int kind = anyk ? (cand2 ? REC_CAND2 : REC_CAND) : (!fast ? REC_NONE : (rec2 ? REC_SLOT2 : REC_SLOT));
-    // The walkers are one latency-bound CTA each: they claim (almost) a whole SM's shared memory so that no other CTA -- in
-    // particular the stream generator that runs concurrently on the side stream -- is scheduled onto the same SM and steals
-    // issue slots.  226 KB + the kernel's static shared memory + the generator's 8 KB exceed the SM's 228 KB.
-    const int smem_walk = 226 * 1024;
-    if (!fast) {
-        if (smem_small > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_serial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_small));
-        if (cand2) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2c, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
-        else if (anyk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_cand, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
-    } else {
-        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
-        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
-        RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_mix_walk_pow2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_walk));
-    }
-    tr.mark("func attributes");
-    if (rec2 || cand2) {
+    // the plan's walkers and their dynamic shared memory
+    const void *bulk = !p.filter ? (p.coords == MIX_CANDS ? (const void *)k_mix_walk_cand : nullptr)
+                                 : (p.coords == MIX_SLOTS ? (const void *)k_mix_walk2 : (const void *)k_mix_walk2c);
+    const auto walk_pow2 = p.filter ? k_mix_walk_pow2<true> : k_mix_walk_pow2<false>;
+    const void *tail = p.coords == MIX_SLOTS ? (const void *)walk_pow2 : (const void *)k_mix_walk_serial;
+    if (bulk) RX_CHECK_CUDA(h, cudaFuncSetAttribute(bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, WALK_SMEM));
+    if (p.smem_tail > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(tail, cudaFuncAttributeMaxDynamicSharedMemorySize, p.smem_tail));
+    if (p.filter) {
         if (!h->d_filt) {
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt, (size_t)3 * K * K + 16));
             RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt_scale, sizeof(double) * 2 * K));
@@ -589,33 +571,14 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
     }
-    tr.mark("filter build");
-    // The filter walker (k_mix_walk2 over slots, k_mix_walk2c over candidate indices) takes the bulk of a pass.  It logs the
-    // attempts it commits sparsely, one word per record (zero = no attempt started there), and reports the extent of that
-    // log in ctl.aux; the pass's tail kernel continues from ctl.head.  Both claim a whole SM like the other walkers.
-    auto filter_walk = [&](size_t nrec) -> int {
-        static_assert(sizeof(SlotRec2) == sizeof(SlotRec), "both record formats share the d_slots buffer");
-        if (smem_w2 > (size_t)smem_walk) RX_FAIL(h, RX_ERR_INVALID, "internal: filter walker shared memory");
-        RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, nrec * sizeof(uint32_t), h->stream));
-        if (cand2)
-            k_mix_walk2c<<<1, W2_THREADS, smem_walk, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos, cand_total(h),
-                                                                    h->d_u, K, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale,
-                                                                    h->d_ctl);
-        else
-            k_mix_walk2<<<1, W2_THREADS, smem_walk, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K,
-                                                                   logK, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
-        RX_CHECK_CUDA(h, cudaGetLastError());
-        *launches += 1;
-        return RX_OK;
-    };
     long long remaining = nswap;
     h->mix_stats[0] = h->mix_stats[1] = h->mix_stats[2] = h->mix_stats[4] = h->mix_stats[5] = 0;
     const uint64_t consumed0 = S.consumed;
     const size_t chunk_words = (size_t)1 << 26;
     while (remaining > 0) {
-        const size_t need = pass_need(remaining, fast, anyk);
+        const size_t need = pass_need(remaining, p);
         int rc;
-        if (h->prepared && h->prepared_kind == kind && S.avail >= need && h->slots_for_avail == S.avail) {
+        if (h->prepared.valid && h->prepared.plan == p && S.avail >= need && h->prepared.avail == S.avail) {
             // produced on the side stream while the replicas were propagating
             RX_CHECK_CUDA(h, cudaStreamWaitEvent(h->stream, h->ev_prepared, 0));
             float ms = 0;
@@ -624,71 +587,63 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
                 h->phase_ms[3] += ms;
             h->mix_stats[5] += (long long)(rx_wall_us() - tw0);
         } else {
-            if (h->prepared) RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream_rng));
-            rc = prepare_pass(h, S, remaining, fast, kind, K, h->stream, launches);
+            if (h->prepared.valid) RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream_rng));
+            rc = prepare_pass(h, S, remaining, p, K, h->stream, launches);
             if (rc) return rc;
         }
-        h->prepared = false;
-        tr.mark("prepared/built");
+        h->prepared.valid = false;
         MixCtl ctl = {0, remaining, 0, 0, 0, 0, 0};
         RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_ctl, &ctl, sizeof(ctl), cudaMemcpyHostToDevice, h->stream));
-        size_t consumed_words;
-        if (fast) {
-            const long long nslots = (long long)(S.avail / 2);
-            // While the walker runs (it only reads words [0, avail)), generate on the side stream about as many words
-            // as the previous call consumed: they are appended behind the valid region and adopted afterwards.
-            size_t ahead = 0;
-            if (!getenv("RX_NO_ASYNC_RNG") && h->last_consumed > 0 && S.avail + h->last_consumed <= S.cap) {
-                ahead = h->last_consumed;
-                k_mt_generate<<<1, 256, 0, h->stream_rng>>>(S.d_window, S.d_words + S.avail, (long long)ahead);
-                RX_CHECK_CUDA(h, cudaGetLastError());
-                RX_CHECK_CUDA(h, cudaEventRecord(h->ev_prepared, h->stream_rng));
-                *launches += 1;
-            }
-            RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
-            if (rec2) {
-                if ((rc = filter_walk((size_t)nslots))) return rc;
-                k_mix_walk_pow2<true><<<1, 64, smem_walk, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, h->d_filt, h->d_filt_scale, h->d_ctl);
-            } else
-                k_mix_walk_pow2<false><<<1, 64, smem_walk, h->stream>>>(h->d_slots, S.d_words, (unsigned)nslots, h->d_u, K, logK, h->d_perm, h->d_log, nullptr, nullptr, h->d_ctl);
+        const size_t nrec = p.coords == MIX_SLOTS ? S.avail / 2 : S.avail;   // records: per slot, or <= 1 per word
+        // Passes over slots: while the walkers run (they only read words [0, avail)), generate on the side stream about as many
+        // words as the previous call consumed; they are appended behind the valid region and adopted afterwards.
+        size_t ahead = 0;
+        if (p.coords == MIX_SLOTS && !getenv("RX_NO_ASYNC_RNG") && h->last_consumed > 0 && S.avail + h->last_consumed <= S.cap) {
+            ahead = h->last_consumed;
+            k_mt_generate<<<1, 256, 0, h->stream_rng>>>(S.d_window, S.d_words + S.avail, (long long)ahead);
             RX_CHECK_CUDA(h, cudaGetLastError());
-            RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
-            tr.mark("walker");
+            RX_CHECK_CUDA(h, cudaEventRecord(h->ev_prepared, h->stream_rng));
             *launches += 1;
-            RX_CHECK_CUDA(h, cudaMemcpyAsync(&ctl, h->d_ctl, sizeof(ctl), cudaMemcpyDeviceToHost, h->stream));
-            RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
-            { float wms = 0; if (cudaEventElapsedTime(&wms, h->ev_walk[0], h->ev_walk[1]) == cudaSuccess) h->mix_stats[4] += (long long)(wms * 1e3f); }
-            consumed_words = (size_t)(2 * ctl.head);
-            if (ahead) {   // adopt the words generated during the walk
-                RX_CHECK_CUDA(h, cudaStreamWaitEvent(h->stream, h->ev_prepared, 0));
-                S.avail += ahead;
-            }
-        } else {
-            if (anyk) {
-                // bulk of the pass: a walker over candidate indices (the filter walker, or the exact one, which claims the SM
-                // like the others); the plain loop below finishes the pass
-                RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
-                if (cand2) {
-                    if ((rc = filter_walk(S.avail))) return rc;
-                } else {
-                    k_mix_walk_cand<<<1, 64, smem_walk, h->stream>>>((const CandRec *)h->d_slots, S.d_words, h->d_cpos, cand_total(h),
-                                                                       h->d_u, K, h->d_perm, h->d_log, h->d_ctl);
-                    RX_CHECK_CUDA(h, cudaGetLastError());
-                    *launches += 1;
-                }
-                RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
-            }
-            k_mix_walk_serial<<<1, 32, smem_small, h->stream>>>(S.d_words, (long long)S.avail, h->d_u, K, M, h->d_perm, h->d_nacc,
-                                                        h->d_nprop, h->d_ctl);
+        }
+        // walker_ms times the speculative walkers of a pass (the bulk walker, and k_mix_walk_pow2 over slots), never the plain loop
+        const bool timed = p.coords != MIX_LOOP;
+        if (timed) RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[0], h->stream));
+        if (p.filter) {
+            // the filter walker logs the attempts it commits sparsely, one word per record (zero = no attempt started there),
+            // and reports the extent of that log in ctl.aux
+            RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, nrec * sizeof(uint32_t), h->stream));
+            if (p.coords == MIX_SLOTS)
+                k_mix_walk2<<<1, W2_THREADS, WALK_SMEM, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K,
+                                                                   logK, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
+            else
+                k_mix_walk2c<<<1, W2_THREADS, WALK_SMEM, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos, cand_total(h),
+                                                                    h->d_u, K, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale,
+                                                                    h->d_ctl);
+        } else if (p.coords == MIX_CANDS)
+            k_mix_walk_cand<<<1, 64, WALK_SMEM, h->stream>>>((const CandRec *)h->d_slots, S.d_words, h->d_cpos, cand_total(h), h->d_u, K,
+                                                               h->d_perm, h->d_log, h->d_ctl);
+        if (bulk) {
             RX_CHECK_CUDA(h, cudaGetLastError());
             *launches += 1;
-            RX_CHECK_CUDA(h, cudaMemcpyAsync(&ctl, h->d_ctl, sizeof(ctl), cudaMemcpyDeviceToHost, h->stream));
-            RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
-            consumed_words = (size_t)ctl.head;
-            if (anyk) {
-                float wms = 0;
-                if (cudaEventElapsedTime(&wms, h->ev_walk[0], h->ev_walk[1]) == cudaSuccess) h->mix_stats[4] += (long long)(wms * 1e3f);
-            }
+        }
+        // the pass's tail continues from ctl.head
+        if (p.coords == MIX_SLOTS)
+            walk_pow2<<<1, 64, p.smem_tail, h->stream>>>((const SlotRec *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K, logK, h->d_perm,
+                                                         h->d_log, p.filter ? h->d_filt : nullptr, p.filter ? h->d_filt_scale : nullptr, h->d_ctl);
+        if (timed) RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
+        if (p.coords != MIX_SLOTS)
+            k_mix_walk_serial<<<1, 32, p.smem_tail, h->stream>>>(S.d_words, (long long)S.avail, h->d_u, K, M, h->d_perm, h->d_nacc,
+                                                                 h->d_nprop, h->d_ctl);
+        RX_CHECK_CUDA(h, cudaGetLastError());
+        *launches += 1;
+        RX_CHECK_CUDA(h, cudaMemcpyAsync(&ctl, h->d_ctl, sizeof(ctl), cudaMemcpyDeviceToHost, h->stream));
+        RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+        float wms = 0;
+        if (timed && cudaEventElapsedTime(&wms, h->ev_walk[0], h->ev_walk[1]) == cudaSuccess) h->mix_stats[4] += (long long)(wms * 1e3f);
+        const size_t consumed_words = (size_t)ctl.head * p.head_unit;
+        if (ahead) {   // adopt the words generated during the walk
+            RX_CHECK_CUDA(h, cudaStreamWaitEvent(h->stream, h->ev_prepared, 0));
+            S.avail += ahead;
         }
         // count matrices from the commit logs (k_mix_walk_serial counts as it goes)
         if (ctl.aux > 0) {   // the filter walker's sparse log
@@ -701,7 +656,6 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
             RX_CHECK_CUDA(h, cudaGetLastError());
             *launches += 1;
         }
-        tr.mark("adopt-ahead + count");
         if (ctl.remaining == remaining && consumed_words == 0 && need >= chunk_words)
             RX_FAIL(h, RX_ERR_INVALID, "internal: mixing made no progress");
         remaining = ctl.remaining;
@@ -710,9 +664,7 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         h->mix_stats[2] += 1;
         rc = stream_consume(h, S, consumed_words, launches);
         if (rc) return rc;
-        tr.mark("consume copy");
     }
-    tr.dump();
     h->mix_stats[3] = (long long)(S.consumed - consumed0);
     h->last_consumed = (size_t)(S.consumed - consumed0);
     if (!getenv("RX_NO_ASYNC_RNG")) {
@@ -721,13 +673,12 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         RX_CHECK_CUDA(h, cudaStreamWaitEvent(h->stream_rng, h->ev_consumed, 0));
         RX_CHECK_CUDA(h, cudaEventRecord(h->ev[6], h->stream_rng));
         int l2 = 0;
-        int rc2 = prepare_pass(h, S, nswap, fast, kind, K, h->stream_rng, &l2);
-        h->prepared_kind = kind;
+        int rc2 = prepare_pass(h, S, nswap, p, K, h->stream_rng, &l2);
         if (rc2) return rc2;
         RX_CHECK_CUDA(h, cudaEventRecord(h->ev[7], h->stream_rng));
         RX_CHECK_CUDA(h, cudaEventRecord(h->ev_prepared, h->stream_rng));
         h->phase_launches[3] += l2;
-        h->prepared = true;
+        h->prepared.valid = true;
     }
     return RX_OK;
 }
