@@ -884,7 +884,7 @@ int rxi_convert_out(rx_engine *h, const float4 *src, int first_local, int count,
 #include "rx_molecule.cuh"
 
 // A block may take 48 KB of shared memory, static and dynamic together, unless the kernel has opted in to more (up to
-// cudaDevAttrMaxSharedMemoryPerBlockOptin, which rxi_set_molecule checks).  The molecule's tables grow with its terms, the
+// cudaDevAttrMaxSharedMemoryPerBlockOptin, which mol_check_shared checks).  The molecule's tables grow with its terms, the
 // energy kernel's coordinates with the atoms (48 KB of them at 2048 atoms, over the limit with its static arrays).
 static int smem_opt_in(rx_engine *h, const void *kern, int dyn) {
     cudaFuncAttributes fa;
@@ -893,6 +893,9 @@ static int smem_opt_in(rx_engine *h, const void *kern, int dyn) {
         RX_CHECK_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
     return RX_OK;
 }
+
+// The dynamic shared memory of the molecule kernels (mol_gb_at): k_propagate_mol's (f32) or the others'; g: the GB kernels'.
+static int mol_dyn_bytes(const MolDev &m, const MolGB *g, bool f32) { return mol_gb_at(m, f32) + (g ? g->prop_bytes : 0); }
 
 // ---------------------------------------------------------------------------------------------------
 // The move of a splitting program (V, R, O substeps) run n_steps times with timestep dt and friction gamma.
@@ -1100,7 +1103,7 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         const bool star = md->max_cluster <= 3 && !no_star;
         auto kern = gb ? (star ? k_propagate_mol<true, true> : k_propagate_mol<false, true>)
                        : (star ? k_propagate_mol<true, false> : k_propagate_mol<false, false>);
-        const int dyn = md->dyn_shared_bytes + (gb ? gb->prop_bytes : 0);
+        const int dyn = mol_dyn_bytes(*md, gb, true);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
         kern<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p.move, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
@@ -1360,7 +1363,7 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
         const MolDev *m = (const MolDev *)h->mol_dev;
         const MolGB *gb = (const MolGB *)h->mol_gb;
         auto kern = gb ? k_minimize_mol<true> : k_minimize_mol<false>;
-        const int dyn = m->shared_bytes + (gb ? MOL_GB_LANE_BYTES : 0);
+        const int dyn = mol_dyn_bytes(*m, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
         kern<<<h->kloc, 32, dyn, h->stream>>>(*m, (double *)h->d_pos, h->k0, tolerance, max_iterations > 0 ? max_iterations : 100000,
@@ -1429,7 +1432,7 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
         const MolDev *m = (const MolDev *)h->mol_dev;
         const MolGB *gb = (const MolGB *)h->mol_gb;
         auto kern = gb ? k_energy_mol<true> : k_energy_mol<false>;
-        const int dyn = m->shared_bytes + (gb ? MOL_GB_LANE_BYTES : 0);
+        const int dyn = mol_dyn_bytes(*m, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
         kern<<<h->kloc, 32, dyn, h->stream>>>(*m, d_states, n_states, (const double *)h->d_pos, h->k0, d_out, gb ? *gb : MolGB{});
@@ -1469,18 +1472,86 @@ int rxi_compute_energy_rows(rx_engine *h, int *launches) {
 
 
 // ---------------------------------------------------------------------------------------------------
-// Molecule tables (rx_set_molecule): per-atom term lists, the pair mask, constraint clusters.
+// Molecule tables (rx_set_molecule): the term list with its slots, packed in f32 and in f64; constraint clusters.
 // ---------------------------------------------------------------------------------------------------
 template <typename T>
 static int mol_upload(rx_engine *h, const std::vector<T> &v, const T **out) {
     void *d = nullptr;
-    // (+16: the kernels stage these tables into shared memory in 8-byte pieces and may read up to the next multiple of 8)
-    const size_t bytes = sizeof(T) * (v.empty() ? 1 : v.size()) + 16;
+    const size_t bytes = sizeof(T) * (v.empty() ? 1 : v.size());
     RX_CHECK_CUDA(h, cudaMalloc(&d, bytes));
     RX_CHECK_CUDA(h, cudaMemset(d, 0, bytes));
     if (!v.empty()) RX_CHECK_CUDA(h, cudaMemcpy(d, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
     h->mol_allocs.push_back(d);
     *out = (const T *)d;
+    return RX_OK;
+}
+
+struct MolTermList {   // every term once with the slots of its contributions; parameters in f64
+    std::vector<TBond<double>> b;
+    std::vector<TAngle<double>> a;
+    std::vector<TTors<double>> t;
+    std::vector<TPair<double>> p;   // the plain pairs (the first n_plain), then the exceptions
+    int n_plain = 0;
+    std::vector<int> goff;
+};
+
+// A plain pair's epsilon: the f32 table has always held the rounded sqrt(eps_i eps_j), the f64 evaluation the product of the
+// square roots; each precision keeps its expression, so that neither result changes.
+static void mol_pair_eps(float &e, double ei, double ej) { e = (float)sqrt(ei * ej); }
+static void mol_pair_eps(double &e, double ei, double ej) { e = sqrt(ei) * sqrt(ej); }
+
+// The term list in precision T as one blob: MolTerms, then the four tables and goff, each padded to 16 bytes.
+template <typename T>
+static std::vector<unsigned char> mol_pack(const MolTermList &L, const std::vector<double> &eps) {
+    std::vector<TBond<T>> b;
+    std::vector<TAngle<T>> a;
+    std::vector<TTors<T>> t;
+    std::vector<TPair<T>> p;
+    for (const auto &x : L.b) b.push_back({x.i, x.j, x.si, x.sj, (T)x.K, (T)x.r0});
+    for (const auto &x : L.a) a.push_back({x.i, x.j, x.k, x.si, x.sj, x.sk, (T)x.K, (T)x.t0});
+    for (const auto &x : L.t) t.push_back({x.i, x.j, x.k, x.l, x.si, x.sj, x.sk, x.sl, (T)x.n, (T)x.phase, (T)x.kk});
+    for (size_t q = 0; q < L.p.size(); q++) {
+        const auto &x = L.p[q];
+        p.push_back({x.i, x.j, x.si, x.sj, (T)x.qq, (T)x.sig, (T)x.eps});
+        if ((int)q < L.n_plain) mol_pair_eps(p.back().eps, eps[x.i], eps[x.j]);
+    }
+    auto up = [](size_t bytes) { return (bytes + 15) & ~(size_t)15; };
+    MolTerms hd;
+    memset(&hd, 0, sizeof(hd));
+    size_t off = up(sizeof(MolTerms));
+    hd.o_bond = (int)off; off += up(sizeof(TBond<T>) * b.size());
+    hd.o_angle = (int)off; off += up(sizeof(TAngle<T>) * a.size());
+    hd.o_tors = (int)off; off += up(sizeof(TTors<T>) * t.size());
+    hd.o_pair = (int)off; off += up(sizeof(TPair<T>) * p.size());
+    hd.o_goff = (int)off; off += up(sizeof(int) * L.goff.size());
+    std::vector<unsigned char> blob(off, 0);
+    memcpy(blob.data(), &hd, sizeof(hd));
+    auto put = [&](int o, const auto &v) { if (!v.empty()) memcpy(blob.data() + o, v.data(), sizeof(v[0]) * v.size()); };
+    put(hd.o_bond, b); put(hd.o_angle, a); put(hd.o_tors, t); put(hd.o_pair, p); put(hd.o_goff, L.goff);
+    return blob;
+}
+
+// What no block of the molecule kernels (vacuum, or GB with g) can hold is refused here rather than at launch (which opts in
+// above 48 KB: smem_opt_in).  The slot indices of the term tables are shorts; tables that fit in shared memory have far fewer
+// slots, checked all the same.
+static int mol_check_shared(rx_engine *h, const MolDev &m, const MolGB *g, const char *what) {
+    int dev = 0, optin = 0;
+    RX_CHECK_CUDA(h, cudaGetDevice(&dev));
+    RX_CHECK_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    const struct { const void *kern; int dyn; } use[] = {
+        {g ? (const void *)k_propagate_mol<true, true> : (const void *)k_propagate_mol<true, false>, mol_dyn_bytes(m, g, true)},
+        {g ? (const void *)k_propagate_mol<false, true> : (const void *)k_propagate_mol<false, false>, mol_dyn_bytes(m, g, true)},
+        {g ? (const void *)k_minimize_mol<true> : (const void *)k_minimize_mol<false>, mol_dyn_bytes(m, g, false)},
+        {g ? (const void *)k_energy_mol<true> : (const void *)k_energy_mol<false>, mol_dyn_bytes(m, g, false)}};
+    size_t need = 0;
+    for (const auto &u : use) {
+        cudaFuncAttributes fa;
+        RX_CHECK_CUDA(h, cudaFuncGetAttributes(&fa, u.kern));
+        need = std::max(need, fa.sharedSizeBytes + (size_t)u.dyn);
+    }
+    if (need > (size_t)optin || m.n_slots > 32767)
+        RX_FAIL(h, RX_ERR_UNSUPPORTED, std::string(what) + " need " + std::to_string(need) +
+                                           " bytes of shared memory per block, more than the device's " + std::to_string(optin));
     return RX_OK;
 }
 
@@ -1495,44 +1566,69 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
         eps(mol->epsilon, mol->epsilon + n);
     for (int i = 0; i < n; i++)
         if (!(mass[i] > 0) || !(sigma[i] > 0) || eps[i] < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: need mass > 0, sigma > 0, epsilon >= 0");
-    std::vector<std::vector<MolBond>> ba(n);
-    std::vector<std::vector<MolAngle>> aa(n);
-    std::vector<std::vector<MolTorsion>> ta(n);
-    std::vector<std::vector<MolExc>> xa(n);
-    std::vector<unsigned> mask(n);
-    for (int i = 0; i < n; i++) mask[i] = (n == 32 ? 0xffffffffu : ((1u << n) - 1u)) & ~(1u << i);
+    // the term list: every term once; each atom's contributions get consecutive slots in the order bonds, angles, torsions,
+    // pairs (the plain ones by partner index, then the exceptions in list order), each kind in list order
+    MolTermList L;
+    struct Contrib { int kind, term, role; };
+    std::vector<std::vector<Contrib>> per_atom(n);
+    std::vector<unsigned> nb_mask(n);   // bit j of nb_mask[i]: the pair (i, j) has the plain Coulomb + LJ interaction
+    for (int i = 0; i < n; i++) nb_mask[i] = (n == 32 ? 0xffffffffu : ((1u << n) - 1u)) & ~(1u << i);
     for (int b = 0; b < mol->n_bonds; b++) {
         const double *q = mol->bonds + 4 * b;
         if (!atom_ok(q[0]) || !atom_ok(q[1]) || q[0] == q[1]) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: bad bond");
-        const int i = (int)q[0], j = (int)q[1];
-        ba[i].push_back(MolBond{j, 0, q[2], q[3]});
-        ba[j].push_back(MolBond{i, 0, q[2], q[3]});
+        L.b.push_back({(short)q[0], (short)q[1], 0, 0, q[2], q[3]});
+        for (int r = 0; r < 2; r++) per_atom[(int)q[r]].push_back({0, b, r});
     }
     for (int a = 0; a < mol->n_angles; a++) {
         const double *q = mol->angles + 5 * a;
         if (!atom_ok(q[0]) || !atom_ok(q[1]) || !atom_ok(q[2])) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: bad angle");
-        const int id[3] = {(int)q[0], (int)q[1], (int)q[2]};
-        for (int role = 0; role < 3; role++) aa[id[role]].push_back(MolAngle{id[0], id[1], id[2], role, q[3], q[4]});
+        L.a.push_back({(short)q[0], (short)q[1], (short)q[2], 0, 0, 0, q[3], q[4]});
+        for (int r = 0; r < 3; r++) per_atom[(int)q[r]].push_back({1, a, r});
     }
     for (int t = 0; t < mol->n_torsions; t++) {
         const double *q = mol->torsions + 7 * t;
         if (!atom_ok(q[0]) || !atom_ok(q[1]) || !atom_ok(q[2]) || !atom_ok(q[3])) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: bad torsion");
-        const int id[4] = {(int)q[0], (int)q[1], (int)q[2], (int)q[3]};
-        for (int role = 0; role < 4; role++) ta[id[role]].push_back(MolTorsion{id[0], id[1], id[2], id[3], (int)q[4], role, q[5], q[6]});
+        L.t.push_back({(short)q[0], (short)q[1], (short)q[2], (short)q[3], 0, 0, 0, 0, q[4], q[5], q[6]});
+        for (int r = 0; r < 4; r++) per_atom[(int)q[r]].push_back({2, t, r});
     }
     for (int e = 0; e < mol->n_exclusions; e++) {
         const int64_t i = mol->exclusions[2 * e], j = mol->exclusions[2 * e + 1];
         if (i < 0 || i >= n || j < 0 || j >= n || i == j) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: bad exclusion");
-        mask[i] &= ~(1u << j); mask[j] &= ~(1u << i);
+        nb_mask[i] &= ~(1u << j); nb_mask[j] &= ~(1u << i);
     }
     for (int e = 0; e < mol->n_exceptions; e++) {
         const double *q = mol->exceptions + 5 * e;
         if (!atom_ok(q[0]) || !atom_ok(q[1]) || q[0] == q[1]) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: bad exception");
         const int i = (int)q[0], j = (int)q[1];
-        mask[i] &= ~(1u << j); mask[j] &= ~(1u << i);
-        xa[i].push_back(MolExc{j, 0, q[2], q[3], q[4]});
-        xa[j].push_back(MolExc{i, 0, q[2], q[3], q[4]});
+        nb_mask[i] &= ~(1u << j); nb_mask[j] &= ~(1u << i);
     }
+    auto add_pair = [&](const TPair<double> &p) {
+        L.p.push_back(p);
+        per_atom[p.i].push_back({3, (int)L.p.size() - 1, 0}); per_atom[p.j].push_back({3, (int)L.p.size() - 1, 1});
+    };
+    for (int i = 0; i < n; i++)
+        for (int j = i + 1; j < n; j++)
+            if ((nb_mask[i] >> j) & 1u)   // (epsilon: mol_pack)
+                add_pair({(short)i, (short)j, 0, 0, MOL_ONE_4PI_EPS0 * charge[i] * charge[j], 0.5 * (sigma[i] + sigma[j]), 0.0});
+    L.n_plain = (int)L.p.size();
+    for (int e = 0; e < mol->n_exceptions; e++) {
+        const double *q = mol->exceptions + 5 * e;
+        add_pair({(short)q[0], (short)q[1], 0, 0, MOL_ONE_4PI_EPS0 * q[2], q[3], q[4]});
+    }
+    L.goff.assign(1, 0);
+    int slot = 0;
+    for (int i = 0; i < n; i++) {
+        for (const Contrib &c : per_atom[i]) {
+            short *dst = nullptr;
+            if (c.kind == 0) dst = c.role == 0 ? &L.b[c.term].si : &L.b[c.term].sj;
+            else if (c.kind == 1) dst = c.role == 0 ? &L.a[c.term].si : (c.role == 1 ? &L.a[c.term].sj : &L.a[c.term].sk);
+            else if (c.kind == 2) dst = c.role == 0 ? &L.t[c.term].si : (c.role == 1 ? &L.t[c.term].sj : (c.role == 2 ? &L.t[c.term].sk : &L.t[c.term].sl));
+            else dst = c.role == 0 ? &L.p[c.term].si : &L.p[c.term].sj;
+            *dst = (short)slot++;
+        }
+        L.goff.push_back(slot);
+    }
+    L.goff.push_back(slot);   // (padding to an even count)
     // constraint clusters: connected components, constraints kept in list order inside a cluster
     std::vector<int> comp(n);
     for (int i = 0; i < n; i++) comp[i] = i;
@@ -1553,134 +1649,22 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
     if ((int)cl.size() > 32) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_molecule: more than 32 constraint clusters");
     std::vector<MolCons> cons;
     for (auto &c : cl) { cons.insert(cons.end(), c.begin(), c.end()); c_off.push_back((int)cons.size()); }
-    auto flatten = [&](auto &per_atom, auto &flat, std::vector<int> &off) {
-        off.assign(1, 0);
-        for (int i = 0; i < n; i++) { flat.insert(flat.end(), per_atom[i].begin(), per_atom[i].end()); off.push_back((int)flat.size()); }
-    };
-    std::vector<MolBond> bonds; std::vector<MolAngle> angles; std::vector<MolTorsion> tors; std::vector<MolExc> exc;
-    std::vector<int> b_off, a_off, t_off, x_off;
-    flatten(ba, bonds, b_off); flatten(aa, angles, a_off); flatten(ta, tors, t_off); flatten(xa, exc, x_off);
-    std::vector<double> seps(n);
-    for (int i = 0; i < n; i++) seps[i] = sqrt(eps[i]);
-    // (padding so that the 8-byte staging copies never read past an allocation)
-    b_off.push_back(0); a_off.push_back(0); t_off.push_back(0); x_off.push_back(0); mask.push_back(0);
     MolDev *m = (MolDev *)h->mol_dev;
     if (!m) { m = new MolDev(); h->mol_dev = m; }
     memset(m, 0, sizeof(*m));
-    for (int i = 0; i <= n; i++) { m->b_off_h[i] = b_off[i]; m->a_off_h[i] = a_off[i]; m->t_off_h[i] = t_off[i]; m->x_off_h[i] = x_off[i]; }
-    {
-        auto up = [](size_t b) { return (b + 15) & ~(size_t)15; };
-        m->shared_bytes = (int)(up(sizeof(MolBond) * bonds.size()) + up(sizeof(MolAngle) * angles.size()) + up(sizeof(MolTorsion) * tors.size()) +
-                                up(sizeof(MolExc) * exc.size()) + 4 * up(sizeof(int) * (n + 2)) + 3 * up(sizeof(double) * n) + up(sizeof(unsigned) * (n + 1)) + 64);
-    }
     m->n = n; m->n_clusters = (int)cl.size(); m->remove_cm = mol->remove_cm_motion ? 1 : 0;
     for (auto &c : cl) m->max_cluster = std::max(m->max_cluster, (int)c.size());
     m->tol = mol->constraint_tolerance > 0 ? mol->constraint_tolerance : 1e-8;   // integrators.py constraint_tolerance default
-    // ---- term tables of the dynamics (each term once) and the slots of their force contributions: atom by atom, in the
-    // order bonds, angles, torsions, pairs, each in list order
-    {
-        struct Contrib { int kind, term, role; };
-        std::vector<std::vector<Contrib>> per_atom(n);
-        std::vector<TBond> tb((size_t)mol->n_bonds);
-        std::vector<TAngle> tang((size_t)mol->n_angles);
-        std::vector<TTors> tt((size_t)mol->n_torsions);
-        std::vector<TPair> tp;
-        for (int b = 0; b < mol->n_bonds; b++) {
-            const double *q = mol->bonds + 4 * b;
-            tb[b] = TBond{(short)q[0], (short)q[1], 0, 0, (float)q[2], (float)q[3]};
-            per_atom[(int)q[0]].push_back({0, b, 0}); per_atom[(int)q[1]].push_back({0, b, 1});
-        }
-        for (int a = 0; a < mol->n_angles; a++) {
-            const double *q = mol->angles + 5 * a;
-            tang[a] = TAngle{(short)q[0], (short)q[1], (short)q[2], 0, 0, 0, (float)q[3], (float)q[4]};
-            for (int r = 0; r < 3; r++) per_atom[(int)q[r]].push_back({1, a, r});
-        }
-        for (int t = 0; t < mol->n_torsions; t++) {
-            const double *q = mol->torsions + 7 * t;
-            tt[t] = TTors{(short)q[0], (short)q[1], (short)q[2], (short)q[3], 0, 0, 0, 0, (float)q[4], (float)q[5], (float)q[6]};
-            for (int r = 0; r < 4; r++) per_atom[(int)q[r]].push_back({2, t, r});
-        }
-        for (int i = 0; i < n; i++)
-            for (int j = i + 1; j < n; j++)
-                if ((mask[i] >> j) & 1u) {
-                    tp.push_back(TPair{(short)i, (short)j, 0, 0, (float)(MOL_ONE_4PI_EPS0 * charge[i] * charge[j]),
-                                       (float)(0.5 * (sigma[i] + sigma[j])), (float)sqrt(eps[i] * eps[j])});
-                    per_atom[i].push_back({3, (int)tp.size() - 1, 0}); per_atom[j].push_back({3, (int)tp.size() - 1, 1});
-                }
-        for (int e = 0; e < mol->n_exceptions; e++) {
-            const double *q = mol->exceptions + 5 * e;
-            tp.push_back(TPair{(short)q[0], (short)q[1], 0, 0, (float)(MOL_ONE_4PI_EPS0 * q[2]), (float)q[3], (float)q[4]});
-            per_atom[(int)q[0]].push_back({3, (int)tp.size() - 1, 0}); per_atom[(int)q[1]].push_back({3, (int)tp.size() - 1, 1});
-        }
-        std::vector<int> goff(1, 0);
-        int slot = 0;
-        for (int i = 0; i < n; i++) {
-            for (const Contrib &c : per_atom[i]) {
-                short *dst = nullptr;
-                if (c.kind == 0) dst = c.role == 0 ? &tb[c.term].si : &tb[c.term].sj;
-                else if (c.kind == 1) dst = c.role == 0 ? &tang[c.term].si : (c.role == 1 ? &tang[c.term].sj : &tang[c.term].sk);
-                else if (c.kind == 2) dst = c.role == 0 ? &tt[c.term].si : (c.role == 1 ? &tt[c.term].sj : (c.role == 2 ? &tt[c.term].sk : &tt[c.term].sl));
-                else dst = c.role == 0 ? &tp[c.term].si : &tp[c.term].sj;
-                *dst = (short)slot++;
-            }
-            goff.push_back(slot);
-        }
-        goff.push_back(slot);   // (padding to an even count)
-        auto up = [](size_t b) { return (b + 15) & ~(size_t)15; };
-        MolTerms hd;
-        memset(&hd, 0, sizeof(hd));
-        size_t off = up(sizeof(MolTerms));
-        hd.o_bond = (int)off; off += up(sizeof(TBond) * tb.size());
-        hd.o_angle = (int)off; off += up(sizeof(TAngle) * tang.size());
-        hd.o_tors = (int)off; off += up(sizeof(TTors) * tt.size());
-        hd.o_pair = (int)off; off += up(sizeof(TPair) * tp.size());
-        hd.o_goff = (int)off; off += up(sizeof(int) * goff.size());
-        std::vector<unsigned char> blob(off, 0);
-        memcpy(blob.data(), &hd, sizeof(hd));
-        if (!tb.empty()) memcpy(blob.data() + hd.o_bond, tb.data(), sizeof(TBond) * tb.size());
-        if (!tang.empty()) memcpy(blob.data() + hd.o_angle, tang.data(), sizeof(TAngle) * tang.size());
-        if (!tt.empty()) memcpy(blob.data() + hd.o_tors, tt.data(), sizeof(TTors) * tt.size());
-        if (!tp.empty()) memcpy(blob.data() + hd.o_pair, tp.data(), sizeof(TPair) * tp.size());
-        memcpy(blob.data() + hd.o_goff, goff.data(), sizeof(int) * goff.size());
-        const unsigned char *d_blob = nullptr;
-        int rcb = mol_upload(h, blob, &d_blob);
-        if (rcb) return rcb;
-        m->terms = (const MolTerms *)d_blob;
-        m->terms_bytes = (int)off;
-        m->n_tb = (int)tb.size(); m->n_ta = (int)tang.size(); m->n_tt = (int)tt.size(); m->n_tp = (int)tp.size(); m->n_slots = slot;
-        m->dyn_shared_bytes = m->shared_bytes + (int)up(off) + (int)up(sizeof(float) * 3 * (size_t)(slot > 0 ? slot : 1));
-    }
-    // What no block can hold is refused here rather than at launch (which opts in above 48 KB: smem_opt_in).  The slot
-    // indices of the term tables are shorts; tables that fit in shared memory have far fewer slots, checked all the same.
-    {
-        int dev = 0, optin = 0;
-        RX_CHECK_CUDA(h, cudaGetDevice(&dev));
-        RX_CHECK_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        const struct { const void *kern; int dyn; } use[] = {{(const void *)k_propagate_mol<true, false>, m->dyn_shared_bytes},
-                                                             {(const void *)k_propagate_mol<false, false>, m->dyn_shared_bytes},
-                                                             {(const void *)k_minimize_mol<false>, m->shared_bytes},
-                                                             {(const void *)k_energy_mol<false>, m->shared_bytes}};
-        size_t need = 0;
-        for (const auto &u : use) {
-            cudaFuncAttributes fa;
-            RX_CHECK_CUDA(h, cudaFuncGetAttributes(&fa, u.kern));
-            need = std::max(need, fa.sharedSizeBytes + (size_t)u.dyn);
-        }
-        const int slots = m->n_slots;
-        if (need > (size_t)optin || slots > 32767) {
-            rxi_free_molecule(h);
-            RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_molecule: the term tables need " + std::to_string(need) +
-                                               " bytes of shared memory per block, more than the device's " + std::to_string(optin) +
-                                               " (too many bonded terms)");
-        }
-    }
-    int rc = 0;
-    if ((rc = mol_upload(h, mass, &m->mass)) || (rc = mol_upload(h, charge, &m->charge)) || (rc = mol_upload(h, sigma, &m->sigma)) ||
-        (rc = mol_upload(h, eps, &m->eps)) || (rc = mol_upload(h, seps, &m->seps)) || (rc = mol_upload(h, b_off, &m->b_off)) || (rc = mol_upload(h, a_off, &m->a_off)) ||
-        (rc = mol_upload(h, t_off, &m->t_off)) || (rc = mol_upload(h, x_off, &m->x_off)) || (rc = mol_upload(h, c_off, &m->c_off)) ||
-        (rc = mol_upload(h, bonds, &m->bonds)) || (rc = mol_upload(h, angles, &m->angles)) || (rc = mol_upload(h, tors, &m->torsions)) ||
-        (rc = mol_upload(h, exc, &m->exc)) || (rc = mol_upload(h, cons, &m->cons)) || (rc = mol_upload(h, mask, &m->nb_mask)))
+    const std::vector<unsigned char> t32 = mol_pack<float>(L, eps), t64 = mol_pack<double>(L, eps);
+    m->bytes32 = (int)t32.size(); m->bytes64 = (int)t64.size();
+    m->n_tb = (int)L.b.size(); m->n_ta = (int)L.a.size(); m->n_tt = (int)L.t.size(); m->n_tp = (int)L.p.size(); m->n_slots = slot;
+    int rc = mol_check_shared(h, *m, nullptr, "rx_set_molecule: the term tables");
+    if (rc) { rxi_free_molecule(h); return rc; }
+    const unsigned char *d32 = nullptr, *d64 = nullptr;
+    if ((rc = mol_upload(h, mass, &m->mass)) || (rc = mol_upload(h, charge, &m->charge)) || (rc = mol_upload(h, c_off, &m->c_off)) ||
+        (rc = mol_upload(h, cons, &m->cons)) || (rc = mol_upload(h, t32, &d32)) || (rc = mol_upload(h, t64, &d64)))
         return rc;
+    m->terms32 = (const MolTerms *)d32; m->terms64 = (const MolTerms *)d64;
     h->have_particles = true;
     return RX_OK;
 }
@@ -1724,24 +1708,8 @@ int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s) {
     g.pre = -MOL_ONE_4PI_EPS0 * (1.0 / s->solute_dielectric - 1.0 / s->solvent_dielectric);
     g.on = 1;
     g.prop_bytes = (int)(sizeof(double) * (4 * (size_t)n * n + 3 * (size_t)n));
-    {
-        int dev = 0, optin = 0;
-        RX_CHECK_CUDA(h, cudaGetDevice(&dev));
-        RX_CHECK_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        const struct { const void *kern; int dyn; } use[] = {{(const void *)k_propagate_mol<true, true>, m->dyn_shared_bytes + g.prop_bytes},
-                                                             {(const void *)k_propagate_mol<false, true>, m->dyn_shared_bytes + g.prop_bytes},
-                                                             {(const void *)k_minimize_mol<true>, m->shared_bytes + MOL_GB_LANE_BYTES},
-                                                             {(const void *)k_energy_mol<true>, m->shared_bytes + MOL_GB_LANE_BYTES}};
-        size_t need = 0;
-        for (const auto &u : use) {
-            cudaFuncAttributes fa;
-            RX_CHECK_CUDA(h, cudaFuncGetAttributes(&fa, u.kern));
-            need = std::max(need, fa.sharedSizeBytes + (size_t)u.dyn);
-        }
-        if (need > (size_t)optin)
-            RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_implicit_solvent: the term and solvent tables need " + std::to_string(need) +
-                                               " bytes of shared memory per block, more than the device's " + std::to_string(optin));
-    }
+    const int rc = mol_check_shared(h, *m, &g, "rx_set_implicit_solvent: the term and solvent tables");
+    if (rc) return rc;
     void *d = nullptr;
     RX_CHECK_CUDA(h, cudaMalloc(&d, sizeof(double) * tab.size()));
     const cudaError_t e = cudaMemcpy(d, tab.data(), sizeof(double) * tab.size(), cudaMemcpyHostToDevice);

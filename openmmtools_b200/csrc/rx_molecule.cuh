@@ -17,47 +17,35 @@
 // cluster's <= 4 atoms, the RATTLE matrix inverted once per position update in closed form, SHAKE as chord iterations on that
 // inverse (k_propagate_mol<true>); larger clusters a Newton M-SHAKE (<= 4 constraints) or Gauss-Seidel sweeps
 // (k_propagate_mol<false>).  All of them reach the constrained point of oracle/rx_oracle_mol.c's sweeps to the tolerance.
-// The energy kernel (k_energy_mol, f64) and the minimiser (k_minimize_mol) use one warp per replica and the per-atom term
-// lists (a lane computes the terms that contain its atom).
+// The energy kernel (k_energy_mol) and the minimiser (k_minimize_mol) use one warp per replica and the same term list packed
+// in f64 (mol_terms<double, .>); the energy a launch of k_propagate_mol reports is k_energy_mol's function (mol_energy).
 #pragma once
 
 #define MOL_MAX_ATOMS 32
 #define MOL_ONE_4PI_EPS0 138.935456
 
-struct MolBond { int j, pad; double K, r0; };
-struct MolAngle { int i, j, k, role; double K, t0; };
-struct MolTorsion { int i, j, k, l, n, role; double phase, kk; };
-struct MolExc { int j, pad; double qq, sig, eps; };
 struct MolCons { int i, j; double d; };
 
-// Term tables of the dynamics' force evaluation: every bond / angle / torsion / interacting pair is evaluated ONCE, by
-// whichever lane its index falls to (t = lane, lane + 32, ...), in f32; its contributions go to fixed slots of a shared-memory
-// array and every atom then adds up ITS slots in slot order -- no atomics, the same bits every run.  (The per-atom
-// evaluation of mol_atom() runs each angle three and each torsion four times, with loops of unequal length per lane.)
-struct TBond { short i, j, si, sj; float K, r0; };
-struct TAngle { short i, j, k, si, sj, sk; float K, t0; };
-struct TTors { short i, j, k, l, si, sj, sk, sl; float n, phase, kk; };
-struct TPair { short i, j, si, sj; float qq, sig, eps; };   // qq = 138.935456 q_i q_j (exceptions: their own values)
+// The term list of a molecule, packed in the precision T of its evaluation: rx_set_molecule packs it twice in one layout, f32
+// for the dynamics' forces and f64 for the energies and the minimiser.  Every bond / angle / torsion / interacting pair is
+// evaluated ONCE, by whichever thread its index falls to; its contributions go to fixed slots of a shared-memory array and
+// every atom then adds up ITS slots in slot order -- no atomics, the same bits every run whatever the thread count.
+template <typename T> struct TBond { short i, j, si, sj; T K, r0; };
+template <typename T> struct TAngle { short i, j, k, si, sj, sk; T K, t0; };
+template <typename T> struct TTors { short i, j, k, l, si, sj, sk, sl; T n, phase, kk; };
+template <typename T> struct TPair { short i, j, si, sj; T qq, sig, eps; };   // qq = 138.935456 q_i q_j (exceptions: their own values)
 struct MolTerms {      // one contiguous blob: header, then the arrays (offsets in bytes from the blob's start)
-    int o_bond, o_angle, o_tors, o_pair, o_goff, pad[3];
+    int o_bond, o_angle, o_tors, o_pair, o_goff, pad[3];   // goff (at o_goff): atom a's slots are [goff[a], goff[a + 1])
 };
 
 struct MolDev {
     int n, n_clusters, remove_cm, max_cluster;   // max_cluster: constraints in the largest cluster
     double tol;
-    const double *mass, *charge, *sigma, *eps, *seps;
-    const int *b_off, *a_off, *t_off, *x_off, *c_off;
-    int b_off_h[MOL_MAX_ATOMS + 1], a_off_h[MOL_MAX_ATOMS + 1], t_off_h[MOL_MAX_ATOMS + 1], x_off_h[MOL_MAX_ATOMS + 1];   // (host copies: counts)
-    int shared_bytes;
-    const MolBond *bonds;
-    const MolAngle *angles;
-    const MolTorsion *torsions;
-    const MolExc *exc;
+    const double *mass, *charge;
+    const int *c_off;
     const MolCons *cons;
-    const unsigned *nb_mask;     // bit b of nb_mask[a]: the pair (a, b) has the plain Coulomb + LJ interaction
-    // term-parallel force evaluation of the dynamics (one entry per TERM, see mol_forces_terms)
-    const struct MolTerms *terms;
-    int terms_bytes, n_tb, n_ta, n_tt, n_tp, n_slots, dyn_shared_bytes;
+    const MolTerms *terms32, *terms64;   // the term list in f32 and in f64 (bytes32, bytes64: multiples of 16)
+    int bytes32, bytes64, n_tb, n_ta, n_tt, n_tp, n_slots;
 };
 
 // OBC generalized Born implicit solvent (rx_set_implicit_solvent), passed to the kernels as a trailing argument so that the
@@ -72,9 +60,14 @@ struct MolGB {
     const double *atom;   // [n][4]: rt, sr, rho, ace
     double alpha, beta, gamma, pre;
     int on;               // (0: vacuum; the GB = true kernels are only launched with 1)
-    int prop_bytes;       // k_propagate_mol<., true>'s arrays behind MolDev::dyn_shared_bytes
+    int prop_bytes;       // the arrays of MolGBArrays, behind the slots (mol_gb_at)
 };
-#define MOL_GB_LANE_BYTES (2 * MOL_MAX_ATOMS * 8)   // k_energy_mol / k_minimize_mol: B_i and C_i behind MolDev::shared_bytes
+
+// Dynamic shared memory of the molecule kernels: the staged term table (f32: k_propagate_mol, f64: k_energy_mol and
+// k_minimize_mol), then one double[3] per slot (k_propagate_mol: the float[3] forces of its steps, then the energy slots of
+// its final energy), then with GB the arrays of MolGBArrays.
+__host__ __device__ inline int mol_slots_at(const MolDev &m, bool f32) { return f32 ? m.bytes32 : m.bytes64; }
+__host__ __device__ inline int mol_gb_at(const MolDev &m, bool f32) { return mol_slots_at(m, f32) + 24 * m.n_slots; }
 
 // I_ij at distance r of atom i (offset radius rt) descreened by j (scaled radius sr); *dIdr its derivative.
 __device__ __forceinline__ double gb_descreen(double r, double rt, double sr, double *dIdr) {
@@ -116,236 +109,112 @@ __device__ __forceinline__ double gb_dist(const double (*X)[3], int i, int j, do
     return sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
 }
 
-// GB energy owned by lane a (its self and ACE terms, its pairs with larger partners) of one warp, one lane per atom, f64;
-// FORCES: f += the GB force on atom a.  Bs, Cs: double[MOL_MAX_ATOMS] in shared memory.  Every lane of the warp calls it.
-template <bool FORCES>
-__device__ double mol_gb_lane(const MolGB &g, const double (*X)[3], const double *q, int a, int n, double *Bs, double *Cs, double *f) {
-    const bool active = a < n;
-    double rt = 1.0, rho = 1.0, ace = 0.0, B = 1.0, dBdI = 0.0, e = 0.0, dEdB = 0.0, d[3], dI;
-    if (active) {
-        rt = g.atom[4 * a]; rho = g.atom[4 * a + 2]; ace = g.atom[4 * a + 3];
-        double I = 0.0;
-        for (int j = 0; j < n; j++) if (j != a) I += gb_descreen(gb_dist(X, a, j, d), rt, g.atom[4 * j + 1], &dI);
-        B = gb_born(g, I, rt, rho, &dBdI);
-        Bs[a] = B;
-    }
-    __syncwarp();
-    if (active) {
-        e = gb_self(g, q[a], B, rho, ace, &dEdB);
-        for (int j = 0; j < n; j++) {
-            if (j == a || (!FORCES && j < a)) continue;
-            const double r = gb_dist(X, a, j, d);
-            double dr, dbi, dbj;
-            const double ep = gb_pair(r * r, B, Bs[j], g.pre * q[a] * q[j], &dr, &dbi, &dbj);
-            if (j > a) e += ep;
-            if (FORCES) { dEdB += dbi; for (int c = 0; c < 3; c++) f[c] -= dr * d[c]; }
-        }
-        if (FORCES) Cs[a] = dEdB * dBdI;
-    }
-    if (FORCES) {
-        __syncwarp();
-        if (active) {
-            const double sa = g.atom[4 * a + 1];
-            for (int j = 0; j < n; j++) {
-                if (j == a) continue;
-                const double r = gb_dist(X, a, j, d);
-                double dIa, dIj;
-                gb_descreen(r, rt, g.atom[4 * j + 1], &dIa);
-                gb_descreen(r, g.atom[4 * j], sa, &dIj);
-                const double s = (Cs[a] * dIa + Cs[j] * dIj) / r;
-                for (int c = 0; c < 3; c++) f[c] -= s * d[c];
-            }
-        }
-        __syncwarp();
-    }
-    return e;
-}
-
 __device__ __forceinline__ void mol_cross(const double *a, const double *b, double *c) {
     c[0] = a[1] * b[2] - a[2] * b[1]; c[1] = a[2] * b[0] - a[0] * b[2]; c[2] = a[0] * b[1] - a[1] * b[0];
 }
 __device__ __forceinline__ double mol_dot(const double *a, const double *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
-// The term tables of one molecule in shared memory (a few KB: read every step by every lane).
-struct MolShared {
-    const MolBond *bonds; const MolAngle *angles; const MolTorsion *torsions; const MolExc *exc;
-    const int *b_off, *a_off, *t_off, *x_off;
-    const double *charge, *sigma, *seps;   // seps = sqrt(epsilon)
-    const unsigned *nb_mask;
-    int n;
-};
+// The f32 and f64 forms of the math of mol_terms (the f32 ones are those the dynamics has always used).
+__device__ __forceinline__ float mol_sqrt(float x) { return sqrtf(x); }
+__device__ __forceinline__ double mol_sqrt(double x) { return sqrt(x); }
+__device__ __forceinline__ float mol_rsqrt(float x) { return rsqrtf(x); }
+__device__ __forceinline__ double mol_rsqrt(double x) { return 1.0 / sqrt(x); }
+__device__ __forceinline__ float mol_clamp1(float x) { return fminf(1.f, fmaxf(-1.f, x)); }
+__device__ __forceinline__ double mol_clamp1(double x) { return x > 1.0 ? 1.0 : (x < -1.0 ? -1.0 : x); }
+__device__ __forceinline__ float mol_acos(float x) { return acosf(x); }
+__device__ __forceinline__ double mol_acos(double x) { return acos(x); }
+__device__ __forceinline__ float mol_atan2(float y, float x) { return atan2f(y, x); }
+__device__ __forceinline__ double mol_atan2(double y, double x) { return atan2(y, x); }
+__device__ __forceinline__ void mol_sincos(float x, float *s, float *c) { sincosf(x, s, c); }
+__device__ __forceinline__ void mol_sincos(double x, double *s, double *c) { sincos(x, s, c); }
 
-// Force on atom a (ENERGY: instead the energy of the terms this atom owns: bonds/exceptions/pairs with the larger partner
-// index, angles and torsions in which it has role 0).  X: positions of all atoms in shared memory.  In f64 (the dynamics'
-// forces are mol_forces_terms).
-template <bool ENERGY>
-__device__ double mol_atom(const MolShared &m, const double (*X)[3], int a, double *f) {
-    double e = 0.0;
-    double fx = 0, fy = 0, fz = 0;
-    const double xa[3] = {X[a][0], X[a][1], X[a][2]};
-    for (int q = m.b_off[a]; q < m.b_off[a + 1]; q++) {
-        const MolBond b = m.bonds[q];
-        const double d[3] = {xa[0] - X[b.j][0], xa[1] - X[b.j][1], xa[2] - X[b.j][2]};
-        const double r = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), dr = r - b.r0;
-        if (ENERGY) { if (b.j > a) e += 0.5 * b.K * dr * dr; }
-        else { const double c = -b.K * dr / r; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
-    }
-    for (int q = m.a_off[a]; q < m.a_off[a + 1]; q++) {
-        const MolAngle g = m.angles[q];
-        double u[3], v[3];
-        for (int c = 0; c < 3; c++) { u[c] = X[g.i][c] - X[g.j][c]; v[c] = X[g.k][c] - X[g.j][c]; }
-        const double ru2 = u[0] * u[0] + u[1] * u[1] + u[2] * u[2], rv2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
-        const double iruv = 1.0 / sqrt(ru2 * rv2);
-        double cs = (u[0] * v[0] + u[1] * v[1] + u[2] * v[2]) * iruv;
-        cs = cs > 1.0 ? 1.0 : (cs < -1.0 ? -1.0 : cs);
-        const double dt = acos(cs) - g.t0;
-        if (ENERGY) { if (g.role == 0) e += 0.5 * g.K * dt * dt; }
-        else {
-            const double sn = sqrt(1.0 - cs * cs);
-            const double gg = (sn > 1e-6) ? g.K * dt / sn : 0.0;
-            double o[3];
-            for (int c = 0; c < 3; c++) {
-                const double fi = gg * (v[c] * iruv - cs * u[c] / ru2);
-                const double fk = gg * (u[c] * iruv - cs * v[c] / rv2);
-                o[c] = g.role == 0 ? fi : (g.role == 2 ? fk : -(fi + fk));
-            }
-            fx += o[0]; fy += o[1]; fz += o[2];
-        }
-    }
-    for (int q = m.t_off[a]; q < m.t_off[a + 1]; q++) {
-        const MolTorsion t = m.torsions[q];
-        double rij[3], rkj[3], rkl[3], mm[3], nn[3];
-        for (int c = 0; c < 3; c++) { rij[c] = X[t.i][c] - X[t.j][c]; rkj[c] = X[t.k][c] - X[t.j][c]; rkl[c] = X[t.k][c] - X[t.l][c]; }
-        mm[0] = rij[1] * rkj[2] - rij[2] * rkj[1]; mm[1] = rij[2] * rkj[0] - rij[0] * rkj[2]; mm[2] = rij[0] * rkj[1] - rij[1] * rkj[0];
-        nn[0] = rkj[1] * rkl[2] - rkj[2] * rkl[1]; nn[1] = rkj[2] * rkl[0] - rkj[0] * rkl[2]; nn[2] = rkj[0] * rkl[1] - rkj[1] * rkl[0];
-        const double rkj2 = rkj[0] * rkj[0] + rkj[1] * rkj[1] + rkj[2] * rkj[2], nrkj = sqrt(rkj2);
-        const double phi = atan2(nrkj * (rij[0] * nn[0] + rij[1] * nn[1] + rij[2] * nn[2]), mm[0] * nn[0] + mm[1] * nn[1] + mm[2] * nn[2]);
-        double sn, cs;
-        sincos(t.n * phi - t.phase, &sn, &cs);
-        if (ENERGY) { if (t.role == 0) e += t.kk * (1.0 + cs); }
-        else {
-            const double dU = -t.kk * t.n * sn;
-            const double m2 = mm[0] * mm[0] + mm[1] * mm[1] + mm[2] * mm[2], n2 = nn[0] * nn[0] + nn[1] * nn[1] + nn[2] * nn[2];
-            const double pp = (rij[0] * rkj[0] + rij[1] * rkj[1] + rij[2] * rkj[2]) / rkj2, qq = (rkl[0] * rkj[0] + rkl[1] * rkj[1] + rkl[2] * rkj[2]) / rkj2;
-            const double ci = -dU * nrkj / m2, cl = dU * nrkj / n2;
-            double o[3];
-            for (int c = 0; c < 3; c++) {
-                const double fi = ci * mm[c], fl = cl * nn[c];
-                const double sv = pp * fi - qq * fl;
-                o[c] = t.role == 0 ? fi : (t.role == 1 ? sv - fi : (t.role == 2 ? -sv - fl : fl));
-            }
-            fx += o[0]; fy += o[1]; fz += o[2];
-        }
-    }
-    const unsigned mask = m.nb_mask[a];
-    const double qa = MOL_ONE_4PI_EPS0 * m.charge[a], sa = m.sigma[a], ea = m.seps[a];
-    for (int b = 0; b < m.n; b++) {
-        if (!((mask >> b) & 1u)) continue;
-        if (ENERGY && b < a) continue;
-        const double d[3] = {xa[0] - X[b][0], xa[1] - X[b][1], xa[2] - X[b][2]};
-        const double ir2 = 1.0 / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = sqrt(ir2);
-        const double qq = qa * m.charge[b], s = 0.5 * (sa + m.sigma[b]), ee = ea * m.seps[b];
-        const double s2 = s * s * ir2, s6 = s2 * s2 * s2;
-        if (ENERGY) e += qq * ir + 4.0 * ee * (s6 * s6 - s6);
-        else { const double c = (qq * ir + 24.0 * ee * (2.0 * s6 * s6 - s6)) * ir2; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
-    }
-    for (int q = m.x_off[a]; q < m.x_off[a + 1]; q++) {
-        const MolExc x = m.exc[q];
-        if (ENERGY && x.j < a) continue;
-        const double d[3] = {xa[0] - X[x.j][0], xa[1] - X[x.j][1], xa[2] - X[x.j][2]};
-        const double ir2 = 1.0 / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = sqrt(ir2);
-        const double qq = MOL_ONE_4PI_EPS0 * x.qq;
-        const double s2 = (x.sig * x.sig) * ir2, s6 = s2 * s2 * s2;
-        if (ENERGY) e += qq * ir + 4.0 * x.eps * (s6 * s6 - s6);
-        else { const double c = (qq * ir + 24.0 * x.eps * (2.0 * s6 * s6 - s6)) * ir2; fx += c * d[0]; fy += c * d[1]; fz += c * d[2]; }
-    }
-    if (!ENERGY) { f[0] = fx; f[1] = fy; f[2] = fz; }
-    return e;
+// Stage a term table (bytes: a multiple of 16) into shared memory; every thread of the block.
+__device__ __forceinline__ void mol_stage(unsigned char *dst, const MolTerms *src, int bytes) {
+    for (int q = threadIdx.x * 8; q < bytes; q += blockDim.x * 8) *(unsigned long long *)(dst + q) = *(const unsigned long long *)((const unsigned char *)src + q);
 }
 
-// All terms, each once (see MolTerms).  FS: float[n_slots][3] in shared memory.
-__device__ __forceinline__ void mol_forces_terms(const MolDev &m, const unsigned char *tb, const double (*X)[3], float (*FS)[3]) {
+// All terms of the table tb, each once, by every thread of the block (the f64 table: T = double).  Forces: S[slot] = the
+// term's force on that atom.  ENERGY (T = double): the term's energy goes to the slot of its owner -- the smaller atom index
+// of a bond or pair, role 0 of an angle or torsion -- as the two factors x, y of its last product, so that the owner's sum
+// e = fma(x, y, e) over its slots in slot order (mol_energy) rounds as one fused multiply-add per term; its other slots get 0.
+template <typename T, bool ENERGY>
+__device__ __forceinline__ void mol_terms(const MolDev &m, const unsigned char *tb, const double (*X)[3], T (*S)[3]) {
     const MolTerms *h = (const MolTerms *)tb;
     const int lane = threadIdx.x, nth = blockDim.x;   // (k_propagate_mol: all warps of the block; the other kernels: one warp)
-    const TBond *B = (const TBond *)(tb + h->o_bond);
+    auto energy = [&](int s, bool own, T x, T y) { S[s][0] = own ? x : T(0); S[s][1] = own ? y : T(0); };
+    const TBond<T> *B = (const TBond<T> *)(tb + h->o_bond);
     // (which thread evaluates a term does not matter for the result -- fixed slots; the four kinds start at different threads so
     // that no thread gets a torsion AND an angle AND two pairs: the evaluation is as long as its busiest thread)
     for (int t = (lane + nth / 2) % nth; t < m.n_tb; t += nth) {
-        const TBond b = B[t];
-        const float d[3] = {(float)(X[b.i][0] - X[b.j][0]), (float)(X[b.i][1] - X[b.j][1]), (float)(X[b.i][2] - X[b.j][2])};
-        const float r = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-        const float c = -b.K * (r - b.r0) / r;
-        for (int q = 0; q < 3; q++) { FS[b.si][q] = c * d[q]; FS[b.sj][q] = -c * d[q]; }
-    }
-    const TAngle *A = (const TAngle *)(tb + h->o_angle);
-    for (int t = nth - 1 - lane; t < m.n_ta; t += nth) {
-        const TAngle g = A[t];
-        float u[3], v[3];
-        for (int c = 0; c < 3; c++) { u[c] = (float)(X[g.i][c] - X[g.j][c]); v[c] = (float)(X[g.k][c] - X[g.j][c]); }
-        const float ru2 = u[0] * u[0] + u[1] * u[1] + u[2] * u[2], rv2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
-        const float iruv = rsqrtf(ru2 * rv2);
-        float cs = (u[0] * v[0] + u[1] * v[1] + u[2] * v[2]) * iruv;
-        cs = fminf(1.f, fmaxf(-1.f, cs));
-        const float dt = acosf(cs) - g.t0, sn = sqrtf(1.f - cs * cs);
-        const float gg = (sn > 1e-6f) ? g.K * dt / sn : 0.f;
-        for (int c = 0; c < 3; c++) {
-            const float fi = gg * (v[c] * iruv - cs * u[c] / ru2), fk = gg * (u[c] * iruv - cs * v[c] / rv2);
-            FS[g.si][c] = fi; FS[g.sk][c] = fk; FS[g.sj][c] = -(fi + fk);
+        const TBond<T> b = B[t];
+        const T d[3] = {(T)(X[b.i][0] - X[b.j][0]), (T)(X[b.i][1] - X[b.j][1]), (T)(X[b.i][2] - X[b.j][2])};
+        const T r = mol_sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+        if (ENERGY) {
+            const T dr = r - b.r0;
+            energy(b.si, b.i < b.j, T(0.5) * b.K * dr, dr); energy(b.sj, b.j < b.i, T(0.5) * b.K * dr, dr);
+        } else {
+            const T c = -b.K * (r - b.r0) / r;
+            for (int q = 0; q < 3; q++) { S[b.si][q] = c * d[q]; S[b.sj][q] = -c * d[q]; }
         }
     }
-    const TTors *T = (const TTors *)(tb + h->o_tors);
+    const TAngle<T> *A = (const TAngle<T> *)(tb + h->o_angle);
+    for (int t = nth - 1 - lane; t < m.n_ta; t += nth) {
+        const TAngle<T> g = A[t];
+        T u[3], v[3];
+        for (int c = 0; c < 3; c++) { u[c] = (T)(X[g.i][c] - X[g.j][c]); v[c] = (T)(X[g.k][c] - X[g.j][c]); }
+        const T ru2 = u[0] * u[0] + u[1] * u[1] + u[2] * u[2], rv2 = v[0] * v[0] + v[1] * v[1] + v[2] * v[2];
+        const T iruv = mol_rsqrt(ru2 * rv2);
+        const T cs = mol_clamp1((u[0] * v[0] + u[1] * v[1] + u[2] * v[2]) * iruv);
+        const T dt = mol_acos(cs) - g.t0;
+        if (ENERGY) {
+            energy(g.si, true, T(0.5) * g.K * dt, dt); energy(g.sj, false, 0, 0); energy(g.sk, false, 0, 0);
+        } else {
+            const T sn = mol_sqrt(T(1) - cs * cs);
+            const T gg = (sn > T(1e-6)) ? g.K * dt / sn : T(0);
+            for (int c = 0; c < 3; c++) {
+                const T fi = gg * (v[c] * iruv - cs * u[c] / ru2), fk = gg * (u[c] * iruv - cs * v[c] / rv2);
+                S[g.si][c] = fi; S[g.sk][c] = fk; S[g.sj][c] = -(fi + fk);
+            }
+        }
+    }
+    const TTors<T> *W = (const TTors<T> *)(tb + h->o_tors);
     for (int t = lane; t < m.n_tt; t += nth) {
-        const TTors w = T[t];
-        float rij[3], rkj[3], rkl[3], mm[3], nn[3];
-        for (int c = 0; c < 3; c++) { rij[c] = (float)(X[w.i][c] - X[w.j][c]); rkj[c] = (float)(X[w.k][c] - X[w.j][c]); rkl[c] = (float)(X[w.k][c] - X[w.l][c]); }
+        const TTors<T> w = W[t];
+        T rij[3], rkj[3], rkl[3], mm[3], nn[3];
+        for (int c = 0; c < 3; c++) { rij[c] = (T)(X[w.i][c] - X[w.j][c]); rkj[c] = (T)(X[w.k][c] - X[w.j][c]); rkl[c] = (T)(X[w.k][c] - X[w.l][c]); }
         mm[0] = rij[1] * rkj[2] - rij[2] * rkj[1]; mm[1] = rij[2] * rkj[0] - rij[0] * rkj[2]; mm[2] = rij[0] * rkj[1] - rij[1] * rkj[0];
         nn[0] = rkj[1] * rkl[2] - rkj[2] * rkl[1]; nn[1] = rkj[2] * rkl[0] - rkj[0] * rkl[2]; nn[2] = rkj[0] * rkl[1] - rkj[1] * rkl[0];
-        const float rkj2 = rkj[0] * rkj[0] + rkj[1] * rkj[1] + rkj[2] * rkj[2], nrkj = sqrtf(rkj2);
-        const float phi = atan2f(nrkj * (rij[0] * nn[0] + rij[1] * nn[1] + rij[2] * nn[2]), mm[0] * nn[0] + mm[1] * nn[1] + mm[2] * nn[2]);
-        float sn, cs;
-        sincosf(w.n * phi - w.phase, &sn, &cs);
-        const float dU = -w.kk * w.n * sn;
-        const float m2 = mm[0] * mm[0] + mm[1] * mm[1] + mm[2] * mm[2], n2 = nn[0] * nn[0] + nn[1] * nn[1] + nn[2] * nn[2];
-        const float pp = (rij[0] * rkj[0] + rij[1] * rkj[1] + rij[2] * rkj[2]) / rkj2, qq = (rkl[0] * rkj[0] + rkl[1] * rkj[1] + rkl[2] * rkj[2]) / rkj2;
-        const float ci = -dU * nrkj / m2, cl = dU * nrkj / n2;
-        for (int c = 0; c < 3; c++) {
-            const float fi = ci * mm[c], fl = cl * nn[c], sv = pp * fi - qq * fl;
-            FS[w.si][c] = fi; FS[w.sj][c] = sv - fi; FS[w.sk][c] = -sv - fl; FS[w.sl][c] = fl;
+        const T rkj2 = rkj[0] * rkj[0] + rkj[1] * rkj[1] + rkj[2] * rkj[2], nrkj = mol_sqrt(rkj2);
+        const T phi = mol_atan2(nrkj * (rij[0] * nn[0] + rij[1] * nn[1] + rij[2] * nn[2]), mm[0] * nn[0] + mm[1] * nn[1] + mm[2] * nn[2]);
+        T sn, cs;
+        mol_sincos(w.n * phi - w.phase, &sn, &cs);
+        if (ENERGY) {
+            energy(w.si, true, w.kk, T(1) + cs); energy(w.sj, false, 0, 0); energy(w.sk, false, 0, 0); energy(w.sl, false, 0, 0);
+        } else {
+            const T dU = -w.kk * w.n * sn;
+            const T m2 = mm[0] * mm[0] + mm[1] * mm[1] + mm[2] * mm[2], n2 = nn[0] * nn[0] + nn[1] * nn[1] + nn[2] * nn[2];
+            const T pp = (rij[0] * rkj[0] + rij[1] * rkj[1] + rij[2] * rkj[2]) / rkj2, qq = (rkl[0] * rkj[0] + rkl[1] * rkj[1] + rkl[2] * rkj[2]) / rkj2;
+            const T ci = -dU * nrkj / m2, cl = dU * nrkj / n2;
+            for (int c = 0; c < 3; c++) {
+                const T fi = ci * mm[c], fl = cl * nn[c], sv = pp * fi - qq * fl;
+                S[w.si][c] = fi; S[w.sj][c] = sv - fi; S[w.sk][c] = -sv - fl; S[w.sl][c] = fl;
+            }
         }
     }
-    const TPair *P = (const TPair *)(tb + h->o_pair);
+    const TPair<T> *P = (const TPair<T> *)(tb + h->o_pair);
     for (int t = ((lane - m.n_tt) % nth + nth) % nth; t < m.n_tp; t += nth) {
-        const TPair p = P[t];
-        const float d[3] = {(float)(X[p.i][0] - X[p.j][0]), (float)(X[p.i][1] - X[p.j][1]), (float)(X[p.i][2] - X[p.j][2])};
-        const float ir2 = 1.f / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = sqrtf(ir2);
-        const float s2 = p.sig * p.sig * ir2, s6 = s2 * s2 * s2;
-        const float c = (p.qq * ir + 24.f * p.eps * (2.f * s6 * s6 - s6)) * ir2;
-        for (int q = 0; q < 3; q++) { FS[p.si][q] = c * d[q]; FS[p.sj][q] = -c * d[q]; }
+        const TPair<T> p = P[t];
+        const T d[3] = {(T)(X[p.i][0] - X[p.j][0]), (T)(X[p.i][1] - X[p.j][1]), (T)(X[p.i][2] - X[p.j][2])};
+        const T ir2 = T(1) / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), ir = mol_sqrt(ir2);
+        const T s2 = p.sig * p.sig * ir2, s6 = s2 * s2 * s2;
+        if (ENERGY) {
+            const T e = p.qq * ir + T(4) * p.eps * (s6 * s6 - s6);
+            energy(p.si, p.i < p.j, e, 1); energy(p.sj, p.j < p.i, e, 1);
+        } else {
+            const T c = (p.qq * ir + T(24) * p.eps * (T(2) * s6 * s6 - s6)) * ir2;
+            for (int q = 0; q < 3; q++) { S[p.si][q] = c * d[q]; S[p.sj][q] = -c * d[q]; }
+        }
     }
-}
-
-// Copy the term tables into shared memory (all lanes of the warp; `buf` has room for mol_shared_bytes(m)).
-__device__ void mol_stage(const MolDev &m, unsigned char *buf, MolShared &s) {
-    const int n = m.n, lane = threadIdx.x;
-    const size_t stride = (size_t)blockDim.x * 8;
-    auto put = [&](const void *src, size_t bytes) {
-        unsigned char *dst = buf;
-        for (size_t q = lane * 8; q < bytes; q += stride) *(unsigned long long *)(dst + q) = *(const unsigned long long *)((const unsigned char *)src + q);
-        buf += (bytes + 15) & ~(size_t)15;
-        return dst;
-    };
-    s.n = n;
-    const int nb = m.b_off_h[n], na = m.a_off_h[n], nt = m.t_off_h[n], nx = m.x_off_h[n];
-    s.bonds = (const MolBond *)put(m.bonds, sizeof(MolBond) * nb);
-    s.angles = (const MolAngle *)put(m.angles, sizeof(MolAngle) * na);
-    s.torsions = (const MolTorsion *)put(m.torsions, sizeof(MolTorsion) * nt);
-    s.exc = (const MolExc *)put(m.exc, sizeof(MolExc) * nx);
-    s.b_off = (const int *)put(m.b_off, sizeof(int) * (n + 2)); s.a_off = (const int *)put(m.a_off, sizeof(int) * (n + 2));
-    s.t_off = (const int *)put(m.t_off, sizeof(int) * (n + 2)); s.x_off = (const int *)put(m.x_off, sizeof(int) * (n + 2));
-    s.charge = (const double *)put(m.charge, sizeof(double) * n); s.sigma = (const double *)put(m.sigma, sizeof(double) * n);
-    s.seps = (const double *)put(m.seps, sizeof(double) * n);
-    s.nb_mask = (const unsigned *)put(m.nb_mask, sizeof(unsigned) * (n + 1));
-    if (blockDim.x > 32) __syncthreads(); else __syncwarp();
 }
 
 // Constraints are solved per cluster (connected component of the constraint graph) by ONE lane.  Clusters of up to
@@ -702,31 +571,37 @@ __device__ __forceinline__ double mol_warp_sum(double v) {   // fixed tree: bit-
     return v;
 }
 
-// k_propagate_mol's GB force, pair-parallel over the block, in the arrays of MolGB::prop_bytes: n x n matrices I_ij, dI_ij/dr,
-// the pair's dE/dr / r (symmetric) and dE_pair/dB_i, then B_i, dB_i/dI_i and C_i = dE/dB_i dB_i/dI_i.  Every entry is written by
-// one thread and every atom adds up its row in index order: no atomics, the same bits whatever the thread count.
+// The GB terms, pair-parallel over the block, in the arrays of MolGB::prop_bytes: n x n matrices I_ij, dI_ij/dr, the pair's
+// dE/dr / r (symmetric; ENERGY: the pair's energy for j > i) and dE_pair/dB_i, then B_i, dB_i/dI_i and C_i = dE/dB_i dB_i/dI_i.
+// Every entry is written by one thread and every atom adds up its row in index order: no atomics, the same bits whatever the
+// thread count.
 struct MolGBArrays {
     double *I, *D, *P, *EB, *B, *dB, *C;
     __device__ MolGBArrays(double *s, int n) : I(s), D(s + n * n), P(s + 2 * n * n), EB(s + 3 * n * n), B(s + 4 * n * n), dB(B + n), C(dB + n) {}
 };
 
 // phase 1 (before the barrier that ends the term evaluation): the descreening integrals of the ordered pairs
+template <bool ENERGY>
 __device__ __forceinline__ void mol_gb_integrals(const MolGB &g, const double (*X)[3], int n, const MolGBArrays &s) {
     for (int t = threadIdx.x; t < n * n; t += blockDim.x) {
         const int i = t / n, j = t - i * n;
         double d[3], dI = 0.0, I = 0.0;
         if (i != j) I = gb_descreen(gb_dist(X, i, j, d), g.atom[4 * i], g.atom[4 * j + 1], &dI);
-        s.I[t] = I; s.D[t] = dI;
+        s.I[t] = I;
+        if (!ENERGY) s.D[t] = dI;
     }
 }
 
-// phases 2 and 3 (after it; every thread of the block): Born radii, the pair terms, the chain-rule factors C_i
-__device__ __forceinline__ void mol_gb_radii_pairs(const MolGB &g, const double (*X)[3], const double *q, int n, const MolGBArrays &s) {
+// phases 2 and 3 (after it; every thread of the block): Born radii, the pair terms, then the chain-rule factors C_i or, ENERGY,
+// the GB energy atom a < n owns (returned): its self and ACE terms, then its pairs with larger partners in index order.
+template <bool ENERGY>
+__device__ __forceinline__ double mol_gb_radii_pairs(const MolGB &g, const double (*X)[3], const double *q, int n, const MolGBArrays &s) {
     const int a = threadIdx.x;
     if (a < n) {
-        double I = 0.0;
+        double I = 0.0, dB;
         for (int j = 0; j < n; j++) I += s.I[a * n + j];
-        s.B[a] = gb_born(g, I, g.atom[4 * a], g.atom[4 * a + 2], &s.dB[a]);
+        s.B[a] = gb_born(g, I, g.atom[4 * a], g.atom[4 * a + 2], &dB);
+        if (!ENERGY) s.dB[a] = dB;
     }
     __syncthreads();
     for (int t = threadIdx.x; t < n * n; t += blockDim.x) {
@@ -734,25 +609,24 @@ __device__ __forceinline__ void mol_gb_radii_pairs(const MolGB &g, const double 
         if (j <= i) continue;
         double d[3], dr, dbi, dbj;
         const double r = gb_dist(X, i, j, d);
-        gb_pair(r * r, s.B[i], s.B[j], g.pre * q[i] * q[j], &dr, &dbi, &dbj);
-        s.P[t] = s.P[j * n + i] = dr; s.EB[t] = dbi; s.EB[j * n + i] = dbj;
+        const double e = gb_pair(r * r, s.B[i], s.B[j], g.pre * q[i] * q[j], &dr, &dbi, &dbj);
+        if (ENERGY) s.P[t] = e;
+        else { s.P[t] = s.P[j * n + i] = dr; s.EB[t] = dbi; s.EB[j * n + i] = dbj; }
     }
     __syncthreads();
+    double e = 0.0;
     if (a < n) {
         double dEdB;
-        gb_self(g, q[a], s.B[a], g.atom[4 * a + 2], g.atom[4 * a + 3], &dEdB);
-        for (int j = 0; j < n; j++) if (j != a) dEdB += s.EB[a * n + j];
-        s.C[a] = dEdB * s.dB[a];
+        e = gb_self(g, q[a], s.B[a], g.atom[4 * a + 2], g.atom[4 * a + 3], &dEdB);
+        if (ENERGY) {
+            for (int j = a + 1; j < n; j++) e += s.P[a * n + j];
+        } else {
+            for (int j = 0; j < n; j++) if (j != a) dEdB += s.EB[a * n + j];
+            s.C[a] = dEdB * s.dB[a];
+        }
     }
     __syncwarp();
-}
-
-// U of a molecule in implicit solvent (every lane of a warp; the same bits in k_propagate_mol and k_energy_mol)
-__device__ __forceinline__ double mol_energy_gb(const MolDev &m, const MolGB &g, const MolShared &ms, const double (*X)[3], double *Bs,
-                                                double *Cs) {
-    const int a = threadIdx.x;
-    const double e_gb = mol_gb_lane<false>(g, X, ms.charge, a, m.n, Bs, Cs, nullptr);
-    return mol_warp_sum(a < m.n ? mol_atom<true>(ms, X, a, nullptr) + e_gb : 0.0);
+    return e;
 }
 
 // the GB force on atom a (warp 0, after mol_gb_radii_pairs)
@@ -764,6 +638,23 @@ __device__ __forceinline__ void mol_gb_force(const double (*X)[3], int a, int n,
         const double c = s.P[a * n + j] + (s.C[a] * s.D[a * n + j] + s.C[j] * s.D[j * n + a]) / r;
         for (int q = 0; q < 3; q++) f[q] -= c * d[q];
     }
+}
+
+// U of the molecule at X from the f64 term table t64, in k_energy_mol and at the end of k_propagate_mol (the same function:
+// the same bits).  Every thread of the block calls it after a block barrier; S: double[n_slots][3] with, GB, the arrays of gs
+// behind them.  The result is warp 0's.
+template <bool GB>
+__device__ __forceinline__ double mol_energy(const MolDev &m, const MolGB &g, const unsigned char *t64, const double (*X)[3],
+                                             double (*S)[3], const MolGBArrays &gs) {
+    mol_terms<double, true>(m, t64, X, S);
+    if (GB) mol_gb_integrals<true>(g, X, m.n, gs);
+    __syncthreads();
+    const double e_gb = GB ? mol_gb_radii_pairs<true>(g, X, m.charge, m.n, gs) : 0.0;
+    const int a = threadIdx.x, *goff = (const int *)(t64 + ((const MolTerms *)t64)->o_goff);
+    double e = 0.0;
+    if (a < m.n)
+        for (int q = goff[a]; q < goff[a + 1]; q++) e = fma(S[q][0], S[q][1], e);
+    return mol_warp_sum(a < m.n ? (GB ? e + e_gb : e) : 0.0);
 }
 
 // One block of MOL_WARPS warps per owned replica.  Warp 0 integrates (one lane per atom, one lane per constraint cluster);
@@ -787,13 +678,11 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
     extern __shared__ unsigned long long mol_tab[];
     const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
     if (only && !only[k]) return;
-    MolShared ms;
-    mol_stage(m, (unsigned char *)mol_tab, ms);
-    // the dynamics' term tables and the slots of their force contributions, behind the other tables
-    unsigned char *tb = (unsigned char *)mol_tab + m.shared_bytes;
-    for (int q = threadIdx.x * 8; q < m.terms_bytes; q += 32 * MOL_WARPS * 8) *(unsigned long long *)(tb + q) = *(const unsigned long long *)((const unsigned char *)m.terms + q);
-    float (*FS)[3] = (float (*)[3])(tb + ((m.terms_bytes + 15) & ~15));
-    const MolGBArrays gs((double *)((unsigned char *)mol_tab + m.dyn_shared_bytes), n);
+    // the f32 term table and the slots of its force contributions
+    unsigned char *tb = (unsigned char *)mol_tab;
+    mol_stage(tb, m.terms32, m.bytes32);
+    float (*FS)[3] = (float (*)[3])(tb + mol_slots_at(m, true));
+    const MolGBArrays gs((double *)(tb + mol_gb_at(m, true)), n);
     __syncthreads();
     const int *g_off = (const int *)(tb + ((const MolTerms *)tb)->o_goff);
     const bool active = a < n;
@@ -834,10 +723,10 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
             if (op == 'V') {
                 if (!f_valid) {
                     __syncthreads();   // warp 0's positions are in shared memory
-                    mol_forces_terms(m, tb, X, FS);
-                    if (GB) mol_gb_integrals(g, X, n, gs);
+                    mol_terms<float, false>(m, tb, X, FS);
+                    if (GB) mol_gb_integrals<false>(g, X, n, gs);
                     __syncthreads();   // every term's contributions are in their slots
-                    if (GB) mol_gb_radii_pairs(g, X, ms.charge, n, gs);
+                    if (GB) mol_gb_radii_pairs<false>(g, X, m.charge, n, gs);
                     if (active) {   // this atom's slots, in slot order
                         float fx = 0.f, fy = 0.f, fz = 0.f;
                         for (int q = g_off[a]; q < g_off[a + 1]; q++) { fx += FS[q][0]; fy += FS[q][1]; fz += FS[q][2]; }
@@ -878,12 +767,14 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
             }
         }
     }
-    const double U = GB ? mol_energy_gb(m, g, ms, X, gs.B, gs.C) : mol_warp_sum(active ? mol_atom<true>(ms, X, a, nullptr) : 0.0);
+    __syncthreads();   // warp 0's final positions; the force slots are free for the energy's
+    const double U = mol_energy<GB>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs);
     const double KE = mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
     const bool bad = active && !(isfinite(X[a][0]) && isfinite(X[a][1]) && isfinite(X[a][2]) && isfinite(V[a][0]) &&
                                  isfinite(V[a][1]) && isfinite(V[a][2]));
     const unsigned any_bad = __ballot_sync(0xffffffffu, bad);
-    if (a == 0) { pot[k] = U + st.offset; kin[k] = KE; nan_flag[k] = (any_bad || !isfinite(U)) ? 1 : 0; }
+    // (the offset read again: kept in registers across the steps, it costs k_propagate_mol<false, true> a spill)
+    if (a == 0) { pot[k] = U + states[perm[k]].offset; kin[k] = KE; nan_flag[k] = (any_bad || !isfinite(U)) ? 1 : 0; }
     if (active)
         for (int c = 0; c < 3; c++) { pos[((size_t)r * n + a) * 3 + c] = X[a][c]; vel[((size_t)r * n + a) * 3 + c] = V[a][c]; }
 }
@@ -893,7 +784,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
 // weights, unit-weight sweeps for clusters of more than MOL_MAXC constraints), the move is followed by SHAKE, the FIRE
 // velocity is kept tangent.  Converged when the RMS of the projected force
 // falls below tol_rms (kJ/mol/nm); f64 throughout.  (OpenMM's L-BFGS is not reproduced, as for the other systems.)
-// GB: the OBC force of g added to each atom's (mol_gb_lane, f64).
+// GB: the OBC force of g added to each atom's (mol_gb_radii_pairs, mol_gb_force).
 template <bool GB>
 __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restrict__ pos, int k0, double tol_rms, int max_iter,
                                                      double *__restrict__ rms_out, int *__restrict__ iters_out, MolGB g) {
@@ -901,8 +792,11 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
     extern __shared__ unsigned long long mol_tab[];
     const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
     const bool active = a < n;
-    MolShared ms;
-    mol_stage(m, (unsigned char *)mol_tab, ms);
+    unsigned char *tb = (unsigned char *)mol_tab;
+    mol_stage(tb, m.terms64, m.bytes64);
+    double (*FS)[3] = (double (*)[3])(tb + mol_slots_at(m, false));
+    const MolGBArrays gs((double *)(tb + mol_gb_at(m, false)), n);
+    const int *goff = (const int *)(tb + ((const MolTerms *)tb)->o_goff);
     MolCluster kc, ku;   // the cluster with its masses (SHAKE) and with unit weights (projections)
     kc.nc = ku.nc = 0;
     if (a < m.n_clusters) {
@@ -929,10 +823,13 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
     int n_pos = 0, it = 0;
     for (;; it++) {
         double f[3] = {0, 0, 0};
-        if (active) mol_atom<false>(ms, X, a, f);
-        if (GB) {
-            double *gbs = (double *)((unsigned char *)mol_tab + m.shared_bytes);
-            mol_gb_lane<true>(g, X, ms.charge, a, n, gbs, gbs + MOL_MAX_ATOMS, f);
+        mol_terms<double, false>(m, tb, X, FS);
+        if (GB) mol_gb_integrals<false>(g, X, n, gs);
+        __syncwarp();   // every term's contributions are in their slots
+        if (GB) mol_gb_radii_pairs<false>(g, X, m.charge, n, gs);
+        if (active) {   // this atom's slots, in slot order
+            for (int q = goff[a]; q < goff[a + 1]; q++) for (int c = 0; c < 3; c++) f[c] += FS[q][c];
+            if (GB) mol_gb_force(X, a, n, gs, f);
         }
         if (active) for (int c = 0; c < 3; c++) F[a][c] = f[c];
         __syncwarp();
@@ -973,21 +870,19 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
 
 // u[k][l] = beta_l (U(x_k) + offset_l): the states of a molecule differ in temperature only (parallel tempering,
 // paralleltempering.py:175-237: one potential evaluation per replica, scaled by beta_l).
-// GB: with the OBC energy of g (mol_energy_gb).
+// GB: with the OBC energy of g.
 template <bool GB>
 __global__ void __launch_bounds__(32) k_energy_mol(MolDev m, const StateDev *__restrict__ states, int n_states,
                                                    const double *__restrict__ pos, int k0, double *__restrict__ u_out, MolGB g) {
     __shared__ double X[MOL_MAX_ATOMS][3];
     extern __shared__ unsigned long long mol_tab[];
     const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
-    const bool active = a < n;
-    MolShared ms;
-    mol_stage(m, (unsigned char *)mol_tab, ms);
-    if (active) for (int c = 0; c < 3; c++) X[a][c] = pos[((size_t)r * n + a) * 3 + c];
-    __syncwarp();
-    double *gbs = (double *)((unsigned char *)mol_tab + m.shared_bytes);
-    const double U = GB ? mol_energy_gb(m, g, ms, X, gbs, gbs + MOL_MAX_ATOMS)
-                        : mol_warp_sum(active ? mol_atom<true>(ms, X, a, nullptr) : 0.0);
+    unsigned char *tb = (unsigned char *)mol_tab;
+    mol_stage(tb, m.terms64, m.bytes64);
+    if (a < n) for (int c = 0; c < 3; c++) X[a][c] = pos[((size_t)r * n + a) * 3 + c];
+    __syncthreads();
+    const double U = mol_energy<GB>(m, g, tb, X, (double (*)[3])(tb + mol_slots_at(m, false)),
+                                    MolGBArrays((double *)(tb + mol_gb_at(m, false)), n));
     for (int l = a; l < n_states; l += 32) u_out[(size_t)k * n_states + l] = states[l].beta * (U + states[l].offset);
 }
 

@@ -194,6 +194,12 @@ def check_long_launch(name):
     assert np.array_equal(xa, xb) and np.array_equal(va, vb) and np.array_equal(pa, pb)     # bit-reproducible
     assert constraint_error(system, xa) < 1e-9
     assert np.all(np.isfinite(pa)) and np.all(ka > 0)
+    # the replica energies the launch reports are the energy kernel's (u = beta U: equal up to the rounding of beta)
+    e = make_engine(system, temps)
+    e.set_positions(xa)
+    u = e.compute_energies()
+    e.close()
+    assert np.abs(u[np.arange(K), np.arange(K)] * KB * temps - pa).max() <= 1e-14 * np.abs(pa).max()
     if system.n_particles >= 14:
         # hotter replicas have more kinetic energy on average (alanine dipeptide: 51 degrees of freedom each)
         assert ka[-3:].mean() > ka[:3].mean()
