@@ -168,6 +168,42 @@ RX_API int rx_set_integrator(rx_engine *h, double timestep, double collision_rat
 RX_API int rx_set_state_integrator(rx_engine *h, int32_t state, double timestep, double collision_rate, int32_t n_steps,
                                    const char *splitting, int32_t reassign_velocities);
 
+/* ---- Monte Carlo rigid-body moves (MCDisplacementMove, MCRotationMove: mcmc.py:810-970, 1704-1911) ------------------ */
+/* Up to RX_MAX_MC_MOVES Metropolized moves per thermodynamic state, applied in order to every replica in that state at the
+ * start of rx_propagate (before its snapshot, so rx_propagate_retry reruns the dynamics only, from the post-MC state) and of
+ * every iteration of rx_run_iterations / rx_sams_run_iterations.  One proposal per move and replica:
+ *   RX_MC_DISPLACEMENT  the subset moves by sigma_nm * (three standard normals);
+ *   RX_MC_ROTATION      the subset turns about its geometric centre by a uniform random rotation (Shoemake's quaternion).
+ *                       On a periodic box the subset is first made whole by minimum image relative to its first atom, and
+ *                       the proposal is rejected when a rotated offset from that atom reaches half a box edge.
+ * The proposal is accepted iff dU is finite and beta dU <= 0 or u < exp(-beta dU), beta and U of the replica's state; positions
+ * stay f32 (a molecule's f64), and a periodic system's are wrapped into the box as rx_propagate wraps them.  Randoms: Philox4x32-10 keyed as rx_propagate's noise, counter (slot, 0xE0000000, replica,
+ * iteration) for the proposal and (slot, 0xE0000001, replica, iteration) for u.
+ * rx_set_mc_subsets      the atom indices every move's subset points into (subset_offset, subset_len); replaces the previous
+ *                        array and removes every move set so far.
+ * rx_set_state_mc_moves  the n moves of `state` (-1: every state); n = 0 removes them.  RX_ERR_UNSUPPORTED when a subset of a
+ *                        molecule contains part of a constraint cluster (a rigid move keeps the constraints only when it moves
+ *                        whole clusters).
+ * rx_get_mc_statistics / rx_set_mc_statistics  accepted and proposed counts [M][RX_MAX_MC_MOVES] of the replicas this engine
+ *                        owns (with world_size > 1, the totals are the sums over the ranks). */
+#define RX_MAX_MC_MOVES 4
+enum rx_mc_kind { RX_MC_DISPLACEMENT = 0, RX_MC_ROTATION = 1 };
+typedef struct {
+    int32_t kind;              /* rx_mc_kind */
+    int32_t subset_offset, subset_len;
+    int32_t reserved;
+    double sigma_nm;           /* RX_MC_DISPLACEMENT: standard deviation of each component of the displacement */
+} rx_mc_move;
+RX_API int rx_set_mc_subsets(rx_engine *h, const int32_t *atoms, int32_t n);
+RX_API int rx_set_state_mc_moves(rx_engine *h, int32_t state, int32_t n, const rx_mc_move *moves);
+RX_API int rx_get_mc_statistics(rx_engine *h, int64_t *accepted, int64_t *proposed);
+RX_API int rx_set_mc_statistics(rx_engine *h, const int64_t *accepted, const int64_t *proposed);
+/* Diagnostic: du[K][RX_MAX_MC_MOVES] (kJ/mol) of the last proposal of every owned replica in every move slot -- the energy
+ * change the acceptance test used, the difference of the replica's own rows of rx_compute_energies at the proposed and the
+ * current positions, divided by beta; NaN where no energy was computed (a rejected rotation on a periodic box, an unused
+ * slot, a replica this engine does not own). */
+RX_API int rx_get_mc_energy_changes(rx_engine *h, double *du);
+
 /* ---- replica state I/O (SamplerState.apply_to_context / update_from_context, states.py:2215-2279) -- */
 /* xyz: [count][N][3] doubles, global replica indices; replicas not owned by this engine are skipped.    */
 RX_API int rx_set_positions(rx_engine *h, int32_t first, int32_t count, const double *xyz);

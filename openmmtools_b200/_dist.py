@@ -191,6 +191,32 @@ def _decode_shard(buf):
     return out
 
 
+_MAX_EXACT_COUNT = 1 << 53
+
+
+def sum_counts(comm, counts):
+    """The element-wise sum over the ranks of every rank's non-negative integer array `counts` (the same shape everywhere),
+    on rank 0; None on the other ranks.  Every rank takes part.  The array travels as the position rows of a one-record
+    shard, the format both communicators carry; float64 holds every count below 2**53 exactly, and larger ones are refused
+    rather than rounded."""
+    import numpy as np
+    a = np.ascontiguousarray(counts, np.int64)
+    if a.size and (a.min() < 0 or a.max() >= _MAX_EXACT_COUNT):
+        raise ValueError('sum_counts: counts must lie in [0, 2**53)')
+    flat = a.ravel().astype(np.float64)
+    rows = np.concatenate([flat, np.zeros(-flat.size % 3)]).reshape(-1, 3)
+    parts = comm.gather_object([(comm.rank, rows, None, None, None)])
+    if parts is None:
+        return None
+    total = np.zeros(a.size, np.int64)
+    for part in parts:
+        rec = np.asarray(part[0][1], np.float64).ravel()
+        if len(part) != 1 or rec.size != rows.size:
+            raise RuntimeError('sum_counts: a rank sent a record of another size')
+        total += rec[:a.size].astype(np.int64)
+    return total.reshape(a.shape)
+
+
 def default_communicator():
     try:
         import torch.distributed as dist

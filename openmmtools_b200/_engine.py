@@ -171,6 +171,47 @@ class Engine:
         self._check(self._lib.rx_set_state_integrator(self._h, int(state), float(timestep), float(collision_rate), int(n_steps),
                                                       splitting.replace(' ', '').encode(), int(bool(reassign_velocities))))
 
+    # -- Monte Carlo moves (rx_set_mc_subsets, rx_set_state_mc_moves)
+    def set_mc_moves(self, moves):
+        """The Monte Carlo moves of every state: moves[l] is a list of up to RX_MAX_MC_MOVES (kind, sigma_nm, atom indices),
+        kind RX_MC_DISPLACEMENT or RX_MC_ROTATION.  Every distinct subset is uploaded once."""
+        if len(moves) != self.M:
+            raise ValueError('expected the moves of %d states' % self.M)
+        atoms, where = [], {}
+        for state in moves:
+            for _, _, subset in state:
+                key = tuple(int(i) for i in subset)
+                if key not in where:
+                    where[key] = len(atoms)
+                    atoms.extend(key)
+        a = np.ascontiguousarray(atoms, np.int32)
+        self._check(self._lib.rx_set_mc_subsets(self._h, _ptr(a), len(a)))
+        for l, state in enumerate(moves):
+            arr = (_lib.RxMcMove * max(len(state), 1))()
+            for j, (kind, sigma, subset) in enumerate(state):
+                key = tuple(int(i) for i in subset)
+                arr[j].kind, arr[j].subset_offset, arr[j].subset_len, arr[j].sigma_nm = int(kind), where[key], len(key), float(sigma)
+            self._check(self._lib.rx_set_state_mc_moves(self._h, l, len(state), C.cast(arr, C.c_void_p)))
+
+    def get_mc_statistics(self):
+        """(accepted, proposed) int64 [M][RX_MAX_MC_MOVES] of the replicas this engine owns."""
+        acc = np.zeros((self.M, _lib.RX_MAX_MC_MOVES), np.int64); prop = np.zeros_like(acc)
+        self._check(self._lib.rx_get_mc_statistics(self._h, _ptr(acc), _ptr(prop)))
+        return acc, prop
+
+    def get_mc_energy_changes(self):
+        """dU (kJ/mol) [K][RX_MAX_MC_MOVES] of every owned replica's last proposal per move slot; NaN where no energy was
+        computed (rx_get_mc_energy_changes)."""
+        du = np.zeros((self.K, _lib.RX_MAX_MC_MOVES))
+        self._check(self._lib.rx_get_mc_energy_changes(self._h, _ptr(du)))
+        return du
+
+    def set_mc_statistics(self, accepted, proposed):
+        shape = (self.M, _lib.RX_MAX_MC_MOVES)
+        acc = np.ascontiguousarray(accepted, np.int64).reshape(shape)
+        prop = np.ascontiguousarray(proposed, np.int64).reshape(shape)
+        self._check(self._lib.rx_set_mc_statistics(self._h, _ptr(acc), _ptr(prop)))
+
     # -- constant pressure (rx_set_pressures)
     def set_pressures(self, pressure, dispersion):
         """Switch to NPT: per-state pressures (kJ/mol/nm^3) and dispersion coefficients c_l (kJ/mol nm^3, the correction

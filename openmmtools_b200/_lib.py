@@ -24,7 +24,10 @@ SYMBOLS = [
     'rx_run_iterations', 'rx_sams_set', 'rx_sams_step', 'rx_sams_get', 'rx_sams_run_iterations', 'rx_get_phase_times', 'rx_timer_mark', 'rx_timer_elapsed', 'rx_get_mix_stats', 'rx_selftest_exp', 'rx_plan_propagate', 'rx_comm_unique_id', 'rx_comm_init',
     'rx_set_pressures', 'rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat', 'rx_compute_energies_at_npt',
     'rx_set_alchemical_regions', 'rx_set_states_region2', 'rx_compute_energies_at_region2',
+    'rx_set_mc_subsets', 'rx_set_state_mc_moves', 'rx_get_mc_statistics', 'rx_set_mc_statistics', 'rx_get_mc_energy_changes',
 ]
+RX_MAX_MC_MOVES = 4
+RX_MC_DISPLACEMENT, RX_MC_ROTATION = 0, 1
 
 
 class RxConfig(C.Structure):
@@ -70,6 +73,11 @@ class RxMolecule(C.Structure):
                 ('mass', C.c_void_p), ('charge', C.c_void_p), ('sigma', C.c_void_p), ('epsilon', C.c_void_p),
                 ('bonds', C.c_void_p), ('angles', C.c_void_p), ('torsions', C.c_void_p), ('exclusions', C.c_void_p),
                 ('exceptions', C.c_void_p), ('constraints', C.c_void_p)]
+
+
+class RxMcMove(C.Structure):
+    _fields_ = [('kind', C.c_int32), ('subset_offset', C.c_int32), ('subset_len', C.c_int32), ('reserved', C.c_int32),
+                ('sigma_nm', C.c_double)]
 
 
 class RxGbsa(C.Structure):
@@ -142,6 +150,11 @@ def load():
     lib.rx_set_alchemical_regions.argtypes = [vp, vp, i32, i32]
     lib.rx_set_states_region2.argtypes = [vp, vp]
     lib.rx_compute_energies_at_region2.argtypes = [vp, vp, vp, vp, vp, i32, vp]
+    lib.rx_set_mc_subsets.argtypes = [vp, vp, i32]
+    lib.rx_set_state_mc_moves.argtypes = [vp, i32, i32, vp]
+    lib.rx_get_mc_statistics.argtypes = [vp, vp, vp]
+    lib.rx_set_mc_statistics.argtypes = [vp, vp, vp]
+    lib.rx_get_mc_energy_changes.argtypes = [vp, vp]
     for name in ('rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat'):
         getattr(lib, name).argtypes = [vp, i32, i32, vp]
     if lib.rx_abi_version() != RX_ABI_VERSION:

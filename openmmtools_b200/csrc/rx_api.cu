@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
+#include <algorithm>
 
 thread_local std::string g_rx_create_error;
 
@@ -133,6 +134,7 @@ extern "C" void rx_destroy(rx_engine *h) {
     for (int i = 0; i < 2; i++) if (h->ev_walk[i]) cudaEventDestroy(h->ev_walk[i]);
     for (const auto &r : h->pinned) cudaHostUnregister((void *)r.first);
     cudaFree(h->d_moves);
+    cudaFree(h->d_mc_atoms); cudaFree(h->d_mc_moves); cudaFree(h->d_mc_acc); cudaFree(h->d_mc_prop); cudaFree(h->d_mc_du);
     rxi_free_molecule(h);
     if (h->h_io) cudaFreeHost(h->h_io);
     if (h->stream) cudaStreamDestroy(h->stream);
@@ -348,6 +350,129 @@ extern "C" int rx_set_state_integrator(rx_engine *h, int32_t state, double times
     memcpy(m.program, splitting, n);
     h->state_moves_dirty = true;
     return RX_OK;
+}
+
+// ---- Monte Carlo moves (rx_mc.cuh) ----------------------------------------------------------------------------------------
+// Every state's move table on the device, and the number of launches it takes (the most moves any state has).
+static int upload_mc_moves(rx_engine *h) {
+    const int M = h->cfg.n_states;
+    h->mc_slots = 0;
+    for (int l = 0; l < M; l++)
+        for (int j = 0; j < RX_MAX_MC_MOVES; j++)
+            if (h->mc_moves[(size_t)l * RX_MAX_MC_MOVES + j].kind >= 0) h->mc_slots = std::max(h->mc_slots, j + 1);
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_mc_moves, h->mc_moves.data(), sizeof(rx_mc_move) * h->mc_moves.size(), cudaMemcpyHostToDevice));
+    return RX_OK;
+}
+
+extern "C" int rx_set_mc_subsets(rx_engine *h, const int32_t *atoms, int32_t n) {
+    ENTER(h);
+    if (h->cfg.system_kind == RX_SYSTEM_NONE) RX_FAIL(h, RX_ERR_INVALID, "rx_set_mc_subsets: engine has no particle system");
+    if (n < 0 || (n > 0 && !atoms)) RX_FAIL(h, RX_ERR_INVALID, "rx_set_mc_subsets: bad arguments");
+    for (int q = 0; q < n; q++)
+        if (atoms[q] < 0 || atoms[q] >= h->cfg.n_atoms) RX_FAIL(h, RX_ERR_INVALID, "rx_set_mc_subsets: atom index out of range");
+    const size_t mm = (size_t)h->cfg.n_states * RX_MAX_MC_MOVES;
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (!h->d_mc_moves) {
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_moves, sizeof(rx_mc_move) * mm));
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_acc, sizeof(unsigned long long) * mm));
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_prop, sizeof(unsigned long long) * mm));
+        RX_CHECK_CUDA(h, cudaMemset(h->d_mc_acc, 0, sizeof(unsigned long long) * mm));
+        RX_CHECK_CUDA(h, cudaMemset(h->d_mc_prop, 0, sizeof(unsigned long long) * mm));
+        const size_t nd = (size_t)(h->kloc > 0 ? h->kloc : 1) * RX_MAX_MC_MOVES;
+        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_du, sizeof(double) * nd));
+        RX_CHECK_CUDA(h, cudaMemset(h->d_mc_du, 0xff, sizeof(double) * nd));   // (NaN: no proposal yet)
+    }
+    cudaFree(h->d_mc_atoms);
+    h->d_mc_atoms = nullptr;
+    RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_atoms, sizeof(int32_t) * (n > 0 ? n : 1)));
+    if (n > 0) RX_CHECK_CUDA(h, cudaMemcpy(h->d_mc_atoms, atoms, sizeof(int32_t) * n, cudaMemcpyHostToDevice));
+    h->mc_atoms.assign(atoms, atoms + n);
+    rx_mc_move none;
+    memset(&none, 0, sizeof(none));
+    none.kind = -1;
+    h->mc_moves.assign(mm, none);
+    return upload_mc_moves(h);
+}
+
+extern "C" int rx_set_state_mc_moves(rx_engine *h, int32_t state, int32_t n, const rx_mc_move *moves) {
+    ENTER(h);
+    const int M = h->cfg.n_states, N = h->cfg.n_atoms;
+    if (!h->d_mc_moves) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: call rx_set_mc_subsets first");
+    if (state < -1 || state >= M) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: state out of range");
+    if (n < 0 || n > RX_MAX_MC_MOVES || (n > 0 && !moves))
+        RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: a state has 0 to RX_MAX_MC_MOVES (4) moves");
+    if (n > 0 && h->cfg.system_kind == RX_SYSTEM_LJ_ALCH && N > 4096)
+        RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_state_mc_moves: more than 4096 atoms per replica is not supported");
+    if (n > 0 && h->cfg.system_kind == RX_SYSTEM_HARMONIC && N > 1024)
+        RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_state_mc_moves: more than 1024 atoms per replica of a harmonic system is not supported");
+    std::vector<char> seen((size_t)N);
+    for (int j = 0; j < n; j++) {
+        const rx_mc_move &m = moves[j];
+        if (m.kind != RX_MC_DISPLACEMENT && m.kind != RX_MC_ROTATION) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: unknown move kind");
+        if (!(m.sigma_nm >= 0.0) || !isfinite(m.sigma_nm)) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: sigma must be finite and >= 0");
+        if (m.subset_len < 1 || m.subset_offset < 0 || (size_t)m.subset_offset + m.subset_len > h->mc_atoms.size())
+            RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: subset outside the array of rx_set_mc_subsets");
+        std::fill(seen.begin(), seen.end(), 0);
+        const int32_t *sub = h->mc_atoms.data() + m.subset_offset;
+        for (int q = 0; q < m.subset_len; q++) {
+            if (seen[sub[q]]) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: a subset lists an atom twice");
+            seen[sub[q]] = 1;
+        }
+        if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {   // every constraint cluster is in the subset wholly or not at all
+            if (!h->have_particles) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_mc_moves: call rx_set_molecule first");
+            for (int i = 0; i < N; i++)
+                for (int q = 0; q < m.subset_len; q++)
+                    if (h->mol_cluster[i] >= 0 && h->mol_cluster[i] == h->mol_cluster[sub[q]] && !seen[i])
+                        RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_state_mc_moves: a subset holds part of a constraint cluster; a rigid "
+                                                       "move keeps the constraints only when it moves whole clusters");
+        }
+    }
+    for (int l = (state < 0 ? 0 : state); l < (state < 0 ? M : state + 1); l++)
+        for (int j = 0; j < RX_MAX_MC_MOVES; j++) {
+            rx_mc_move &dst = h->mc_moves[(size_t)l * RX_MAX_MC_MOVES + j];
+            if (j < n) dst = moves[j];
+            else { memset(&dst, 0, sizeof(dst)); dst.kind = -1; }
+        }
+    return upload_mc_moves(h);
+}
+
+static int mc_statistics(rx_engine *h, int64_t *acc, int64_t *prop, bool to_device, const char *who) {
+    if (!acc || !prop) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": null argument");
+    const size_t mm = (size_t)h->cfg.n_states * RX_MAX_MC_MOVES;
+    if (!h->d_mc_acc) {
+        if (to_device) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": call rx_set_mc_subsets first");
+        memset(acc, 0, sizeof(int64_t) * mm);
+        memset(prop, 0, sizeof(int64_t) * mm);
+        return RX_OK;
+    }
+    if (to_device)
+        for (size_t q = 0; q < mm; q++)
+            if (acc[q] < 0 || prop[q] < acc[q]) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": need 0 <= accepted <= proposed");
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    const cudaMemcpyKind kind = to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost;
+    RX_CHECK_CUDA(h, cudaMemcpy(to_device ? (void *)h->d_mc_acc : (void *)acc, to_device ? (void *)acc : (void *)h->d_mc_acc, sizeof(int64_t) * mm, kind));
+    RX_CHECK_CUDA(h, cudaMemcpy(to_device ? (void *)h->d_mc_prop : (void *)prop, to_device ? (void *)prop : (void *)h->d_mc_prop, sizeof(int64_t) * mm, kind));
+    return RX_OK;
+}
+extern "C" int rx_get_mc_statistics(rx_engine *h, int64_t *accepted, int64_t *proposed) {
+    ENTER(h);
+    return mc_statistics(h, accepted, proposed, false, "rx_get_mc_statistics");
+}
+extern "C" int rx_get_mc_energy_changes(rx_engine *h, double *du) {
+    ENTER(h);
+    if (!du) RX_FAIL(h, RX_ERR_INVALID, "rx_get_mc_energy_changes: null argument");
+    const int K = h->cfg.n_replicas;
+    for (size_t q = 0; q < (size_t)K * RX_MAX_MC_MOVES; q++) du[q] = NAN;
+    if (!h->d_mc_du || h->kloc == 0) return RX_OK;
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpy(du + (size_t)h->k0 * RX_MAX_MC_MOVES, h->d_mc_du, sizeof(double) * h->kloc * RX_MAX_MC_MOVES,
+                                cudaMemcpyDeviceToHost));
+    return RX_OK;
+}
+extern "C" int rx_set_mc_statistics(rx_engine *h, const int64_t *accepted, const int64_t *proposed) {
+    ENTER(h);
+    return mc_statistics(h, const_cast<int64_t *>(accepted), const_cast<int64_t *>(proposed), true, "rx_set_mc_statistics");
 }
 
 static int local_range(rx_engine *h, int first, int count, int *lo, int *n, int *skip) {
@@ -592,6 +717,8 @@ extern "C" int rx_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int
     if (!h->have_integrator) RX_FAIL(h, RX_ERR_INVALID, "rx_propagate: rx_set_integrator must be called first");
     PhaseTimer T(h, 1);
     int launches = 0;
+    rc = rxi_mc_moves(h, seed, iteration, &launches);   // (before the snapshot: a retry reruns the dynamics only)
+    if (rc) return rc;
     rc = rxi_snapshot_state(h);
     if (rc) return rc;
     rc = rxi_propagate(h, seed, iteration, reassign, &launches);
@@ -804,6 +931,8 @@ static int run_fused(rx_engine *h, const char *who, int32_t n_iterations, uint64
         if (rc) return rc;
         Tm.stop(lm);
         PhaseTimer Tp(h, 1);
+        rc = rxi_mc_moves(h, seed, first_iteration + it, &lp);
+        if (rc) return rc;
         rc = rxi_propagate(h, seed, first_iteration + it, reassign, &lp);
         if (rc) return rc;
         Tp.stop(lp);

@@ -1422,6 +1422,21 @@ int rxi_randomize_velocities(rx_engine *h, uint64_t seed, uint64_t stream_id) {
     return RX_OK;
 }
 
+// The f64 energy parameters of the engine's system (k_energy_rows, k_mc_move) for a table of n_states states.
+static EnParams en_params(const rx_engine *h, int n_states) {
+    const rx_config &c = h->cfg;
+    EnParams p;
+    memset(&p, 0, sizeof(p));
+    p.N = c.n_atoms; p.M = n_states; p.kind = c.system_kind; p.n_alch = h->n_alch;
+    p.Lx = c.box[0]; p.Ly = c.box[1]; p.Lz = c.box[2];
+    p.rc2 = c.r_cutoff * c.r_cutoff; p.rs = c.r_switch; p.rc = c.r_cutoff;
+    p.inv_w = 1.0 / (c.r_cutoff - c.r_switch);
+    p.use_switch = c.use_switch; p.annihilate = h->two_regions ? h->annihilate_mask : c.annihilate_sterics;
+    p.c_is_6 = (c.softcore_c == 6.0); p.sc_c = c.softcore_c;
+    p.pair_cap = h->pair_cap;
+    return p;
+}
+
 // Energy rows of the owned replicas at `n_states` states described by the device table `d_states`, written to
 // d_out[K][n_states] (rows [k0, k0+kloc)).  The resident table/matrix are the default.
 int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_states, double *d_out, int *launches,
@@ -1440,21 +1455,12 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
         (*launches)++;
         return RX_OK;
     }
-    EnParams p;
-    memset(&p, 0, sizeof(p));
-    p.N = c.n_atoms; p.M = n_states; p.kind = c.system_kind; p.n_alch = h->n_alch;
-    p.Lx = c.box[0]; p.Ly = c.box[1]; p.Lz = c.box[2];
-    p.rc2 = c.r_cutoff * c.r_cutoff; p.rs = c.r_switch; p.rc = c.r_cutoff;
-    p.inv_w = 1.0 / (c.r_cutoff - c.r_switch);
-    p.use_switch = c.use_switch; p.annihilate = c.annihilate_sterics;
-    p.c_is_6 = (c.softcore_c == 6.0); p.sc_c = c.softcore_c;
-    p.pair_cap = h->pair_cap;
+    const EnParams p = en_params(h, n_states);
     const size_t smem = (size_t)3 * c.n_atoms * sizeof(double);
     if (h->npt && !d_npt_tab)
         RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at: a constant-pressure engine needs the states' pressures (rx_compute_energies_at_npt)");
     if (!h->npt && d_npt_tab)
         RX_FAIL(h, RX_ERR_INVALID, "rx_compute_energies_at_npt: the engine has no pressure (rx_set_pressures)");
-    if (h->two_regions) p.annihilate = h->annihilate_mask;
     auto kern = h->two_regions ? (h->npt ? k_energy_rows<true, true> : k_energy_rows<false, true>)
                                : (h->npt ? k_energy_rows<true> : k_energy_rows<false>);
     const int rco = smem_opt_in(h, (const void *)kern, (int)smem);
@@ -1647,6 +1653,8 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
         cl[cluster_of[root]].push_back(MolCons{(int)q[0], (int)q[1], q[2]});
     }
     if ((int)cl.size() > 32) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_molecule: more than 32 constraint clusters");
+    h->mol_cluster.assign(n, -1);   // (what a Monte Carlo move's subset must hold whole, rx_set_state_mc_moves)
+    for (int i = 0; i < n; i++) h->mol_cluster[i] = cluster_of[find(i)];
     std::vector<MolCons> cons;
     for (auto &c : cl) { cons.insert(cons.end(), c.begin(), c.end()); c_off.push_back((int)cons.size()); }
     MolDev *m = (MolDev *)h->mol_dev;
@@ -1719,3 +1727,5 @@ int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s) {
     h->mol_gb = new MolGB(g);
     return RX_OK;
 }
+
+#include "rx_mc.cuh"

@@ -122,6 +122,15 @@ struct rx_engine {
     std::vector<rx_state_move> state_moves;   // per-state moves (empty: one move for all states)
     bool state_moves_dirty = false;
     void *d_moves = nullptr;
+    std::vector<int> mol_cluster;            // constraint cluster of each atom of a molecule (-1: unconstrained)
+    // Monte Carlo moves (rx_set_state_mc_moves): [M][RX_MAX_MC_MOVES] records, kind -1 where a state has fewer moves
+    std::vector<int32_t> mc_atoms;           // rx_set_mc_subsets
+    int32_t *d_mc_atoms = nullptr;
+    std::vector<rx_mc_move> mc_moves;
+    rx_mc_move *d_mc_moves = nullptr;
+    int mc_slots = 0;                        // the most moves any state has: launches per propagation
+    unsigned long long *d_mc_acc = nullptr, *d_mc_prop = nullptr;   // [M][RX_MAX_MC_MOVES]
+    double *d_mc_du = nullptr;               // [kloc][RX_MAX_MC_MOVES]: dU of each owned replica's last proposal per slot
     // mixing
     MTStream streams[2];
     uint4 *d_slots = nullptr;   // the 16-byte records of a pass: SlotRec, SlotRec2 or CandRec
@@ -210,6 +219,7 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol);
 void rxi_free_molecule(rx_engine *h);
 int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s);
 void rxi_free_implicit_solvent(rx_engine *h);
+int rxi_mc_moves(rx_engine *h, uint64_t seed, uint64_t iteration, int *launches);   // one launch per MC slot (rx_mc.cuh)
 int rxi_snapshot_state(rx_engine *h);   // positions + velocities at the start of a propagation
 int rxi_restore_failed(rx_engine *h);   // replicas with a NaN flag go back to the snapshot; d_retry = the flags
 int rxi_compute_energy_rows(rx_engine *h, int *launches);  // fills d_u rows [k0, k0+kloc)

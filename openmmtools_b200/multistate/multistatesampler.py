@@ -77,6 +77,7 @@ class MultiStateSampler:
         self._want_async_reporting = False
         self._unsampled_table = None
         self._engine = None
+        self._mc_moves = None          # per state, the Metropolized moves the engine runs (None: no state has one)
         self._states_stale = False     # host copies of sampler states are behind the device
         self._host_x = self._host_v = None   # page-locked backing store of the owned sampler states
         self._host_store = None
@@ -225,6 +226,9 @@ class MultiStateSampler:
         if self._seed is None:
             self._seed = extra.get('seed')
         self._create_engine()
+        if 'mc_accepted' in extra and self._mc_moves:   # the move counts of the checkpoint (the moves may be stored later)
+            self._mc_counts_to_moves(self._mc_moves, np.array(extra['mc_accepted']), np.array(extra['mc_proposed']))
+            self._push_mc_statistics()
         if 'barostat' in extra:     # the NPT run continues with the barostat state it had at the checkpoint
             self._engine.set_barostat({k: np.asarray(v)[self._engine.k0:self._engine.k1] for k, v in extra['barostat'].items()},
                                       first=self._engine.k0)
@@ -346,18 +350,73 @@ class MultiStateSampler:
         self._replica_thermodynamic_states = e.pinned_array(st.shape, np.int64)
         self._replica_thermodynamic_states[...] = st
 
-    def _apply_moves(self):
-        """The moves go to the engine: one for all states, or -- when the states carry different moves
+    def _apply_moves(self, moves=None):
+        """The moves (default: the sampler's) go to the engine: one for all states, or -- when the states carry different moves
         (multistatesampler.py:906-910) -- one per state; a replica is propagated with the move of the state it is in
-        (multistatesampler.py:1311-1322), inside the same fused launch."""
-        mv0 = self._mcmc_moves[0]
+        (multistatesampler.py:1311-1322), inside the same fused launch.  The Metropolized moves of a move
+        (mcmc.split_move) run before the dynamics, per state, with the counts the move objects hold."""
+        own = moves is None
+        moves = self._mcmc_moves if own else moves
+        integrators = [mcmc.integrator_part(mv) for mv in moves]
+        mv0 = integrators[0]
         dt, gamma, n_steps, splitting = mv0._integrator_parameters()
         self._engine.set_integrator(dt, gamma, n_steps, splitting)
         self._reassign = bool(mv0.reassign_velocities)
-        if any(not mcmc.same_integrator(mv, mv0) for mv in self._mcmc_moves[1:]):
-            for l, mv in enumerate(self._mcmc_moves):
+        if own:
+            self._n_restart = mv0.n_restart_attempts
+        if any(not mcmc.same_integrator(mv, mv0) for mv in integrators[1:]):
+            for l, mv in enumerate(integrators):
                 dt, gamma, n_steps, splitting = mv._integrator_parameters()
                 self._engine.set_state_integrator(l, dt, gamma, n_steps, splitting, bool(mv.reassign_velocities))
+        mc = [mcmc.split_move(mv)[0] for mv in moves]
+        if any(mc) or self._mc_moves is not None:
+            n = self._thermodynamic_states[0].n_particles
+            self._engine.set_mc_moves([[m._engine_move(n) for m in ms] for ms in mc])
+            self._mc_moves = mc if any(mc) else None
+            if self._mc_moves:
+                self._push_mc_statistics()
+
+    # Monte Carlo move counts: the device keeps them per state and move slot, summed over the replicas a rank owns; the move
+    # objects get the totals over every rank.  A move object that several states share (equilibrate with one move) gets the
+    # sum over them.
+    @staticmethod
+    def _mc_counts_to_moves(mc, accepted, proposed):
+        totals = {}
+        for l, ms in enumerate(mc):
+            for j, m in enumerate(ms):
+                a, p = totals.get(id(m), (0, 0))
+                totals[id(m)] = (a + int(accepted[l, j]), p + int(proposed[l, j]))
+        for ms in mc:
+            for m in ms:
+                m.n_accepted, m.n_proposed = totals[id(m)]
+
+    def _push_mc_statistics(self):
+        """The counts of the move objects go to the device: all of them to rank 0, so that the ranks' sums are the totals."""
+        acc = np.zeros((self.n_states, mcmc.RX_MAX_MC_MOVES), np.int64)
+        prop = np.zeros_like(acc)
+        seen = set()
+        for l, ms in enumerate(self._mc_moves):
+            for j, m in enumerate(ms):
+                if id(m) not in seen and self._rank == 0:
+                    acc[l, j], prop[l, j] = m.n_accepted, m.n_proposed
+                seen.add(id(m))
+        self._engine.set_mc_statistics(acc, prop)
+        self._mc_last = (acc, prop)
+
+    def _pull_mc_statistics(self):
+        """The device counts, summed over the ranks (every rank takes part), into the move objects on rank 0."""
+        acc, prop = self._engine.get_mc_statistics()
+        if self._world_size > 1:
+            from .._dist import default_communicator, sum_counts
+            comm = self._communicator
+            if comm is None:
+                comm = self._communicator = default_communicator()
+            both = sum_counts(comm, np.stack([acc, prop]))
+            if self._rank != 0:
+                return
+            acc, prop = both
+        self._mc_counts_to_moves(self._mc_moves, acc, prop)
+        self._mc_last = (acc, prop)
 
     def _seed_mixing_streams(self):
         # the reference never seeds numba's / numpy's generators (os.urandom); a user seed makes runs reproducible
@@ -559,10 +618,10 @@ class MultiStateSampler:
             raise RuntimeError('Cannot equilibrate a sampler that has not been created.')
         if mcmc_moves is not None:
             mv = mcmc_moves if isinstance(mcmc_moves, mcmc.MCMCMove) else mcmc_moves[0]
-            self._engine.set_integrator(*mv._integrator_parameters())
-            reassign = bool(mv.reassign_velocities)
-        else:
-            reassign = self._reassign
+            if self._mc_moves:     # the sampler's own moves keep their counts
+                self._pull_mc_statistics()
+            self._apply_moves([mv] * self.n_states)
+        reassign = self._reassign
         self._equil_counter = getattr(self, '_equil_counter', 0)
         for _ in range(n_iterations):
             self._equil_counter += 1
@@ -570,6 +629,8 @@ class MultiStateSampler:
             self._compute_energies()
             self._replica_thermodynamic_states = self._mix_replicas()
         if mcmc_moves is not None:
+            if self._mc_moves:
+                self._pull_mc_statistics()
             self._apply_moves()
 
     def minimize(self, tolerance=1.0 * unit.kilojoules_per_mole / unit.nanometers, max_iterations=0):
@@ -617,7 +678,7 @@ class MultiStateSampler:
                 e.set_positions(self._host_x, first=e.k0)
                 e.set_velocities(self._host_v, first=e.k0)
         it = self._iteration if iteration is None else iteration
-        n_restart = self._mcmc_moves[0].n_restart_attempts
+        n_restart = self._n_restart
         re = self._reassign if reassign is None else reassign
         for attempt in range(n_restart + 1):
             try:
@@ -695,6 +756,8 @@ class MultiStateSampler:
                      mt_numba_words=int(e.mix_stream_position(_lib.RX_STREAM_NUMBA)),
                      mt_numpy_words=int(e.mix_stream_position(_lib.RX_STREAM_NUMPY)),
                      equil_counter=int(getattr(self, '_equil_counter', 0)))
+        if self._mc_moves:        # the move counts as of the last report (rank 0: the totals over the ranks)
+            extra['mc_accepted'], extra['mc_proposed'] = (a.tolist() for a in self._mc_last)
         if self._npt:     # (rank 0: the records gathered for this iteration's report)
             rec = self._last_npt_records if self._world_size > 1 else self._local_npt_records()
             extra['barostat'] = dict(volume_scale=rec[:, 3].tolist(),
@@ -714,6 +777,8 @@ class MultiStateSampler:
             if self._world_size > 1:
                 self._gather_sampler_states()
         npt = self._last_npt_records = self._gather_npt_records() if self._npt else None
+        if self._mc_moves:
+            self._pull_mc_statistics()
         if self._rank != 0:
             self._report_iteration_items()
             return
@@ -724,6 +789,8 @@ class MultiStateSampler:
         if checkpoint or analysis:
             r.write_sampler_states(self._sampler_states, it, extra=self._checkpoint_extra())
         r.write_mixing_statistics(self._n_accepted_matrix, self._n_proposed_matrix, it)
+        if self._mc_moves:        # the moves with their counts, at every reported iteration (multistatesampler.py:1219)
+            r.write_mcmc_moves(self._mcmc_moves)
         r.write_energies(self._energy_thermodynamic_states, self._neighborhoods, self._energy_unsampled_states, it)
         self._report_iteration_items()      # subclass records (SAMS) go in before the commit marker
         r.write_last_iteration(it)
@@ -843,7 +910,7 @@ class MultiStateSampler:
         t['estimated_time_remaining'] = t['average_seconds_per_iteration'] * (iteration_limit - self._iteration)
         t['estimated_total_time'] = t['average_seconds_per_iteration'] * self.number_of_iterations \
             if np.isfinite(self.number_of_iterations) else np.inf
-        mv = self._mcmc_moves[0]
+        mv = mcmc.integrator_part(self._mcmc_moves[0])
         try:
             dt_ns = unit.to_md(mv.timestep) * mv.n_steps * 1e-3
             t['ns_per_day'] = dt_ns / (t['average_seconds_per_iteration'] / 86400.0)
