@@ -69,23 +69,23 @@ extern "C" int rx_create(const rx_config *cfg, rx_engine **out) {
     for (int i = 0; i < 2; i++) CREATE_CUDA(cudaEventCreate(&h->ev_walk[i]));
     CREATE_CUDA(cudaEventCreateWithFlags(&h->ev_prepared, cudaEventDisableTiming));
     CREATE_CUDA(cudaEventCreateWithFlags(&h->ev_consumed, cudaEventDisableTiming));
-    CREATE_CUDA(cudaMalloc(&h->d_perm, sizeof(int) * K));
-    CREATE_CUDA(cudaMalloc(&h->d_u, sizeof(double) * (size_t)K * M));
+    CREATE_CUDA(h->d_perm.alloc(K));
+    CREATE_CUDA(h->d_u.alloc((size_t)K * M));
     CREATE_CUDA(cudaMemset(h->d_u, 0, sizeof(double) * (size_t)K * M));
-    CREATE_CUDA(cudaMalloc(&h->d_nacc, sizeof(unsigned long long) * (size_t)M * M));
-    CREATE_CUDA(cudaMalloc(&h->d_nprop, sizeof(unsigned long long) * (size_t)M * M));
+    CREATE_CUDA(h->d_nacc.alloc((size_t)M * M));
+    CREATE_CUDA(h->d_nprop.alloc((size_t)M * M));
     CREATE_CUDA(cudaMemset(h->d_nacc, 0, sizeof(unsigned long long) * (size_t)M * M));
     CREATE_CUDA(cudaMemset(h->d_nprop, 0, sizeof(unsigned long long) * (size_t)M * M));
-    CREATE_CUDA(cudaMalloc(&h->d_pot, sizeof(double) * K));
-    CREATE_CUDA(cudaMalloc(&h->d_kin, sizeof(double) * K));
+    CREATE_CUDA(h->d_pot.alloc(K));
+    CREATE_CUDA(h->d_kin.alloc(K));
     CREATE_CUDA(cudaMemset(h->d_pot, 0, sizeof(double) * K));
     CREATE_CUDA(cudaMemset(h->d_kin, 0, sizeof(double) * K));
-    CREATE_CUDA(cudaMalloc(&h->d_nan, sizeof(int) * K));
+    CREATE_CUDA(h->d_nan.alloc(K));
     CREATE_CUDA(cudaMemset(h->d_nan, 0, sizeof(int) * K));
-    CREATE_CUDA(cudaMalloc(&h->d_err, sizeof(int)));
+    CREATE_CUDA(h->d_err.alloc(1));
     CREATE_CUDA(cudaMemset(h->d_err, 0, sizeof(int)));
-    CREATE_CUDA(cudaMalloc(&h->d_ctl, sizeof(MixCtl)));
-    CREATE_CUDA(cudaMalloc(&h->d_states, sizeof(StateDev) * M));
+    CREATE_CUDA(h->d_ctl.alloc(1));
+    CREATE_CUDA(h->d_states.alloc(M));
     {
         std::vector<int> perm(K);
         for (int k = 0; k < K; k++) perm[k] = k % M;
@@ -95,20 +95,22 @@ extern "C" int rx_create(const rx_config *cfg, rx_engine **out) {
         const size_t n = (size_t)(h->kloc > 0 ? h->kloc : 1) * N;
         // (a molecule keeps its state as double[3] per atom, the other systems as float4)
         const size_t per_atom = cfg->system_kind == RX_SYSTEM_MOLECULE ? 3 * sizeof(double) : sizeof(float4);
-        CREATE_CUDA(cudaMalloc(&h->d_pos, per_atom * n));
-        CREATE_CUDA(cudaMalloc(&h->d_vel, per_atom * n));
+        CREATE_CUDA(h->d_pos.alloc(n, per_atom));
+        CREATE_CUDA(h->d_vel.alloc(n, per_atom));
         CREATE_CUDA(cudaMemset(h->d_pos, 0, per_atom * n));
         CREATE_CUDA(cudaMemset(h->d_vel, 0, per_atom * n));
-        CREATE_CUDA(cudaMalloc(&h->d_io, sizeof(double) * 3 * n));
-        CREATE_CUDA(cudaHostAlloc(&h->h_io, sizeof(double) * 3 * n, cudaHostAllocDefault));
-        CREATE_CUDA(cudaMalloc(&h->d_atom, sizeof(float4) * N));
-        CREATE_CUDA(cudaMalloc(&h->d_atom_d, sizeof(double4) * N));
-        CREATE_CUDA(cudaMalloc(&h->d_alch_list, sizeof(int) * N));
+        CREATE_CUDA(h->d_io.alloc(3 * n));
+        CREATE_CUDA(h->h_io.alloc(3 * n));
+        CREATE_CUDA(h->d_atom.alloc(N));
+        CREATE_CUDA(h->d_atom_d.alloc(N));
+        CREATE_CUDA(h->d_alch_list.alloc(N));
     }
     *out = h;
     return RX_OK;
 }
 
+// The engine's device and pinned memory is freed with it (CudaBuf, RecordPtr); streams, events, NCCL and the caller's pinned
+// buffers are released here.
 extern "C" void rx_destroy(rx_engine *h) {
     if (!h) return;
     cudaSetDevice(h->cfg.device);
@@ -121,22 +123,10 @@ extern "C" void rx_destroy(rx_engine *h) {
         destroy_t f = (destroy_t)dlsym(h->nccl_lib, "ncclCommDestroy");
         if (f) f(h->nccl_comm);
     }
-    rxi_sams_free(h);
-    rxi_mix_free(h);
-    cudaFree(h->d_atom); cudaFree(h->d_atom_d); cudaFree(h->d_alch_list); cudaFree(h->d_states);
-    cudaFree(h->d_pos_snap); cudaFree(h->d_vel_snap); cudaFree(h->d_retry);
-    cudaFree(h->d_pos); cudaFree(h->d_vel); cudaFree(h->d_io); cudaFree(h->d_perm); cudaFree(h->d_u);
-    cudaFree(h->d_nacc); cudaFree(h->d_nprop); cudaFree(h->d_pot); cudaFree(h->d_kin); cudaFree(h->d_nan);
-    cudaFree(h->d_err); cudaFree(h->d_pairs);
-    cudaFree(h->d_npt); cudaFree(h->d_box); cudaFree(h->d_box_snap); cudaFree(h->d_baro); cudaFree(h->d_baro_snap);
     for (int i = 0; i < 8; i++) if (h->ev[i]) cudaEventDestroy(h->ev[i]);
     for (int i = 0; i < 2; i++) if (h->ev_user[i]) cudaEventDestroy(h->ev_user[i]);
     for (int i = 0; i < 2; i++) if (h->ev_walk[i]) cudaEventDestroy(h->ev_walk[i]);
     for (const auto &r : h->pinned) cudaHostUnregister((void *)r.first);
-    cudaFree(h->d_moves);
-    cudaFree(h->d_mc_atoms); cudaFree(h->d_mc_moves); cudaFree(h->d_mc_acc); cudaFree(h->d_mc_prop); cudaFree(h->d_mc_du);
-    rxi_free_molecule(h);
-    if (h->h_io) cudaFreeHost(h->h_io);
     if (h->stream) cudaStreamDestroy(h->stream);
     if (h->stream_rng) cudaStreamDestroy(h->stream_rng);
     delete h;
@@ -189,10 +179,8 @@ static int upload_atoms(rx_engine *h, const std::vector<int> &al) {
     long long cap = (long long)h->n_alch * (N - 1);
     if (cap > (1 << 18)) cap = 1 << 18;
     if (cap < 1) cap = 1;
-    cudaFree(h->d_pairs);
-    h->d_pairs = nullptr;
+    RX_CHECK_CUDA(h, h->d_pairs.alloc((size_t)cap * (h->kloc > 0 ? h->kloc : 1)));
     h->pair_cap = (int)cap;
-    RX_CHECK_CUDA(h, cudaMalloc(&h->d_pairs, sizeof(double2) * (size_t)cap * (h->kloc > 0 ? h->kloc : 1)));
     h->have_particles = true;
     return RX_OK;
 }
@@ -373,20 +361,25 @@ extern "C" int rx_set_mc_subsets(rx_engine *h, const int32_t *atoms, int32_t n) 
         if (atoms[q] < 0 || atoms[q] >= h->cfg.n_atoms) RX_FAIL(h, RX_ERR_INVALID, "rx_set_mc_subsets: atom index out of range");
     const size_t mm = (size_t)h->cfg.n_states * RX_MAX_MC_MOVES;
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
-    if (!h->d_mc_moves) {
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_moves, sizeof(rx_mc_move) * mm));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_acc, sizeof(unsigned long long) * mm));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_prop, sizeof(unsigned long long) * mm));
-        RX_CHECK_CUDA(h, cudaMemset(h->d_mc_acc, 0, sizeof(unsigned long long) * mm));
-        RX_CHECK_CUDA(h, cudaMemset(h->d_mc_prop, 0, sizeof(unsigned long long) * mm));
+    DevBuf<int32_t> d_atoms;
+    RX_CHECK_CUDA(h, d_atoms.alloc(n > 0 ? n : 1));
+    if (n > 0) RX_CHECK_CUDA(h, cudaMemcpy(d_atoms, atoms, sizeof(int32_t) * n, cudaMemcpyHostToDevice));
+    if (!h->d_mc_moves) {   // the move table and its statistics, taken by the engine once all of them exist
+        DevBuf<rx_mc_move> d_moves;
+        DevBuf<unsigned long long> d_acc, d_prop;
+        DevBuf<double> d_du;
         const size_t nd = (size_t)(h->kloc > 0 ? h->kloc : 1) * RX_MAX_MC_MOVES;
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_du, sizeof(double) * nd));
-        RX_CHECK_CUDA(h, cudaMemset(h->d_mc_du, 0xff, sizeof(double) * nd));   // (NaN: no proposal yet)
+        RX_CHECK_CUDA(h, d_moves.alloc(mm));
+        RX_CHECK_CUDA(h, d_acc.alloc(mm));
+        RX_CHECK_CUDA(h, d_prop.alloc(mm));
+        RX_CHECK_CUDA(h, d_du.alloc(nd));
+        RX_CHECK_CUDA(h, cudaMemset(d_acc, 0, sizeof(unsigned long long) * mm));
+        RX_CHECK_CUDA(h, cudaMemset(d_prop, 0, sizeof(unsigned long long) * mm));
+        RX_CHECK_CUDA(h, cudaMemset(d_du, 0xff, sizeof(double) * nd));   // (NaN: no proposal yet)
+        h->d_mc_moves = std::move(d_moves); h->d_mc_du = std::move(d_du);
+        h->d_mc_acc = std::move(d_acc); h->d_mc_prop = std::move(d_prop);
     }
-    cudaFree(h->d_mc_atoms);
-    h->d_mc_atoms = nullptr;
-    RX_CHECK_CUDA(h, cudaMalloc(&h->d_mc_atoms, sizeof(int32_t) * (n > 0 ? n : 1)));
-    if (n > 0) RX_CHECK_CUDA(h, cudaMemcpy(h->d_mc_atoms, atoms, sizeof(int32_t) * n, cudaMemcpyHostToDevice));
+    h->d_mc_atoms = std::move(d_atoms);
     h->mc_atoms.assign(atoms, atoms + n);
     rx_mc_move none;
     memset(&none, 0, sizeof(none));
@@ -533,12 +526,17 @@ extern "C" int rx_set_pressures(rx_engine *h, const double *pressure, const doub
         tab[l] = make_double2(pressure[l], dispersion[l]);
     }
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
-    if (!h->d_npt) {
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_npt, sizeof(double2) * M));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_box, sizeof(double4) * n));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_box_snap, sizeof(double4) * n));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_baro, sizeof(rx_barostat_state) * n));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_baro_snap, sizeof(rx_barostat_state) * n));
+    if (!h->d_npt) {   // taken by the engine once all of them exist
+        DevBuf<double2> d_npt;
+        DevBuf<double4> d_box, d_box_snap;
+        DevBuf<rx_barostat_state> d_baro, d_baro_snap;
+        RX_CHECK_CUDA(h, d_npt.alloc(M));
+        RX_CHECK_CUDA(h, d_box.alloc(n));
+        RX_CHECK_CUDA(h, d_box_snap.alloc(n));
+        RX_CHECK_CUDA(h, d_baro.alloc(n));
+        RX_CHECK_CUDA(h, d_baro_snap.alloc(n));
+        h->d_npt = std::move(d_npt); h->d_box = std::move(d_box); h->d_box_snap = std::move(d_box_snap);
+        h->d_baro = std::move(d_baro); h->d_baro_snap = std::move(d_baro_snap);
     }
     RX_CHECK_CUDA(h, cudaMemcpy(h->d_npt, tab.data(), sizeof(double2) * M, cudaMemcpyHostToDevice));
     const double *L = h->cfg.box;
@@ -579,13 +577,13 @@ extern "C" int rx_set_boxes(rx_engine *h, int32_t first, int32_t count, const do
                 RX_FAIL(h, RX_ERR_INVALID, "rx_set_boxes: every box edge must be at least twice the cutoff");
         b[i] = make_double4(edges[3 * i], edges[3 * i + 1], edges[3 * i + 2], 0.0);
     }
-    return replica_rows(h, h->d_box, first, count, b.data(), true, "rx_set_boxes");
+    return replica_rows(h, h->d_box.get(), first, count, b.data(), true, "rx_set_boxes");
 }
 extern "C" int rx_get_boxes(rx_engine *h, int32_t first, int32_t count, double *edges) {
     ENTER(h);
     if (!edges || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_get_boxes: bad arguments");
     std::vector<double4> b((size_t)count, make_double4(0.0, 0.0, 0.0, 0.0));
-    int rc = replica_rows(h, h->d_box, first, count, b.data(), false, "rx_get_boxes");
+    int rc = replica_rows(h, h->d_box.get(), first, count, b.data(), false, "rx_get_boxes");
     if (rc) return rc;
     int lo, n, skip;
     local_range(h, first, count, &lo, &n, &skip);
@@ -598,12 +596,12 @@ extern "C" int rx_set_barostat(rx_engine *h, int32_t first, int32_t count, const
     for (int i = 0; i < count; i++)
         if (!(state[i].volume_scale > 0) || state[i].step < 0 || state[i].n_attempted < 0 || state[i].n_accepted < 0)
             RX_FAIL(h, RX_ERR_INVALID, "rx_set_barostat: need volume_scale > 0 and non-negative counters");
-    return replica_rows(h, h->d_baro, first, count, const_cast<rx_barostat_state *>(state), true, "rx_set_barostat");
+    return replica_rows(h, h->d_baro.get(), first, count, const_cast<rx_barostat_state *>(state), true, "rx_set_barostat");
 }
 extern "C" int rx_get_barostat(rx_engine *h, int32_t first, int32_t count, rx_barostat_state *state) {
     ENTER(h);
     if (!state || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_get_barostat: bad arguments");
-    return replica_rows(h, h->d_baro, first, count, state, false, "rx_get_barostat");
+    return replica_rows(h, h->d_baro.get(), first, count, state, false, "rx_get_barostat");
 }
 
 bool rxi_is_pinned(const rx_engine *h, const void *p, size_t bytes) {
@@ -656,17 +654,16 @@ extern "C" int rx_minimize(rx_engine *h, double tolerance, int32_t max_iteration
     if (!(tolerance > 0.0)) RX_FAIL(h, RX_ERR_INVALID, "rx_minimize: tolerance must be positive");
     if (max_iterations < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_minimize: max_iterations must be >= 0");
     const int K = h->cfg.n_replicas;
-    double *d_rms = nullptr;
-    int *d_it = nullptr;
-    RX_CHECK_CUDA(h, cudaMalloc(&d_rms, sizeof(double) * K));
-    if (cudaMalloc(&d_it, sizeof(int) * K) != cudaSuccess) { cudaFree(d_rms); RX_FAIL(h, RX_ERR_CUDA, "rx_minimize: out of device memory"); }
+    DevBuf<double> d_rms;
+    DevBuf<int> d_it;
+    RX_CHECK_CUDA(h, d_rms.alloc(K));
+    RX_CHECK_CUDA(h, d_it.alloc(K));
     cudaMemsetAsync(d_rms, 0, sizeof(double) * K, h->stream);
     cudaMemsetAsync(d_it, 0, sizeof(int) * K, h->stream);
     int rc = rxi_minimize(h, tolerance, max_iterations == 0 ? 20000 : max_iterations, d_rms, d_it);
     if (rc == RX_OK && cudaStreamSynchronize(h->stream) != cudaSuccess) { h->err = "rx_minimize: kernel failed"; rc = RX_ERR_CUDA; }
     if (rc == RX_OK && rms_force) cudaMemcpy(rms_force, d_rms, sizeof(double) * K, cudaMemcpyDeviceToHost);
     if (rc == RX_OK && iterations) cudaMemcpy(iterations, d_it, sizeof(int) * K, cudaMemcpyDeviceToHost);
-    cudaFree(d_rms); cudaFree(d_it);
     return rc;
 }
 
@@ -816,13 +813,12 @@ static int energies_at(rx_engine *h, const rx_state_params *st, const double *la
         }
     }
     const int K = h->cfg.n_replicas;
-    StateDev *d_st = nullptr;
-    double *d_out = nullptr;
-    double2 *d_tab = nullptr;
-    RX_CHECK_CUDA(h, cudaMalloc(&d_st, sizeof(StateDev) * n));
-    cudaError_t e = cudaMalloc(&d_out, sizeof(double) * (size_t)K * n);
-    if (e == cudaSuccess && pressure) e = cudaMalloc(&d_tab, sizeof(double2) * n);
-    if (e != cudaSuccess) { cudaFree(d_st); cudaFree(d_out); RX_FAIL(h, RX_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e)); }
+    DevBuf<StateDev> d_st;
+    DevBuf<double> d_out;
+    DevBuf<double2> d_tab;
+    RX_CHECK_CUDA(h, d_st.alloc(n));
+    RX_CHECK_CUDA(h, d_out.alloc((size_t)K * n));
+    if (pressure) RX_CHECK_CUDA(h, d_tab.alloc(n));
     int launches = 0;
     cudaMemcpyAsync(d_st, hs.data(), sizeof(StateDev) * n, cudaMemcpyHostToDevice, h->stream);
     if (pressure) cudaMemcpyAsync(d_tab, tab.data(), sizeof(double2) * n, cudaMemcpyHostToDevice, h->stream);
@@ -830,14 +826,11 @@ static int energies_at(rx_engine *h, const rx_state_params *st, const double *la
     rc = rxi_compute_energy_rows_at(h, d_st, n, d_out, &launches, d_tab);
     if (!rc) rc = rxi_allgather_rows(h, d_out, n);
     if (!rc) {
-        e = cudaMemcpyAsync(u_out, d_out, sizeof(double) * (size_t)K * n, cudaMemcpyDeviceToHost, h->stream);
+        cudaError_t e = cudaMemcpyAsync(u_out, d_out, sizeof(double) * (size_t)K * n, cudaMemcpyDeviceToHost, h->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
         if (e != cudaSuccess) { h->err = std::string(who) + ": " + cudaGetErrorString(e); rc = RX_ERR_CUDA; }
     }
-    cudaStreamSynchronize(h->stream);
-    cudaFree(d_st);
-    cudaFree(d_out);
-    cudaFree(d_tab);
+    cudaStreamSynchronize(h->stream);   // (before the buffers are freed)
     if (rc) return rc;
     h->phase_launches[2] += launches;
     return check_device_error(h);

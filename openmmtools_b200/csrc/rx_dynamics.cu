@@ -883,6 +883,20 @@ int rxi_convert_out(rx_engine *h, const float4 *src, int first_local, int count,
 
 #include "rx_molecule.cuh"
 
+// A molecule's device tables and the views of them the kernels take: MolDev (rx_set_molecule), and MolGB with the OBC
+// per-atom table (rx_set_implicit_solvent; gb.on == 0: vacuum).
+struct MolTables {
+    MolDev dev;
+    DevBuf<double> mass, charge;
+    DevBuf<int> c_off;
+    DevBuf<MolCons> cons;
+    DevBuf<unsigned char> terms32, terms64;
+    MolGB gb;
+    DevBuf<double> gb_atom;
+};
+void RecordDelete::operator()(MolTables *m) const { delete m; }
+static const MolGB *mol_gb_of(const rx_engine *h) { return h->mol->gb.on ? &h->mol->gb : nullptr; }   // nullptr: vacuum
+
 // A block may take 48 KB of shared memory, static and dynamic together, unless the kernel has opted in to more (up to
 // cudaDevAttrMaxSharedMemoryPerBlockOptin, which mol_check_shared checks).  The molecule's tables grow with its terms, the
 // energy kernel's coordinates with the atoms (48 KB of them at 2048 atoms, over the limit with its static arrays).
@@ -935,7 +949,7 @@ int rxi_upload_state_moves(rx_engine *h) {
         const rx_state_move &m = h->state_moves[(size_t)l];
         tab[(size_t)l] = make_move(m.dt, m.gamma, m.n_steps, m.program, m.reassign);
     }
-    if (!h->d_moves) RX_CHECK_CUDA(h, cudaMalloc(&h->d_moves, sizeof(MoveDev) * (size_t)M));
+    if (!h->d_moves) RX_CHECK_CUDA(h, h->d_moves.alloc((size_t)M));
     RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_moves, tab.data(), sizeof(MoveDev) * (size_t)M, cudaMemcpyHostToDevice, h->stream));
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));   // (tab is a stack object)
     h->state_moves_dirty = false;
@@ -1097,8 +1111,8 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
         if (!h->state_moves.empty()) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_propagate: per-state moves are not provided for molecules");
         const uint2 mkey = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(iteration >> 32));
-        const MolDev *md = (const MolDev *)h->mol_dev;
-        const MolGB *gb = (const MolGB *)h->mol_gb;
+        const MolDev *md = &h->mol->dev;
+        const MolGB *gb = mol_gb_of(h);
         const bool no_star = getenv("RX_MOL_NO_STAR") != nullptr;   // cross-check: the general cluster path for every molecule
         const bool star = md->max_cluster <= 3 && !no_star;
         auto kern = gb ? (star ? k_propagate_mol<true, true> : k_propagate_mol<false, true>)
@@ -1106,8 +1120,8 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         const int dyn = mol_dyn_bytes(*md, gb, true);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
-        kern<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p.move, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos,
-                                                            (double *)h->d_vel, h->k0, mkey, (uint32_t)iteration, reassign, h->d_pot,
+        kern<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p.move, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos.get(),
+                                                            (double *)h->d_vel.get(), h->k0, mkey, (uint32_t)iteration, reassign, h->d_pot,
                                                             h->d_kin, h->d_nan, d_only, gb ? *gb : MolGB{});
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
@@ -1164,8 +1178,9 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
                     return with_layout(PropagateLayouts{}, plan, per_state, rc, [&](auto L) {
                         return launch_kernel(h, lc, smem > 48 * 1024, k_propagate<c6, sw, L.cl, L.ps, L.compact, np, rg>, p,
                                              (const float4 *)h->d_atom, (const StateDev *)h->d_states, (const int *)h->d_perm,
-                                             h->d_pos, h->d_vel, h->k0, key, it32, h->d_pot, h->d_kin, h->d_nan, d_only,
-                                             (const MoveDev *)h->d_moves, h->d_box, h->d_baro, (const double2 *)h->d_npt, min_edge);
+                                             h->d_pos.get(), h->d_vel.get(), h->k0, key, it32, h->d_pot.get(), h->d_kin.get(),
+                                             h->d_nan.get(), d_only, (const MoveDev *)h->d_moves, h->d_box.get(), h->d_baro.get(),
+                                             (const double2 *)h->d_npt, min_edge);
                     });
                 });
             });
@@ -1183,10 +1198,13 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
 int rxi_snapshot_state(rx_engine *h) {
     if (h->kloc == 0) return RX_OK;
     const size_t bytes = (h->cfg.system_kind == RX_SYSTEM_MOLECULE ? 3 * sizeof(double) : sizeof(float4)) * (size_t)h->kloc * h->cfg.n_atoms;
-    if (!h->d_pos_snap) {
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_pos_snap, bytes));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_vel_snap, bytes));
-        RX_CHECK_CUDA(h, cudaMalloc(&h->d_retry, sizeof(int) * h->cfg.n_replicas));
+    if (!h->d_pos_snap) {   // taken by the engine once all of them exist
+        DevBuf<float4> pos, vel;
+        DevBuf<int> retry;
+        RX_CHECK_CUDA(h, pos.alloc(bytes, 1));
+        RX_CHECK_CUDA(h, vel.alloc(bytes, 1));
+        RX_CHECK_CUDA(h, retry.alloc(h->cfg.n_replicas));
+        h->d_pos_snap = std::move(pos); h->d_vel_snap = std::move(vel); h->d_retry = std::move(retry);
     }
     RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_pos_snap, h->d_pos, bytes, cudaMemcpyDeviceToDevice, h->stream));
     RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_vel_snap, h->d_vel, bytes, cudaMemcpyDeviceToDevice, h->stream));
@@ -1222,9 +1240,9 @@ int rxi_restore_failed(rx_engine *h) {
     // a molecule's rows are double[N][3], an LJ replica's float4[N]
     const int words = (h->cfg.system_kind == RX_SYSTEM_MOLECULE ? 3 : 2) * h->cfg.n_atoms;
     using W = unsigned long long;
-    k_restore_failed<<<h->kloc, 256, 0, h->stream>>>(h->d_nan, h->d_retry, h->k0, words, (const W *)h->d_pos_snap,
-                                                    (const W *)h->d_vel_snap, (W *)h->d_pos, (W *)h->d_vel, h->d_box_snap,
-                                                    h->d_baro_snap, h->npt ? h->d_box : nullptr, h->d_baro);
+    k_restore_failed<<<h->kloc, 256, 0, h->stream>>>(h->d_nan, h->d_retry, h->k0, words, (const W *)h->d_pos_snap.get(),
+                                                    (const W *)h->d_vel_snap.get(), (W *)h->d_pos.get(), (W *)h->d_vel.get(), h->d_box_snap,
+                                                    h->d_baro_snap, h->npt ? h->d_box.get() : nullptr, h->d_baro);
     RX_CHECK_CUDA(h, cudaGetLastError());
     return RX_OK;
 }
@@ -1360,13 +1378,13 @@ __global__ void __launch_bounds__(1024) k_minimize(DynParams p, const float4 *__
 int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_rms, int *d_iters) {
     if (h->kloc == 0) return RX_OK;
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
-        const MolDev *m = (const MolDev *)h->mol_dev;
-        const MolGB *gb = (const MolGB *)h->mol_gb;
+        const MolDev *m = &h->mol->dev;
+        const MolGB *gb = mol_gb_of(h);
         auto kern = gb ? k_minimize_mol<true> : k_minimize_mol<false>;
         const int dyn = mol_dyn_bytes(*m, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
-        kern<<<h->kloc, 32, dyn, h->stream>>>(*m, (double *)h->d_pos, h->k0, tolerance, max_iterations > 0 ? max_iterations : 100000,
+        kern<<<h->kloc, 32, dyn, h->stream>>>(*m, (double *)h->d_pos.get(), h->k0, tolerance, max_iterations > 0 ? max_iterations : 100000,
                                               d_rms, d_iters, gb ? *gb : MolGB{});
         RX_CHECK_CUDA(h, cudaGetLastError());
         return RX_OK;
@@ -1393,7 +1411,7 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
                 return with_flag(wide, [&](auto w) {
                     return with_flag(h->two_regions, [&](auto rg) {
                         return launch_kernel(h, lc, wide, k_minimize<c6, sw, w ? 4 : 1, np, rg>, p, (const float4 *)h->d_atom,
-                                             (const StateDev *)h->d_states, (const int *)h->d_perm, h->d_pos, h->k0,
+                                             (const StateDev *)h->d_states, (const int *)h->d_perm, h->d_pos.get(), h->k0,
                                              (float)tolerance, max_iterations, d_rms, d_iters, (const double4 *)h->d_box);
                     });
                 });
@@ -1409,8 +1427,8 @@ int rxi_randomize_velocities(rx_engine *h, uint64_t seed, uint64_t stream_id) {
     if (h->kloc == 0) return RX_OK;
     const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {   // (k_propagate_mol projects incoming velocities onto the constraints)
-        k_randomize_velocities_mol<<<h->kloc, 32, 0, h->stream>>>(*(const MolDev *)h->mol_dev, (const StateDev *)h->d_states,
-                                                                 (const int *)h->d_perm, (double *)h->d_vel, h->k0, key, (uint32_t)stream_id);
+        k_randomize_velocities_mol<<<h->kloc, 32, 0, h->stream>>>(h->mol->dev, (const StateDev *)h->d_states,
+                                                                 (const int *)h->d_perm, (double *)h->d_vel.get(), h->k0, key, (uint32_t)stream_id);
         RX_CHECK_CUDA(h, cudaGetLastError());
         RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
         return RX_OK;
@@ -1444,13 +1462,13 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     if (h->kloc == 0) return RX_OK;
     const rx_config &c = h->cfg;
     if (c.system_kind == RX_SYSTEM_MOLECULE) {
-        const MolDev *m = (const MolDev *)h->mol_dev;
-        const MolGB *gb = (const MolGB *)h->mol_gb;
+        const MolDev *m = &h->mol->dev;
+        const MolGB *gb = mol_gb_of(h);
         auto kern = gb ? k_energy_mol<true> : k_energy_mol<false>;
         const int dyn = mol_dyn_bytes(*m, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
-        kern<<<h->kloc, 32, dyn, h->stream>>>(*m, d_states, n_states, (const double *)h->d_pos, h->k0, d_out, gb ? *gb : MolGB{});
+        kern<<<h->kloc, 32, dyn, h->stream>>>(*m, d_states, n_states, (const double *)h->d_pos.get(), h->k0, d_out, gb ? *gb : MolGB{});
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
         return RX_OK;
@@ -1466,14 +1484,14 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     const int rco = smem_opt_in(h, (const void *)kern, (int)smem);
     if (rco) return rco;
     kern<<<h->kloc, 512, smem, h->stream>>>(p, h->d_atom_d, h->d_alch_list, d_states, h->d_pos, h->k0,
-                                           (double2 *)h->d_pairs, d_out, h->d_err, h->d_box, d_npt_tab);
+                                           h->d_pairs, d_out, h->d_err, h->d_box, d_npt_tab);
     RX_CHECK_CUDA(h, cudaGetLastError());
     (*launches)++;
     return RX_OK;
 }
 
 int rxi_compute_energy_rows(rx_engine *h, int *launches) {
-    return rxi_compute_energy_rows_at(h, h->d_states, h->cfg.n_states, h->d_u, launches, h->npt ? h->d_npt : nullptr);
+    return rxi_compute_energy_rows_at(h, h->d_states, h->cfg.n_states, h->d_u, launches, h->npt ? h->d_npt.get() : nullptr);
 }
 
 
@@ -1481,14 +1499,11 @@ int rxi_compute_energy_rows(rx_engine *h, int *launches) {
 // Molecule tables (rx_set_molecule): the term list with its slots, packed in f32 and in f64; constraint clusters.
 // ---------------------------------------------------------------------------------------------------
 template <typename T>
-static int mol_upload(rx_engine *h, const std::vector<T> &v, const T **out) {
-    void *d = nullptr;
-    const size_t bytes = sizeof(T) * (v.empty() ? 1 : v.size());
-    RX_CHECK_CUDA(h, cudaMalloc(&d, bytes));
-    RX_CHECK_CUDA(h, cudaMemset(d, 0, bytes));
+static int mol_upload(rx_engine *h, const std::vector<T> &v, DevBuf<T> &d) {
+    const size_t n = v.empty() ? 1 : v.size();
+    RX_CHECK_CUDA(h, d.alloc(n));
+    RX_CHECK_CUDA(h, cudaMemset(d, 0, sizeof(T) * n));
     if (!v.empty()) RX_CHECK_CUDA(h, cudaMemcpy(d, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
-    h->mol_allocs.push_back(d);
-    *out = (const T *)d;
     return RX_OK;
 }
 
@@ -1566,7 +1581,7 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
     if (n > MOL_MAX_ATOMS) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_set_molecule: more than 32 atoms per molecule is not provided");
     if (!mol->mass || !mol->charge || !mol->sigma || !mol->epsilon) RX_FAIL(h, RX_ERR_INVALID, "rx_set_molecule: null per-atom arrays");
     auto atom_ok = [&](double v) { return v >= 0 && v < n && v == floor(v); };
-    rxi_free_molecule(h);         // (a refused molecule leaves the engine without one, not with freed tables)
+    h->mol.reset();               // (a refused molecule leaves the engine without one, not with freed tables)
     h->have_particles = false;
     std::vector<double> mass(mol->mass, mol->mass + n), charge(mol->charge, mol->charge + n), sigma(mol->sigma, mol->sigma + n),
         eps(mol->epsilon, mol->epsilon + n);
@@ -1657,8 +1672,8 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
     for (int i = 0; i < n; i++) h->mol_cluster[i] = cluster_of[find(i)];
     std::vector<MolCons> cons;
     for (auto &c : cl) { cons.insert(cons.end(), c.begin(), c.end()); c_off.push_back((int)cons.size()); }
-    MolDev *m = (MolDev *)h->mol_dev;
-    if (!m) { m = new MolDev(); h->mol_dev = m; }
+    RecordPtr<MolTables> tables(new MolTables());   // (value-initialised: gb.on == 0)
+    MolDev *m = &tables->dev;
     memset(m, 0, sizeof(*m));
     m->n = n; m->n_clusters = (int)cl.size(); m->remove_cm = mol->remove_cm_motion ? 1 : 0;
     for (auto &c : cl) m->max_cluster = std::max(m->max_cluster, (int)c.size());
@@ -1667,35 +1682,23 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
     m->bytes32 = (int)t32.size(); m->bytes64 = (int)t64.size();
     m->n_tb = (int)L.b.size(); m->n_ta = (int)L.a.size(); m->n_tt = (int)L.t.size(); m->n_tp = (int)L.p.size(); m->n_slots = slot;
     int rc = mol_check_shared(h, *m, nullptr, "rx_set_molecule: the term tables");
-    if (rc) { rxi_free_molecule(h); return rc; }
-    const unsigned char *d32 = nullptr, *d64 = nullptr;
-    if ((rc = mol_upload(h, mass, &m->mass)) || (rc = mol_upload(h, charge, &m->charge)) || (rc = mol_upload(h, c_off, &m->c_off)) ||
-        (rc = mol_upload(h, cons, &m->cons)) || (rc = mol_upload(h, t32, &d32)) || (rc = mol_upload(h, t64, &d64)))
+    if (rc) return rc;
+    MolTables &t = *tables;
+    if ((rc = mol_upload(h, mass, t.mass)) || (rc = mol_upload(h, charge, t.charge)) || (rc = mol_upload(h, c_off, t.c_off)) ||
+        (rc = mol_upload(h, cons, t.cons)) || (rc = mol_upload(h, t32, t.terms32)) || (rc = mol_upload(h, t64, t.terms64)))
         return rc;
-    m->terms32 = (const MolTerms *)d32; m->terms64 = (const MolTerms *)d64;
+    m->mass = t.mass; m->charge = t.charge; m->c_off = t.c_off; m->cons = t.cons;
+    m->terms32 = (const MolTerms *)t.terms32.get(); m->terms64 = (const MolTerms *)t.terms64.get();
+    h->mol = std::move(tables);
     h->have_particles = true;
     return RX_OK;
-}
-
-void rxi_free_molecule(rx_engine *h) {
-    for (void *d : h->mol_allocs) cudaFree(d);
-    h->mol_allocs.clear();
-    delete (MolDev *)h->mol_dev;
-    h->mol_dev = nullptr;
-    rxi_free_implicit_solvent(h);
-}
-
-void rxi_free_implicit_solvent(rx_engine *h) {
-    if (h->mol_gb) cudaFree((void *)((MolGB *)h->mol_gb)->atom);
-    delete (MolGB *)h->mol_gb;
-    h->mol_gb = nullptr;
 }
 
 // OBC implicit solvent (rx_set_implicit_solvent): the per-atom table and the constants of MolGB.  A refused call leaves the
 // engine as it was.
 int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s) {
-    const MolDev *m = (const MolDev *)h->mol_dev;
-    if (!m) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: call rx_set_molecule first");
+    if (!h->mol) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: call rx_set_molecule first");
+    const MolDev *m = &h->mol->dev;
     const int n = m->n;
     if (!s->radius || !s->scale) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: null per-atom arrays");
     if (!(s->offset >= 0) || !(s->solute_dielectric > 0) || !(s->solvent_dielectric > 0) || !(s->sa_energy >= 0) ||
@@ -1718,13 +1721,12 @@ int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s) {
     g.prop_bytes = (int)(sizeof(double) * (4 * (size_t)n * n + 3 * (size_t)n));
     const int rc = mol_check_shared(h, *m, &g, "rx_set_implicit_solvent: the term and solvent tables");
     if (rc) return rc;
-    void *d = nullptr;
-    RX_CHECK_CUDA(h, cudaMalloc(&d, sizeof(double) * tab.size()));
-    const cudaError_t e = cudaMemcpy(d, tab.data(), sizeof(double) * tab.size(), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { cudaFree(d); RX_CHECK_CUDA(h, e); }
-    rxi_free_implicit_solvent(h);
-    g.atom = (const double *)d;
-    h->mol_gb = new MolGB(g);
+    DevBuf<double> atom;
+    RX_CHECK_CUDA(h, atom.alloc(tab.size()));
+    RX_CHECK_CUDA(h, cudaMemcpy(atom, tab.data(), sizeof(double) * tab.size(), cudaMemcpyHostToDevice));
+    g.atom = atom;
+    h->mol->gb = g;
+    h->mol->gb_atom = std::move(atom);
     return RX_OK;
 }
 

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <memory>
 #include <string>
 #include <vector>
 #include <utility>
@@ -25,11 +26,49 @@ struct StateDev {
     double lambda2, la2, ob2;
 };
 
+// ---- owned memory ---------------------------------------------------------------------------------------------------
+// n elements of T in device memory (Pinned: page-locked host memory), freed by the destructor.  Move-only.  It converts to its
+// raw pointer: the kernels' arguments and parameter structs (MolDev, MolGB, EnParams, DynParams) are views of owned memory.
+template <typename T, bool Pinned = false> class CudaBuf {
+  public:
+    CudaBuf() = default;
+    CudaBuf(CudaBuf &&o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+    CudaBuf &operator=(CudaBuf &&o) noexcept {
+        if (this != &o) { release(p_); p_ = o.p_; o.p_ = nullptr; }
+        return *this;
+    }
+    ~CudaBuf() { release(p_); }
+    operator T *() const { return p_; }
+    T *get() const { return p_; }
+    // n elements of `elem` bytes each in place of what it holds, which is released only once the new storage exists: a
+    // failure leaves the buffer as it was.
+    cudaError_t alloc(size_t n, size_t elem = sizeof(T)) {
+        void *q = nullptr;
+        const cudaError_t e = Pinned ? cudaHostAlloc(&q, n * elem, cudaHostAllocDefault) : cudaMalloc(&q, n * elem);
+        if (e == cudaSuccess) { release(p_); p_ = (T *)q; }
+        return e;
+    }
+
+  private:
+    static void release(T *p) { if (p && Pinned) cudaFreeHost(p); else if (p) cudaFree(p); }
+    T *p_ = nullptr;
+};
+template <typename T> using DevBuf = CudaBuf<T>;
+template <typename T> using PinnedBuf = CudaBuf<T, true>;
+
+struct MoveDev;     // rx_dynamics.cu: the elements of rx_engine::d_moves
+// Host records that own device buffers, complete only in the translation unit that uses them, where each overload of
+// RecordDelete is defined.
+struct SamsState;   // rx_sams.cuh
+struct MolTables;   // rx_dynamics.cu
+struct RecordDelete { void operator()(SamsState *) const; void operator()(MolTables *) const; };
+template <typename T> using RecordPtr = std::unique_ptr<T, RecordDelete>;
+
 // ---- MT19937 stream resident on the device (numba's / numpy's generator restated) ---------------------
 struct MTStream {
-    uint32_t *d_window = nullptr;  // last 624 raw words x_n .. x_{n+623}
-    uint32_t *d_words = nullptr;   // tempered outputs not yet consumed: d_words[0..avail)
-    uint32_t *d_words_alt = nullptr;
+    DevBuf<uint32_t> d_window;   // last 624 raw words x_n .. x_{n+623}
+    DevBuf<uint32_t> d_words;    // tempered outputs not yet consumed: d_words[0..avail)
+    DevBuf<uint32_t> d_words_alt;
     size_t cap = 0;
     size_t avail = 0;
     uint64_t consumed = 0;  // words consumed since seeding
@@ -82,67 +121,65 @@ struct rx_engine {
     long long mix_stats[6] = {0, 0, 0, 0, 0, 0};   // rounds, exact-exp, passes, words, walker us, prepare-wait us
     cudaEvent_t ev_walk[2] = {};
     // particles
-    float4 *d_atom = nullptr;     // (sigma, sqrt_eps, inv_mass, alch ? 1 : 0), or the region id (0, 1, 2) with two regions
-    double4 *d_atom_d = nullptr;  // (sigma, eps, mass, alch or region id)
+    DevBuf<float4> d_atom;        // (sigma, sqrt_eps, inv_mass, alch ? 1 : 0), or the region id (0, 1, 2) with two regions
+    DevBuf<double4> d_atom_d;     // (sigma, eps, mass, alch or region id)
     std::vector<float4> h_atom;   // host copies of both (rx_set_alchemical_regions rewrites their w)
     std::vector<double4> h_atom_d;
     int n_alch = 0;
-    int *d_alch_list = nullptr;   // indices of the alchemical atoms (of either region)
+    DevBuf<int> d_alch_list;      // indices of the alchemical atoms (of either region)
     // two alchemical regions (rx_set_alchemical_regions): the two-region kernel instantiations run, and their pair rules
     // read the annihilate flags as bit 0 (region 1) and bit 1 (region 2) of DynParams / EnParams::annihilate
     bool two_regions = false;
     int annihilate_mask = 0;
     bool have_particles = false, have_states = false, have_integrator = false;
-    StateDev *d_states = nullptr;
+    DevBuf<StateDev> d_states;
     std::vector<StateDev> h_states;
     // replica state
-    float4 *d_pos = nullptr, *d_vel = nullptr;  // [kloc][N]
-    float4 *d_pos_snap = nullptr, *d_vel_snap = nullptr;   // start-of-iteration copy for the NaN restart policy
-    int *d_retry = nullptr;                     // [K] replicas to propagate again
+    DevBuf<float4> d_pos, d_vel;                // [kloc][N]
+    DevBuf<float4> d_pos_snap, d_vel_snap;      // start-of-iteration copy for the NaN restart policy
+    DevBuf<int> d_retry;                        // [K] replicas to propagate again
     bool have_snapshot = false;
-    double *d_io = nullptr;                     // staging for set/get: [kloc][N][3]
-    double *h_io = nullptr;                     // pinned host staging of the same size
+    DevBuf<double> d_io;                        // staging for set/get: [kloc][N][3]
+    PinnedBuf<double> h_io;                     // pinned host staging of the same size
     std::vector<std::pair<const char *, size_t>> pinned;   // caller buffers registered with rx_pin_host_memory
-    int *d_perm = nullptr;                      // [K] replica -> state
-    double *d_u = nullptr;                      // [K][M]
-    unsigned long long *d_nacc = nullptr, *d_nprop = nullptr;  // [M][M]
-    double *d_pot = nullptr, *d_kin = nullptr;  // [K]
-    int *d_nan = nullptr;                       // [K]
-    int *d_err = nullptr;                       // device error flag (capacity overflow, ...)
+    DevBuf<int> d_perm;                         // [K] replica -> state
+    DevBuf<double> d_u;                         // [K][M]
+    DevBuf<unsigned long long> d_nacc, d_nprop;  // [M][M]
+    DevBuf<double> d_pot, d_kin;                // [K]
+    DevBuf<int> d_nan;                          // [K]
+    DevBuf<int> d_err;                          // device error flag (capacity overflow, ...)
     // energy kernel scratch: lambda-controlled pairs per owned replica
-    double4 *d_pairs = nullptr;  // (r, sigma, eps, S) ... see rx_dynamics.cu
+    DevBuf<double2> d_pairs;   // [kloc][pair_cap]: ((r / sigma)^c, negative in region 2; 4 eps S(r)) of k_energy_rows
     int pair_cap = 0;
     // integrator
     double dt = 0, gamma = 0;
     int n_steps = 0;
     char program[RX_MAX_PROGRAM] = {0};
-    void *mol_dev = nullptr;                 // MolDev (host copy of the device table of a RX_SYSTEM_MOLECULE engine)
-    std::vector<void *> mol_allocs;
-    void *mol_gb = nullptr;                  // MolGB (host copy; nullptr: vacuum) and its device table, rx_set_implicit_solvent
+    RecordPtr<MolTables> mol;                // the molecule of a RX_SYSTEM_MOLECULE engine: device tables, MolDev and MolGB
     std::vector<rx_state_move> state_moves;   // per-state moves (empty: one move for all states)
     bool state_moves_dirty = false;
-    void *d_moves = nullptr;
+    DevBuf<MoveDev> d_moves;
     std::vector<int> mol_cluster;            // constraint cluster of each atom of a molecule (-1: unconstrained)
     // Monte Carlo moves (rx_set_state_mc_moves): [M][RX_MAX_MC_MOVES] records, kind -1 where a state has fewer moves
     std::vector<int32_t> mc_atoms;           // rx_set_mc_subsets
-    int32_t *d_mc_atoms = nullptr;
+    DevBuf<int32_t> d_mc_atoms;
     std::vector<rx_mc_move> mc_moves;
-    rx_mc_move *d_mc_moves = nullptr;
+    DevBuf<rx_mc_move> d_mc_moves;
     int mc_slots = 0;                        // the most moves any state has: launches per propagation
-    unsigned long long *d_mc_acc = nullptr, *d_mc_prop = nullptr;   // [M][RX_MAX_MC_MOVES]
-    double *d_mc_du = nullptr;               // [kloc][RX_MAX_MC_MOVES]: dU of each owned replica's last proposal per slot
+    DevBuf<unsigned long long> d_mc_acc, d_mc_prop;   // [M][RX_MAX_MC_MOVES]
+    DevBuf<double> d_mc_du;                  // [kloc][RX_MAX_MC_MOVES]: dU of each owned replica's last proposal per slot
     // mixing
     MTStream streams[2];
-    uint4 *d_slots = nullptr;   // the 16-byte records of a pass: SlotRec, SlotRec2 or CandRec
+    DevBuf<uint4> d_slots;      // the 16-byte records of a pass: SlotRec, SlotRec2 or CandRec
     size_t slots_cap = 0;
-    MixCtl *d_ctl = nullptr;
-    uint32_t *d_log = nullptr;   // commit log of the walker: packed (si, sj, accepted)
-    uint32_t *d_slotlog = nullptr;   // sparse commit log of k_mix_walk2: one word per slot
-    uint32_t *d_cpos = nullptr;      // k_mix_walk2c / k_mix_walk_cand: word position of every candidate of the pass
-    uint32_t *d_ctile = nullptr;     // ... candidates per tile / their exclusive scan, then [last] = number of candidates
+    DevBuf<MixCtl> d_ctl;
+    DevBuf<uint32_t> d_log;      // commit log of the walker: packed (si, sj, accepted)
+    DevBuf<uint32_t> d_slotlog;      // sparse commit log of k_mix_walk2: one word per slot
+    DevBuf<uint32_t> d_cpos;         // k_mix_walk2c / k_mix_walk_cand: word position of every candidate of the pass
+    DevBuf<uint32_t> d_ctile;        // ... candidates per tile / their exclusive scan, then [last] = number of candidates
     size_t ctile_cap = 0;
-    unsigned char *d_filt = nullptr;   // 24-bit row image of u for the K=256 walker
-    double *d_filt_scale = nullptr;    // [K] scales + [K] row abs-max
+    DevBuf<unsigned char> d_filt;      // 24-bit row image of u for the K=256 walker
+    DevBuf<double> d_filt_scale;       // [K] scales + [K] row abs-max
     struct {
         bool valid = false;       // words + records for the next swap-all call were produced on stream_rng ...
         MixPlan plan = {};        // ... for this plan
@@ -150,15 +187,15 @@ struct rx_engine {
     } prepared;
     size_t last_consumed = 0;     // words the previous swap-all call consumed (sizes the generate-ahead)
     cudaEvent_t ev_prepared = nullptr, ev_consumed = nullptr;
-    void *sams = nullptr;         // SamsState (rx_sams.cuh): device-resident logZ / weights / histogram of a SAMSSampler
+    RecordPtr<SamsState> sams;    // SamsState (rx_sams.cuh): device-resident logZ / weights / histogram of a SAMSSampler
     // timing
     double phase_ms[4] = {0, 0, 0, 0};
     long long phase_launches[4] = {0, 0, 0, 0};
     // constant pressure (rx_set_pressures): per owned replica box (x, y, z, -) and barostat state, per state (p, c)
     bool npt = false;
-    double4 *d_box = nullptr, *d_box_snap = nullptr;
-    rx_barostat_state *d_baro = nullptr, *d_baro_snap = nullptr;
-    double2 *d_npt = nullptr;
+    DevBuf<double4> d_box, d_box_snap;
+    DevBuf<rx_barostat_state> d_baro, d_baro_snap;
+    DevBuf<double2> d_npt;
     // nccl
     void *nccl_lib = nullptr;
     void *nccl_comm = nullptr;
@@ -203,22 +240,18 @@ int rxi_mix_skip(rx_engine *h, int stream, unsigned long long n);
 int rxi_selftest_exp(rx_engine *h, const double *x, double *y, int n);
 int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches);
 int rxi_mix_swap_neighbors(rx_engine *h, int *launches);
-void rxi_mix_free(rx_engine *h);
 int rxi_sams_set(rx_engine *h, const rx_sams_config *c, const double *log_target, const double *logZ, const int64_t *histogram);
 int rxi_sams_step(rx_engine *h, long long iteration, int update, int *launches);
 int rxi_sams_get(rx_engine *h, double *logZ, double *log_weights, int64_t *histogram, int32_t *stage, int64_t *t0, double *gamma,
                  int64_t *states, int64_t *previous_states);
 int rxi_sams_set_histogram(rx_engine *h, const int64_t *histogram);
-void rxi_sams_free(rx_engine *h);
 
 // ---- implemented in rx_dynamics.cu ----
 int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign, int *launches, const int *d_only = nullptr);
 int rxi_plan_propagate(const rx_propagate_query *q, rx_propagate_plan *out, std::string &err);   // host arithmetic only
 int rxi_upload_state_moves(rx_engine *h);
 int rxi_set_molecule(rx_engine *h, const rx_molecule *mol);
-void rxi_free_molecule(rx_engine *h);
 int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s);
-void rxi_free_implicit_solvent(rx_engine *h);
 int rxi_mc_moves(rx_engine *h, uint64_t seed, uint64_t iteration, int *launches);   // one launch per MC slot (rx_mc.cuh)
 int rxi_snapshot_state(rx_engine *h);   // positions + velocities at the start of a propagation
 int rxi_restore_failed(rx_engine *h);   // replicas with a NaN flag go back to the snapshot; d_retry = the flags

@@ -274,14 +274,14 @@ int rxi_mc_moves(rx_engine *h, uint64_t seed, uint64_t iteration, int *launches)
     const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(iteration >> 32));
     const uint32_t it32 = (uint32_t)iteration;
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
-        const MolDev *md = (const MolDev *)h->mol_dev;
-        const MolGB *gb = (const MolGB *)h->mol_gb;
+        const MolDev *md = &h->mol->dev;
+        const MolGB *gb = mol_gb_of(h);
         auto kern = gb ? k_mc_move_mol<true> : k_mc_move_mol<false>;
         const int dyn = mol_dyn_bytes(*md, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
         for (int s = 0; s < h->mc_slots; s++) {
-            kern<<<h->kloc, 32, dyn, h->stream>>>(*md, h->d_states, h->d_perm, h->d_mc_moves, h->d_mc_atoms, (double *)h->d_pos, h->k0,
+            kern<<<h->kloc, 32, dyn, h->stream>>>(*md, h->d_states, h->d_perm, h->d_mc_moves, h->d_mc_atoms, (double *)h->d_pos.get(), h->k0,
                                                   s, key, it32, h->d_mc_acc, h->d_mc_prop, h->d_mc_du, gb ? *gb : MolGB{});
             RX_CHECK_CUDA(h, cudaGetLastError());
         }

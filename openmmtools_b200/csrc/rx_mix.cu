@@ -161,15 +161,14 @@ __global__ void k_selftest_exp(const double *__restrict__ x, double *__restrict_
     if (t < n) y[t] = rx_exp_cr(x[t]);
 }
 int rxi_selftest_exp(rx_engine *h, const double *x, double *y, int n) {
-    double *d = nullptr;
+    DevBuf<double> d;
     if (n <= 0) return RX_OK;
-    RX_CHECK_CUDA(h, cudaMalloc(&d, 2 * (size_t)n * sizeof(double)));
+    RX_CHECK_CUDA(h, d.alloc(2 * (size_t)n));
     RX_CHECK_CUDA(h, cudaMemcpy(d, x, (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
     k_selftest_exp<<<(n + 127) / 128, 128, 0, h->stream>>>(d, d + n, n);
     RX_CHECK_CUDA(h, cudaGetLastError());
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
     RX_CHECK_CUDA(h, cudaMemcpy(y, d + n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
-    cudaFree(d);
     return RX_OK;
 }
 
@@ -341,15 +340,12 @@ __global__ void __launch_bounds__(32) k_mix_neighbors(const uint32_t *__restrict
 // ------------------------------------------------------------------------------------------------------
 static int stream_reserve(rx_engine *h, MTStream &S, size_t cap) {
     if (cap <= S.cap) return RX_OK;
-    uint32_t *a = nullptr, *b = nullptr;
-    RX_CHECK_CUDA(h, cudaMalloc(&a, cap * sizeof(uint32_t)));
-    RX_CHECK_CUDA(h, cudaMalloc(&b, cap * sizeof(uint32_t)));
+    DevBuf<uint32_t> a, b;
+    RX_CHECK_CUDA(h, a.alloc(cap));
+    RX_CHECK_CUDA(h, b.alloc(cap));
     if (S.avail) RX_CHECK_CUDA(h, cudaMemcpyAsync(a, S.d_words, S.avail * sizeof(uint32_t), cudaMemcpyDeviceToDevice, h->stream));
     RX_CHECK_CUDA(h, cudaDeviceSynchronize());
-    cudaFree(S.d_words);
-    cudaFree(S.d_words_alt);
-    S.d_words = a;
-    S.d_words_alt = b;
+    S.d_words = std::move(a); S.d_words_alt = std::move(b);
     S.cap = cap;
     return RX_OK;
 }
@@ -388,7 +384,7 @@ int rxi_mix_seed(rx_engine *h, int stream, uint32_t seed) {
     uint32_t mt[624];
     mt[0] = seed;  // init_genrand, numba/_random.c:59-73
     for (int i = 1; i < 624; i++) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (uint32_t)i;
-    if (!S.d_window) RX_CHECK_CUDA(h, cudaMalloc(&S.d_window, 624 * sizeof(uint32_t)));
+    if (!S.d_window) RX_CHECK_CUDA(h, S.d_window.alloc(624));
     RX_CHECK_CUDA(h, cudaMemcpy(S.d_window, mt, sizeof(mt), cudaMemcpyHostToDevice));
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream_rng));
     if (stream == RX_STREAM_NUMBA) { h->prepared.valid = false; h->last_consumed = 0; }
@@ -488,24 +484,21 @@ static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, const Mi
             // `avail` of every iteration never triggers another cudaFree/cudaMalloc (tens of ms each, device-synchronising)
             size_t want = cand ? S.cap : (S.cap + 1) / 2;
             if (want < (size_t)nslots) want = (size_t)nslots;
+            DevBuf<uint4> slots;
+            DevBuf<uint32_t> log, slotlog;
+            RX_CHECK_CUDA(h, slots.alloc(want));
+            RX_CHECK_CUDA(h, log.alloc(want));
+            RX_CHECK_CUDA(h, slotlog.alloc(want));
             RX_CHECK_CUDA(h, cudaDeviceSynchronize());
-            cudaFree(h->d_slots);
-            cudaFree(h->d_log);
-            h->d_slots = nullptr; h->d_log = nullptr;
-            h->slots_cap = 0;
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_slots, want * sizeof(uint4)));
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_log, want * sizeof(uint32_t)));
-            cudaFree(h->d_slotlog);
-            h->d_slotlog = nullptr;
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_slotlog, want * sizeof(uint32_t)));
+            h->d_slots = std::move(slots); h->d_log = std::move(log); h->d_slotlog = std::move(slotlog);
             h->slots_cap = want;
         }
         if (cand && (!h->d_cpos || h->ctile_cap < h->slots_cap)) {
+            DevBuf<uint32_t> cpos, ctile;
+            RX_CHECK_CUDA(h, cpos.alloc(h->slots_cap + 8));
+            RX_CHECK_CUDA(h, ctile.alloc(h->slots_cap / CAND_TILE + 8));
             RX_CHECK_CUDA(h, cudaDeviceSynchronize());
-            cudaFree(h->d_cpos); cudaFree(h->d_ctile);
-            h->d_cpos = nullptr; h->d_ctile = nullptr;
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_cpos, (h->slots_cap + 8) * sizeof(uint32_t)));
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_ctile, (h->slots_cap / CAND_TILE + 8) * sizeof(uint32_t)));
+            h->d_cpos = std::move(cpos); h->d_ctile = std::move(ctile);
             h->ctile_cap = h->slots_cap;
         }
         if (cand) {
@@ -519,14 +512,14 @@ static int prepare_pass(rx_engine *h, MTStream &S, long long remaining, const Mi
             k_cand_scan<<<1, 1024, 0, st>>>(h->d_ctile, ntiles, cand_total(h));
             k_cand_scatter<<<ntiles, 256, 0, st>>>(S.d_words, nslots, K, mask, h->d_ctile, h->d_cpos);
             if (p.filter)
-                k_cand_records<false><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (SlotRec2 *)h->d_slots);
+                k_cand_records<false><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (SlotRec2 *)h->d_slots.get());
             else
-                k_cand_records<true><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (CandRec *)h->d_slots);
+                k_cand_records<true><<<nblk, 256, 0, st>>>(S.d_words, h->d_cpos, cand_total(h), mask, (CandRec *)h->d_slots.get());
             *launches += 3;
         } else if (p.filter)
-            k_slots_build<true><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec2 *)h->d_slots);
+            k_slots_build<true><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec2 *)h->d_slots.get());
         else
-            k_slots_build<false><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec *)h->d_slots);
+            k_slots_build<false><<<(unsigned)((nslots + 255) / 256), 256, 0, st>>>(S.d_words, nslots, (uint32_t)(K - 1), (SlotRec *)h->d_slots.get());
         RX_CHECK_CUDA(h, cudaGetLastError());
         (*launches)++;
     }
@@ -562,8 +555,11 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
     if (p.smem_tail > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(tail, cudaFuncAttributeMaxDynamicSharedMemorySize, p.smem_tail));
     if (p.filter) {
         if (!h->d_filt) {
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt, (size_t)3 * K * K + 16));
-            RX_CHECK_CUDA(h, cudaMalloc(&h->d_filt_scale, sizeof(double) * 2 * K));
+            DevBuf<unsigned char> filt;
+            DevBuf<double> scale;
+            RX_CHECK_CUDA(h, filt.alloc((size_t)3 * K * K + 16));
+            RX_CHECK_CUDA(h, scale.alloc(2 * (size_t)K));
+            h->d_filt = std::move(filt); h->d_filt_scale = std::move(scale);
         }
         // row image + |row minimum| for the per-lane error bound; non-finite or astronomically large entries only send the
         // lanes that touch them to the exact path (no host round trip, no global fallback)
@@ -613,14 +609,14 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
             // and reports the extent of that log in ctl.aux
             RX_CHECK_CUDA(h, cudaMemsetAsync(h->d_slotlog, 0, nrec * sizeof(uint32_t), h->stream));
             if (p.coords == MIX_SLOTS)
-                k_mix_walk2<<<1, W2_THREADS, WALK_SMEM, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K,
+                k_mix_walk2<<<1, W2_THREADS, WALK_SMEM, h->stream>>>((const SlotRec2 *)h->d_slots.get(), S.d_words, (unsigned)nrec, h->d_u, K,
                                                                    logK, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale, h->d_ctl);
             else
-                k_mix_walk2c<<<1, W2_THREADS, WALK_SMEM, h->stream>>>((const SlotRec2 *)h->d_slots, S.d_words, h->d_cpos, cand_total(h),
+                k_mix_walk2c<<<1, W2_THREADS, WALK_SMEM, h->stream>>>((const SlotRec2 *)h->d_slots.get(), S.d_words, h->d_cpos, cand_total(h),
                                                                     h->d_u, K, h->d_perm, h->d_slotlog, h->d_filt, h->d_filt_scale,
                                                                     h->d_ctl);
         } else if (p.coords == MIX_CANDS)
-            k_mix_walk_cand<<<1, 64, WALK_SMEM, h->stream>>>((const CandRec *)h->d_slots, S.d_words, h->d_cpos, cand_total(h), h->d_u, K,
+            k_mix_walk_cand<<<1, 64, WALK_SMEM, h->stream>>>((const CandRec *)h->d_slots.get(), S.d_words, h->d_cpos, cand_total(h), h->d_u, K,
                                                                h->d_perm, h->d_log, h->d_ctl);
         if (bulk) {
             RX_CHECK_CUDA(h, cudaGetLastError());
@@ -628,8 +624,8 @@ int rxi_mix_swap_all(rx_engine *h, long long nswap, int *launches) {
         }
         // the pass's tail continues from ctl.head
         if (p.coords == MIX_SLOTS)
-            walk_pow2<<<1, 64, p.smem_tail, h->stream>>>((const SlotRec *)h->d_slots, S.d_words, (unsigned)nrec, h->d_u, K, logK, h->d_perm,
-                                                         h->d_log, p.filter ? h->d_filt : nullptr, p.filter ? h->d_filt_scale : nullptr, h->d_ctl);
+            walk_pow2<<<1, 64, p.smem_tail, h->stream>>>((const SlotRec *)h->d_slots.get(), S.d_words, (unsigned)nrec, h->d_u, K, logK, h->d_perm,
+                                                         h->d_log, p.filter ? h->d_filt.get() : nullptr, p.filter ? h->d_filt_scale.get() : nullptr, h->d_ctl);
         if (timed) RX_CHECK_CUDA(h, cudaEventRecord(h->ev_walk[1], h->stream));
         if (p.coords != MIX_SLOTS)
             k_mix_walk_serial<<<1, 32, p.smem_tail, h->stream>>>(S.d_words, (long long)S.avail, h->d_u, K, M, h->d_perm, h->d_nacc,
@@ -705,22 +701,6 @@ int rxi_mix_swap_neighbors(rx_engine *h, int *launches) {
     RX_CHECK_CUDA(h, cudaMemcpyAsync(&ctl, h->d_ctl, sizeof(ctl), cudaMemcpyDeviceToHost, h->stream));
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
     return stream_consume(h, S, (size_t)ctl.head, launches);
-}
-
-void rxi_mix_free(rx_engine *h) {
-    for (int s = 0; s < 2; s++) {
-        cudaFree(h->streams[s].d_window);
-        cudaFree(h->streams[s].d_words);
-        cudaFree(h->streams[s].d_words_alt);
-    }
-    cudaFree(h->d_slots);
-    cudaFree(h->d_log);
-    cudaFree(h->d_slotlog);
-    cudaFree(h->d_cpos);
-    cudaFree(h->d_ctile);
-    cudaFree(h->d_filt);
-    cudaFree(h->d_filt_scale);
-    cudaFree(h->d_ctl);
 }
 
 #include "rx_sams.cuh"

@@ -37,11 +37,12 @@ struct SamsCtl {      // device-resident scalars
 struct SamsState {
     SamsCfg cfg;
     int M = 0;
-    double *d_logZ = nullptr, *d_log_pi = nullptr, *d_log_w = nullptr;
-    long long *d_hist = nullptr;
-    int *d_prev = nullptr;   // [K] states before the last jump
-    SamsCtl *d_ctl = nullptr;
+    DevBuf<double> d_logZ, d_log_pi, d_log_w;
+    DevBuf<long long> d_hist;
+    DevBuf<int> d_prev;   // [K] states before the last jump
+    DevBuf<SamsCtl> d_ctl;
 };
+void RecordDelete::operator()(SamsState *s) const { delete s; }
 
 #define SAMS_THREADS 256
 
@@ -147,26 +148,24 @@ __global__ void __launch_bounds__(SAMS_THREADS) k_sams_step(const uint32_t *__re
     }
 }
 
-static SamsState *sams_of(rx_engine *h) { return (SamsState *)h->sams; }
-
 int rxi_sams_set(rx_engine *h, const rx_sams_config *c, const double *log_target, const double *logZ, const int64_t *histogram) {
     const int M = h->cfg.n_states, K = h->cfg.n_replicas;
     if (M > 4096) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_sams_set: more than 4096 states");
     if (c->weight_update_method < 0 || c->weight_update_method > 1 || c->flatness_criteria < 0 || c->flatness_criteria > 2 ||
         c->stage < 0 || c->stage > 1 || !(c->gamma0 > 0))
         RX_FAIL(h, RX_ERR_INVALID, "rx_sams_set: bad configuration");
-    SamsState *s = sams_of(h);
-    if (!s) {
-        s = new SamsState();
-        h->sams = s;
-        s->M = M;
-        RX_CHECK_CUDA(h, cudaMalloc(&s->d_logZ, sizeof(double) * M));
-        RX_CHECK_CUDA(h, cudaMalloc(&s->d_log_pi, sizeof(double) * M));
-        RX_CHECK_CUDA(h, cudaMalloc(&s->d_log_w, sizeof(double) * M));
-        RX_CHECK_CUDA(h, cudaMalloc(&s->d_hist, sizeof(long long) * M));
-        RX_CHECK_CUDA(h, cudaMalloc(&s->d_prev, sizeof(int) * K));
-        RX_CHECK_CUDA(h, cudaMalloc(&s->d_ctl, sizeof(SamsCtl)));
+    if (!h->sams) {   // taken by the engine once all its buffers exist
+        RecordPtr<SamsState> fresh(new SamsState());
+        fresh->M = M;
+        RX_CHECK_CUDA(h, fresh->d_logZ.alloc(M));
+        RX_CHECK_CUDA(h, fresh->d_log_pi.alloc(M));
+        RX_CHECK_CUDA(h, fresh->d_log_w.alloc(M));
+        RX_CHECK_CUDA(h, fresh->d_hist.alloc(M));
+        RX_CHECK_CUDA(h, fresh->d_prev.alloc(K));
+        RX_CHECK_CUDA(h, fresh->d_ctl.alloc(1));
+        h->sams = std::move(fresh);
     }
+    SamsState *s = h->sams.get();
     s->cfg = SamsCfg{c->gamma0, c->flatness_threshold, 0.8, c->weight_update_method, c->two_stage ? 1 : 0, c->flatness_criteria, 0};
     std::vector<double> lw(M);
     std::vector<long long> hh(M, 0);
@@ -183,7 +182,7 @@ int rxi_sams_set(rx_engine *h, const rx_sams_config *c, const double *log_target
 }
 
 int rxi_sams_set_histogram(rx_engine *h, const int64_t *histogram) {
-    SamsState *s = sams_of(h);
+    const SamsState *s = h->sams.get();
     if (!s) RX_FAIL(h, RX_ERR_INVALID, "rx_sams_step: rx_sams_set must be called first");
     RX_CHECK_CUDA(h, cudaMemcpyAsync(s->d_hist, histogram, sizeof(long long) * s->M, cudaMemcpyHostToDevice, h->stream));
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));   // (the caller's buffer may be pageable and short-lived)
@@ -192,7 +191,7 @@ int rxi_sams_set_histogram(rx_engine *h, const int64_t *histogram) {
 
 // one jump (+ update) on the engine's stream; no host synchronisation
 int rxi_sams_step(rx_engine *h, long long iteration, int update, int *launches) {
-    SamsState *s = sams_of(h);
+    const SamsState *s = h->sams.get();
     if (!s) RX_FAIL(h, RX_ERR_INVALID, "rx_sams_step: rx_sams_set must be called first");
     MTStream &S = h->streams[RX_STREAM_NUMPY];
     if (!S.seeded) RX_FAIL(h, RX_ERR_INVALID, "rx_sams_step: the numpy MT19937 stream has not been seeded (rx_mix_seed)");
@@ -202,7 +201,7 @@ int rxi_sams_step(rx_engine *h, long long iteration, int update, int *launches) 
     const size_t smem = 2 * (size_t)M * sizeof(double);
     if (smem > 48 * 1024) RX_CHECK_CUDA(h, cudaFuncSetAttribute(k_sams_step, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_sams_step<<<1, SAMS_THREADS, smem, h->stream>>>(S.d_words, h->d_u, K, M, h->d_perm, s->cfg, s->d_logZ, s->d_log_pi, s->d_log_w,
-                                                      (long long *)s->d_hist, s->d_ctl, s->d_prev, iteration, update);
+                                                      s->d_hist, s->d_ctl, s->d_prev, iteration, update);
     RX_CHECK_CUDA(h, cudaGetLastError());
     (*launches)++;
     return stream_consume(h, S, (size_t)2 * K, launches);   // (one uniform per replica: known without reading the device)
@@ -210,7 +209,7 @@ int rxi_sams_step(rx_engine *h, long long iteration, int update, int *launches) 
 
 int rxi_sams_get(rx_engine *h, double *logZ, double *log_weights, int64_t *histogram, int32_t *stage, int64_t *t0, double *gamma,
                  int64_t *states, int64_t *previous_states) {
-    SamsState *s = sams_of(h);
+    const SamsState *s = h->sams.get();
     if (!s) RX_FAIL(h, RX_ERR_INVALID, "rx_sams_get: rx_sams_set must be called first");
     const int M = s->M, K = h->cfg.n_replicas;
     SamsCtl ctl;
@@ -227,12 +226,4 @@ int rxi_sams_get(rx_engine *h, double *logZ, double *log_weights, int64_t *histo
     if (gamma) *gamma = ctl.gamma;
     for (int k = 0; k < K; k++) { if (states) states[k] = a[k]; if (previous_states) previous_states[k] = b[k]; }
     return RX_OK;
-}
-
-void rxi_sams_free(rx_engine *h) {
-    SamsState *s = sams_of(h);
-    if (!s) return;
-    cudaFree(s->d_logZ); cudaFree(s->d_log_pi); cudaFree(s->d_log_w); cudaFree(s->d_hist); cudaFree(s->d_prev); cudaFree(s->d_ctl);
-    delete s;
-    h->sams = nullptr;
 }
