@@ -379,6 +379,29 @@ RX_API int rx_set_barostat(rx_engine *h, int32_t first, int32_t count, const rx_
 RX_API int rx_get_barostat(rx_engine *h, int32_t first, int32_t count, rx_barostat_state *state);
 RX_API int rx_compute_energies_at_npt(rx_engine *h, const rx_state_params *states, const double *pressure,
                                       const double *dispersion, int32_t n, double *u_out);
+/* Anisotropic barostat (OpenMM's MonteCarloAnisotropicBarostat with a common pressure on the scaled axes, atomic scaling):
+ * every 25 steps, at the same Philox draw as the isotropic attempt, rr.z picks one of the scaled axes uniformly (the
+ * floor(rr.z n_scaled / 2^32)-th set bit of scale_mask), dV = volume_scale[axis] (2 u1 - 1), and only that box edge and
+ * that coordinate of every atom are scaled, by V'/V.  Acceptance as above with the pressure of rx_set_pressures; only the
+ * scaled edge is held at twice the cutoff.  Each axis adapts its own volume_scale (start 0.01 V) after every 10 of its
+ * own attempts, by the isotropic rule.  The energy matrix is the isotropic one.
+ *
+ * rx_set_anisotropic_barostat  switches an NPT engine's owned replicas to the anisotropic barostat: scale_mask bit d (x, y, z
+ *                   = 1, 2, 4) marks a scaled axis; every replica gets a fresh per-axis state (0.01 V of the rx_config box).
+ *                   RX_ERR_INVALID for a mask of 0 or above 7, or an engine without pressure.  rx_set_pressures returns
+ *                   the engine to the isotropic barostat.
+ * rx_set_barostat_anisotropic / rx_get_barostat_anisotropic  the per-axis state of replicas [first, first + count)
+ *                   (checkpoints); `step` is the counter rx_get_barostat reports, which both calls share. */
+typedef struct {
+    double volume_scale[3];    /* nm^3, per axis x, y, z */
+    int32_t n_attempted[3];    /* per axis, since that axis's last adaptation */
+    int32_t n_accepted[3];
+    int32_t step;              /* steps since the last attempt (rx_barostat_state.step) */
+    int32_t scale_mask;        /* bit d: axis d is scaled */
+} rx_anisotropic_barostat_state;
+RX_API int rx_set_anisotropic_barostat(rx_engine *h, int32_t scale_mask);
+RX_API int rx_set_barostat_anisotropic(rx_engine *h, int32_t first, int32_t count, const rx_anisotropic_barostat_state *state);
+RX_API int rx_get_barostat_anisotropic(rx_engine *h, int32_t first, int32_t count, rx_anisotropic_barostat_state *state);
 /* rx_compute_energies_at (pressure = dispersion = NULL) or rx_compute_energies_at_npt with the second alchemical region's
  * lambda_sterics [n] of those states (rx_set_alchemical_regions, rx_set_states_region2). */
 RX_API int rx_compute_energies_at_region2(rx_engine *h, const rx_state_params *states, const double *lambda_sterics_2,

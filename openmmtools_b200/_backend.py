@@ -124,8 +124,9 @@ def check_compatible(thermodynamic_states):
     h0 = thermodynamic_states[0]._standard_system_hash
     sys0 = thermodynamic_states[0]._standard_system
     npt = thermodynamic_states[0].pressure is not None
+    scale = barostat_scale(thermodynamic_states)
     for s in thermodynamic_states[1:]:
-        if (s.pressure is not None) != npt:
+        if (s.pressure is not None) != npt or getattr(s, '_barostat_scale', None) != scale:
             from .states import ThermodynamicsError
             raise ThermodynamicsError(ThermodynamicsError.INCOMPATIBLE_ENSEMBLE)
         if s._standard_system_hash != h0:
@@ -136,6 +137,11 @@ def check_compatible(thermodynamic_states):
                     'all thermodynamic states must share one system (differing only in temperature, lambdas or '
                     'harmonic-oscillator parameters): the engine keeps one resident parameter set')
     return sys0
+
+
+def barostat_scale(thermodynamic_states):
+    """The scaled axes (x, y, z) of the states' anisotropic barostat, or None (isotropic or NVT)."""
+    return getattr(thermodynamic_states[0], '_barostat_scale', None)
 
 
 def engine_tables(thermodynamic_states):
@@ -248,6 +254,8 @@ def build_engine(thermodynamic_states, n_replicas, device=0, rank=0, world_size=
     eng.set_states(**tab)
     if npt is not None:
         eng.set_pressures(*npt)
+        if barostat_scale(thermodynamic_states) is not None:
+            eng.set_anisotropic_barostat(barostat_scale(thermodynamic_states))
     return eng
 
 

@@ -29,6 +29,13 @@ def _c64(a, shape=None):
     return a
 
 
+def scale_mask(scale):
+    """(scale_x, scale_y, scale_z) flags -> the barostat's axis mask (bit d: axis d is scaled)."""
+    if len(scale) != 3:
+        raise ValueError('scale needs three flags (x, y, z), got %r' % (scale,))
+    return sum(1 << d for d, f in enumerate(scale) if f)
+
+
 class Engine:
     def __init__(self, system_kind, n_replicas, n_states, n_atoms=0, device=0, rank=0, world_size=1,
                  box=(1.0, 1.0, 1.0), r_cutoff=0.0, r_switch=0.0, use_switch=False, annihilate_sterics=False,
@@ -252,6 +259,36 @@ class Engine:
             for f in self._BARO_FIELDS[1:]:
                 setattr(arr[i], f, int(state[f][i]))
         self._check(self._lib.rx_set_barostat(self._h, first, count, C.cast(arr, C.c_void_p)))
+
+    def set_anisotropic_barostat(self, scale):
+        """Switch the NPT engine to the anisotropic barostat: scale = (scale_x, scale_y, scale_z) flags, at least one set.
+        Every owned replica gets a fresh per-axis state (rx_set_anisotropic_barostat)."""
+        self._check(self._lib.rx_set_anisotropic_barostat(self._h, scale_mask(scale)))
+
+    _ANISO_FIELDS = ('volume_scale', 'n_attempted', 'n_accepted')
+
+    def get_barostat_anisotropic(self, first=None, count=None):
+        """Per-axis barostat state of replicas [first, first + count): dict of volume_scale, n_attempted, n_accepted
+        (count, 3), step and scale_mask (count,)."""
+        first = self.k0 if first is None else first
+        count = (self.k1 - first) if count is None else count
+        arr = (_lib.RxAnisotropicBarostatState * max(count, 1))()
+        self._check(self._lib.rx_get_barostat_anisotropic(self._h, first, count, C.cast(arr, C.c_void_p)))
+        out = {f: np.array([list(getattr(arr[i], f)) for i in range(count)], np.float64 if f == 'volume_scale' else np.int64)
+               .reshape(count, 3) for f in self._ANISO_FIELDS}
+        for f in ('step', 'scale_mask'):
+            out[f] = np.array([getattr(arr[i], f) for i in range(count)], np.int64)
+        return out
+
+    def set_barostat_anisotropic(self, state, first=0):
+        count = len(state['volume_scale'])
+        arr = (_lib.RxAnisotropicBarostatState * max(count, 1))()
+        for i in range(count):
+            arr[i].volume_scale[:] = [float(v) for v in state['volume_scale'][i]]
+            for f in self._ANISO_FIELDS[1:]:
+                getattr(arr[i], f)[:] = [int(v) for v in state[f][i]]
+            arr[i].step, arr[i].scale_mask = int(state['step'][i]), int(state['scale_mask'][i])
+        self._check(self._lib.rx_set_barostat_anisotropic(self._h, first, count, C.cast(arr, C.c_void_p)))
 
     # -- replica state
     def set_positions(self, xyz, first=0):

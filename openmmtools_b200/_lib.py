@@ -25,6 +25,7 @@ SYMBOLS = [
     'rx_set_pressures', 'rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat', 'rx_compute_energies_at_npt',
     'rx_set_alchemical_regions', 'rx_set_states_region2', 'rx_compute_energies_at_region2',
     'rx_set_mc_subsets', 'rx_set_state_mc_moves', 'rx_get_mc_statistics', 'rx_set_mc_statistics', 'rx_get_mc_energy_changes',
+    'rx_set_anisotropic_barostat', 'rx_set_barostat_anisotropic', 'rx_get_barostat_anisotropic',
 ]
 RX_MAX_MC_MOVES = 4
 RX_MC_DISPLACEMENT, RX_MC_ROTATION = 0, 1
@@ -64,6 +65,11 @@ class RxPropagatePlan(C.Structure):
 class RxBarostatState(C.Structure):
     _fields_ = [('volume_scale', C.c_double), ('step', C.c_int32), ('n_attempted', C.c_int32), ('n_accepted', C.c_int32),
                 ('reserved', C.c_int32)]
+
+
+class RxAnisotropicBarostatState(C.Structure):
+    _fields_ = [('volume_scale', C.c_double * 3), ('n_attempted', C.c_int32 * 3), ('n_accepted', C.c_int32 * 3),
+                ('step', C.c_int32), ('scale_mask', C.c_int32)]
 
 
 class RxMolecule(C.Structure):
@@ -155,7 +161,9 @@ def load():
     lib.rx_get_mc_statistics.argtypes = [vp, vp, vp]
     lib.rx_set_mc_statistics.argtypes = [vp, vp, vp]
     lib.rx_get_mc_energy_changes.argtypes = [vp, vp]
-    for name in ('rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat'):
+    lib.rx_set_anisotropic_barostat.argtypes = [vp, i32]
+    for name in ('rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat', 'rx_set_barostat_anisotropic',
+                 'rx_get_barostat_anisotropic'):
         getattr(lib, name).argtypes = [vp, i32, i32, vp]
     if lib.rx_abi_version() != RX_ABI_VERSION:
         raise ImportError('librx_b200.so ABI version mismatch')

@@ -548,7 +548,32 @@ extern "C" int rx_set_pressures(rx_engine *h, const double *pressure, const doub
     RX_CHECK_CUDA(h, cudaMemcpy(h->d_box, b.data(), sizeof(double4) * n, cudaMemcpyHostToDevice));
     RX_CHECK_CUDA(h, cudaMemcpy(h->d_baro, s.data(), sizeof(rx_barostat_state) * n, cudaMemcpyHostToDevice));
     h->npt = true;
+    h->aniso = false;
     h->have_snapshot = false;   // (a snapshot without boxes cannot restore an NPT replica)
+    return RX_OK;
+}
+
+extern "C" int rx_set_anisotropic_barostat(rx_engine *h, int32_t scale_mask) {
+    ENTER(h);
+    if (!h->npt) RX_FAIL(h, RX_ERR_INVALID, "rx_set_anisotropic_barostat: the engine has no pressure (rx_set_pressures)");
+    if (scale_mask < 1 || scale_mask > 7) RX_FAIL(h, RX_ERR_INVALID, "rx_set_anisotropic_barostat: scale_mask must be 1..7");
+    const int n = h->kloc > 0 ? h->kloc : 1;
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (!h->d_aniso) {   // taken by the engine once both exist
+        DevBuf<rx_anisotropic_barostat_state> d_aniso, d_aniso_snap;
+        RX_CHECK_CUDA(h, d_aniso.alloc(n));
+        RX_CHECK_CUDA(h, d_aniso_snap.alloc(n));
+        h->d_aniso = std::move(d_aniso); h->d_aniso_snap = std::move(d_aniso_snap);
+    }
+    const double *L = h->cfg.box;
+    rx_anisotropic_barostat_state s0;
+    memset(&s0, 0, sizeof(s0));
+    for (int d = 0; d < 3; d++) s0.volume_scale[d] = 0.01 * L[0] * L[1] * L[2];   // MonteCarloAnisotropicBarostat's start
+    s0.scale_mask = scale_mask;
+    std::vector<rx_anisotropic_barostat_state> s(n, s0);
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_aniso, s.data(), sizeof(rx_anisotropic_barostat_state) * n, cudaMemcpyHostToDevice));
+    h->aniso = true;
+    h->have_snapshot = false;   // (a snapshot without the per-axis state cannot restore the replica)
     return RX_OK;
 }
 
@@ -602,6 +627,40 @@ extern "C" int rx_get_barostat(rx_engine *h, int32_t first, int32_t count, rx_ba
     ENTER(h);
     if (!state || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_get_barostat: bad arguments");
     return replica_rows(h, h->d_baro.get(), first, count, state, false, "rx_get_barostat");
+}
+// The per-axis rows live in d_aniso; their step is the counter of d_baro, which the kernel advances.
+extern "C" int rx_set_barostat_anisotropic(rx_engine *h, int32_t first, int32_t count, const rx_anisotropic_barostat_state *state) {
+    ENTER(h);
+    if (!state || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_set_barostat_anisotropic: bad arguments");
+    if (!h->aniso) RX_FAIL(h, RX_ERR_INVALID, "rx_set_barostat_anisotropic: the engine has no anisotropic barostat");
+    for (int i = 0; i < count; i++) {
+        bool ok = state[i].step >= 0 && state[i].scale_mask >= 1 && state[i].scale_mask <= 7;
+        for (int d = 0; d < 3; d++)
+            ok = ok && state[i].volume_scale[d] > 0 && state[i].n_attempted[d] >= 0 && state[i].n_accepted[d] >= 0;
+        if (!ok) RX_FAIL(h, RX_ERR_INVALID, "rx_set_barostat_anisotropic: need volume_scale > 0, non-negative counters and a mask of 1..7");
+    }
+    std::vector<rx_barostat_state> b((size_t)count);
+    int rc = replica_rows(h, h->d_baro.get(), first, count, b.data(), false, "rx_set_barostat_anisotropic");
+    if (rc) return rc;
+    for (int i = 0; i < count; i++) b[i].step = state[i].step;
+    rc = replica_rows(h, h->d_aniso.get(), first, count, const_cast<rx_anisotropic_barostat_state *>(state), true,
+                      "rx_set_barostat_anisotropic");
+    if (rc) return rc;
+    return replica_rows(h, h->d_baro.get(), first, count, b.data(), true, "rx_set_barostat_anisotropic");
+}
+extern "C" int rx_get_barostat_anisotropic(rx_engine *h, int32_t first, int32_t count, rx_anisotropic_barostat_state *state) {
+    ENTER(h);
+    if (!state || count < 0) RX_FAIL(h, RX_ERR_INVALID, "rx_get_barostat_anisotropic: bad arguments");
+    if (!h->aniso) RX_FAIL(h, RX_ERR_INVALID, "rx_get_barostat_anisotropic: the engine has no anisotropic barostat");
+    std::vector<rx_barostat_state> b((size_t)count);
+    int rc = replica_rows(h, h->d_baro.get(), first, count, b.data(), false, "rx_get_barostat_anisotropic");
+    if (rc) return rc;
+    rc = replica_rows(h, h->d_aniso.get(), first, count, state, false, "rx_get_barostat_anisotropic");
+    if (rc) return rc;
+    int lo, n, skip;
+    local_range(h, first, count, &lo, &n, &skip);
+    for (int i = skip; i < skip + n; i++) state[i].step = b[i].step;
+    return RX_OK;
 }
 
 bool rxi_is_pinned(const rx_engine *h, const void *p, size_t bytes) {

@@ -265,7 +265,8 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
 // COMPACT: the layout above 1024 atoms (DESIGN 4.2): position buffers strided by N instead of RX_MAX_ATOMS and 8-byte
 // parameter records (sqrt_eps, alch) -- sigma rides in the position's w -- so that 4096 atoms leave room for a list.
 // NPT: the box is the replica's (box[r], kept in f64 there) and a Monte Carlo barostat attempt opens every 25th step
-// (rx_b200.h, rx_set_pressures); npt[state] = (pressure, dispersion coefficient), min_edge = twice the cutoff.
+// (rx_b200.h, rx_set_pressures); npt[state] = (pressure, dispersion coefficient), min_edge = twice the cutoff.  aniso (NPT
+// only; nullptr: isotropic) is the per-axis state of rx_set_anisotropic_barostat, read and written inside an attempt only.
 // REG: two alchemical regions (rx_set_alchemical_regions): the parameter records carry each atom's region id instead of the
 // alchemical flag and the pair rule is region_pair's.
 template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false, bool NPT = false, bool REG = false>
@@ -277,7 +278,7 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
                                                     int *__restrict__ nan_flag, const int *__restrict__ only,
                                                     const MoveDev *__restrict__ moves, double4 *__restrict__ box,
                                                     rx_barostat_state *__restrict__ baro, const double2 *__restrict__ npt,
-                                                    double min_edge) {
+                                                    double min_edge, rx_anisotropic_barostat_state *__restrict__ aniso) {
     extern __shared__ float4 s_dyn[];
     // (the whole cluster takes this exit together: `only` is indexed by replica)
     if (only && !only[k0 + blockIdx.x / CL]) return;   // a retry launch propagates the replicas that failed, nothing else
@@ -542,14 +543,33 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
             const long long U0 = energy_sum(e0, fine0);
             const uint4 rr = philox4x32_10(make_uint4(n_baro++, 0xA0000000u, k, iteration), key);
             const double u1 = ((double)rr.x + 0.5) * 2.3283064365386963e-10, u2 = ((double)rr.y + 0.5) * 2.3283064365386963e-10;
-            const double V = bx * by * bz, dV = bs.volume_scale * (2.0 * u1 - 1.0), V1 = V + dV;
-            const double sc = V1 > 0.0 ? cbrt(V1 / V) : 0.0;
-            bs.n_attempted++;
-            if (fine0 && bx * sc >= min_edge && by * sc >= min_edge && bz * sc >= min_edge) {
+            const double V = bx * by * bz;
+            // the proposal: dV, and the factor s of the scaled edges and coordinates -- (V'/V)^(1/3) on all three, or V'/V
+            // on `axis` alone (anisotropic: the floor(rr.z n / 2^32)-th of the n scaled axes; only its edge is checked)
+            double dV, V1, s;
+            int axis = -1;
+            if (aniso) {
+                const int mask = aniso[r].scale_mask;
+                int pick = (int)(((unsigned long long)rr.z * (unsigned)__popc(mask)) >> 32);
+                for (int d = 0; d < 3; d++)
+                    if (((mask >> d) & 1) && pick-- == 0) axis = d;
+                dV = aniso[r].volume_scale[axis] * (2.0 * u1 - 1.0);
+                V1 = V + dV;
+                s = V1 / V;
+            } else {
+                dV = bs.volume_scale * (2.0 * u1 - 1.0);
+                V1 = V + dV;
+                s = V1 > 0.0 ? cbrt(V1 / V) : 0.0;
+                bs.n_attempted++;
+            }
+            auto f = [&](int d) { return axis < 0 || axis == d ? s : 1.0; };   // (an unscaled edge: times 1.0, exact)
+            const bool edges_ok = axis < 0 ? bx * s >= min_edge && by * s >= min_edge && bz * s >= min_edge
+                                           : (axis == 0 ? bx : axis == 1 ? by : bz) * s >= min_edge;
+            bool accepted = false;
+            if (fine0 && edges_ok) {
                 const int c_old = cur;   // the buffer holding the unscaled positions of every atom
-                const float sf = (float)sc;
-                x *= sf; y *= sf; z *= sf;
-                set_box(bx * sc, by * sc, bz * sc);
+                x *= (float)f(0); y *= (float)f(1); z *= (float)f(2);
+                set_box(bx * f(0), by * f(1), bz * f(2));
                 have_list = false;       // the list is rebuilt for the scaled box (and again after a rejection)
                 f_valid = false;
                 float e1;
@@ -561,8 +581,9 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
                 const double w = (double)(U1 - U0) * (1.0 / 16777216.0) + nst.y * (1.0 / V1 - 1.0 / V) + nst.x * dV -
                                  (double)p.N * kT * log(V1 / V);
                 if (fine1 && (w <= 0.0 || u2 < exp(-w / kT))) {
-                    bx *= sc; by *= sc; bz *= sc;
-                    bs.n_accepted++;
+                    bx *= f(0); by *= f(1); bz *= f(2);
+                    accepted = true;
+                    if (!aniso) bs.n_accepted++;
                 } else {
                     // the thread's atom may have changed in the rebuild: its unscaled position comes from the old buffer
                     if (active) { const float4 o = (s_dyn + (c_old ? pos1 : 0))[a]; x = o.x; y = o.y; z = o.z; }
@@ -571,7 +592,18 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
                     f_valid = false;
                 }
             }
-            if (bs.n_attempted >= 10) {
+            if (aniso) {   // the axis's own counters and scale, by the isotropic rule
+                int na = aniso[r].n_attempted[axis] + 1, nc = aniso[r].n_accepted[axis] + (accepted ? 1 : 0);
+                double vs = aniso[r].volume_scale[axis];
+                if (na >= 10) {
+                    if (nc < 0.25 * na) { vs /= 1.1; na = nc = 0; }
+                    else if (nc > 0.75 * na) { vs = fmin(vs * 1.1, 0.3 * V); na = nc = 0; }
+                }
+                cluster_sync();   // every thread of the cluster has read the row before it changes
+                if (q == 0 && t == 0) {
+                    aniso[r].volume_scale[axis] = vs; aniso[r].n_attempted[axis] = na; aniso[r].n_accepted[axis] = nc;
+                }
+            } else if (bs.n_attempted >= 10) {
                 if (bs.n_accepted < 0.25 * bs.n_attempted) { bs.volume_scale /= 1.1; bs.n_attempted = bs.n_accepted = 0; }
                 else if (bs.n_accepted > 0.75 * bs.n_attempted) {
                     bs.volume_scale = fmin(bs.volume_scale * 1.1, 0.3 * V);
@@ -1180,7 +1212,7 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
                                              (const float4 *)h->d_atom, (const StateDev *)h->d_states, (const int *)h->d_perm,
                                              h->d_pos.get(), h->d_vel.get(), h->k0, key, it32, h->d_pot.get(), h->d_kin.get(),
                                              h->d_nan.get(), d_only, (const MoveDev *)h->d_moves, h->d_box.get(), h->d_baro.get(),
-                                             (const double2 *)h->d_npt, min_edge);
+                                             (const double2 *)h->d_npt, min_edge, h->aniso ? h->d_aniso.get() : nullptr);
                     });
                 });
             });
@@ -1211,18 +1243,23 @@ int rxi_snapshot_state(rx_engine *h) {
     if (h->npt) {
         RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_box_snap, h->d_box, sizeof(double4) * h->kloc, cudaMemcpyDeviceToDevice, h->stream));
         RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_baro_snap, h->d_baro, sizeof(rx_barostat_state) * h->kloc, cudaMemcpyDeviceToDevice, h->stream));
+        if (h->aniso)
+            RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_aniso_snap, h->d_aniso, sizeof(rx_anisotropic_barostat_state) * h->kloc,
+                                             cudaMemcpyDeviceToDevice, h->stream));
     }
     h->have_snapshot = true;
     return RX_OK;
 }
 
 // retry[k] = the NaN flag of replica k; a failed replica's rows of positions and velocities (`words` 8-byte words each)
-// and, under NPT (box != nullptr), its box and barostat state go back to the snapshot.
+// and, under NPT (box != nullptr), its box and barostat state (and per-axis state, aniso != nullptr) go back to the snapshot.
 __global__ void k_restore_failed(const int *__restrict__ nan_flag, int *__restrict__ retry, int k0, int words,
                                  const unsigned long long *__restrict__ pos_snap, const unsigned long long *__restrict__ vel_snap,
                                  unsigned long long *__restrict__ pos, unsigned long long *__restrict__ vel,
                                  const double4 *__restrict__ box_snap, const rx_barostat_state *__restrict__ baro_snap,
-                                 double4 *__restrict__ box, rx_barostat_state *__restrict__ baro) {
+                                 double4 *__restrict__ box, rx_barostat_state *__restrict__ baro,
+                                 const rx_anisotropic_barostat_state *__restrict__ aniso_snap,
+                                 rx_anisotropic_barostat_state *__restrict__ aniso) {
     const int r = blockIdx.x, k = k0 + r;
     const int failed = nan_flag[k];
     if (threadIdx.x == 0) retry[k] = failed;
@@ -1232,6 +1269,7 @@ __global__ void k_restore_failed(const int *__restrict__ nan_flag, int *__restri
         vel[(size_t)r * words + q] = vel_snap[(size_t)r * words + q];
     }
     if (box && threadIdx.x == 0) { box[r] = box_snap[r]; baro[r] = baro_snap[r]; }
+    if (aniso && threadIdx.x == 0) aniso[r] = aniso_snap[r];
 }
 
 int rxi_restore_failed(rx_engine *h) {
@@ -1242,7 +1280,8 @@ int rxi_restore_failed(rx_engine *h) {
     using W = unsigned long long;
     k_restore_failed<<<h->kloc, 256, 0, h->stream>>>(h->d_nan, h->d_retry, h->k0, words, (const W *)h->d_pos_snap.get(),
                                                     (const W *)h->d_vel_snap.get(), (W *)h->d_pos.get(), (W *)h->d_vel.get(), h->d_box_snap,
-                                                    h->d_baro_snap, h->npt ? h->d_box.get() : nullptr, h->d_baro);
+                                                    h->d_baro_snap, h->npt ? h->d_box.get() : nullptr, h->d_baro,
+                                                    h->d_aniso_snap, h->npt && h->aniso ? h->d_aniso.get() : nullptr);
     RX_CHECK_CUDA(h, cudaGetLastError());
     return RX_OK;
 }

@@ -196,6 +196,9 @@ struct rx_engine {
     DevBuf<double4> d_box, d_box_snap;
     DevBuf<rx_barostat_state> d_baro, d_baro_snap;
     DevBuf<double2> d_npt;
+    // anisotropic barostat (rx_set_anisotropic_barostat): per owned replica per-axis state; the step counter stays in d_baro
+    bool aniso = false;
+    DevBuf<rx_anisotropic_barostat_state> d_aniso, d_aniso_snap;
     // nccl
     void *nccl_lib = nullptr;
     void *nccl_comm = nullptr;

@@ -22,7 +22,7 @@ import os
 import time
 import numpy as np
 from .. import unit, mcmc, states, _backend, _lib
-from .._engine import EngineError
+from .._engine import EngineError, scale_mask
 from ..cache import ContextCache
 from .utils import SimulationNaNError
 from .multistatereporter import MultiStateReporter
@@ -232,6 +232,12 @@ class MultiStateSampler:
         if 'barostat' in extra:     # the NPT run continues with the barostat state it had at the checkpoint
             self._engine.set_barostat({k: np.asarray(v)[self._engine.k0:self._engine.k1] for k, v in extra['barostat'].items()},
                                       first=self._engine.k0)
+        if 'barostat_anisotropic' in extra:     # ... and the per-axis state of an anisotropic one
+            k0, k1 = self._engine.k0, self._engine.k1
+            a = {k: np.asarray(v)[k0:k1] for k, v in extra['barostat_anisotropic'].items()}
+            a['step'] = np.asarray(extra['barostat']['step'])[k0:k1]
+            a['scale_mask'] = np.full(k1 - k0, scale_mask(_backend.barostat_scale(self._thermodynamic_states)))
+            self._engine.set_barostat_anisotropic(a, first=k0)
         # energies of the checkpoint iteration are what the next mixing uses
         self._engine.set_energies(self._energy_thermodynamic_states)
         # put the two MT19937 streams back where they were
@@ -519,6 +525,10 @@ class MultiStateSampler:
     def _npt(self):
         return self._thermodynamic_states[0].pressure is not None
 
+    @property
+    def _anisotropic(self):
+        return self._npt and _backend.barostat_scale(self._thermodynamic_states) is not None
+
     def _upload_sampler_states(self):
         e = self._engine
         K = len(self._sampler_states)
@@ -655,6 +665,8 @@ class MultiStateSampler:
                 self._gather_sampler_states()
                 if self._npt:
                     self._last_npt_records = self._gather_npt_records()
+                if self._anisotropic:
+                    self._last_aniso_records = self._gather_aniso_records()
             if self._rank == 0:
                 self._reporter.write_sampler_states(self._sampler_states, self._iteration, extra=self._checkpoint_extra())
 
@@ -762,6 +774,11 @@ class MultiStateSampler:
             rec = self._last_npt_records if self._world_size > 1 else self._local_npt_records()
             extra['barostat'] = dict(volume_scale=rec[:, 3].tolist(),
                                      **{f: [int(q) for q in rec[:, c]] for c, f in ((4, 'step'), (5, 'n_attempted'), (6, 'n_accepted'))})
+        if self._anisotropic:
+            rec = self._last_aniso_records if self._world_size > 1 else self._local_aniso_records()
+            extra['barostat_anisotropic'] = dict(volume_scale=rec[:, 0].tolist(),
+                                                 **{f: [[int(q) for q in row] for row in rec[:, c]]
+                                                    for c, f in ((1, 'n_attempted'), (2, 'n_accepted'))})
         return extra
 
     def _report_iteration(self):
@@ -777,6 +794,7 @@ class MultiStateSampler:
             if self._world_size > 1:
                 self._gather_sampler_states()
         npt = self._last_npt_records = self._gather_npt_records() if self._npt else None
+        self._last_aniso_records = self._gather_aniso_records() if self._anisotropic else None
         if self._mc_moves:
             self._pull_mc_statistics()
         if self._rank != 0:
@@ -844,6 +862,34 @@ class MultiStateSampler:
         for part in gathered:
             for item in part:
                 out[item[0]] = item[5]
+        return out
+
+    def _local_aniso_records(self):
+        """(K_loc, 3, 3): per-axis volume_scale, n_attempted and n_accepted of the owned replicas' anisotropic barostat."""
+        e = self._engine
+        if e.k1 == e.k0:
+            return np.zeros((0, 3, 3))
+        a = e.get_barostat_anisotropic()
+        return np.stack([a['volume_scale'], a['n_attempted'], a['n_accepted']], axis=1).astype(np.float64)
+
+    def _gather_aniso_records(self):
+        """(K, 3, 3) records of every replica on rank 0 (None elsewhere), carried as the position rows of a shard;
+        every rank takes part."""
+        rec = self._local_aniso_records()
+        if self._world_size == 1:
+            return rec
+        e = self._engine
+        comm = self._communicator
+        if comm is None:
+            from .._dist import default_communicator
+            comm = self._communicator = default_communicator()
+        gathered = comm.gather_object([(k, rec[r], None, None, None) for r, k in enumerate(range(e.k0, e.k1))])
+        if self._rank != 0:
+            return None
+        out = np.zeros((self.n_replicas, 3, 3))
+        for part in gathered:
+            for item in part:
+                out[item[0]] = item[1]
         return out
 
     # ------------------------------------------------------------------ online analysis (multistatesampler.py:1625-1695)

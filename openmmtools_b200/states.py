@@ -6,14 +6,16 @@ Mirrors /root/reference/openmmtools/states.py: ``ThermodynamicState`` (:385), ``
 :class:`openmmtools_b200.system.System` parameter record, and energies are evaluated by the CUDA engine
 (``ThermodynamicState.reduced_potential`` -> ``rx_compute_energies``).  OpenMM-typed methods
 (``create_context``, ``apply_to_context`` ...) raise ``NotImplementedError``.  A pressure puts a periodic LJ system in the
-NPT ensemble with an isotropic Monte Carlo barostat that the CUDA engine runs (states.py:1741-1771); surface tensions
-and anisotropic or membrane barostats are not provided.
+NPT ensemble with an isotropic Monte Carlo barostat that the CUDA engine runs (states.py:1741-1771).  A system holding a
+``MonteCarloBarostat`` or ``MonteCarloAnisotropicBarostat`` record (openmmtools_b200.system) is NPT at that barostat's
+pressure; the anisotropic one scales one edge per attempt, chosen among its scaled axes, which must share one pressure
+(states.py:1656-1693; a z-only barostat is accepted).  Surface tensions and membrane barostats are not provided.
 """
 import copy
 import numpy as np
 from . import unit
 from .constants import kB
-from .system import System
+from .system import System, BAROSTATS, MonteCarloBarostat, MonteCarloAnisotropicBarostat
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -31,6 +33,9 @@ class ThermodynamicsError(Exception):
         INCOMPATIBLE_ENSEMBLE: 'Cannot apply to a context in a different thermodynamic ensemble.',
         UNSUPPORTED_BAROSTAT: 'NPT ensembles are outside the GPU replica-exchange hot path.',
         BAROSTATED_NONPERIODIC: 'Non-periodic systems cannot have a barostat.',
+        MULTIPLE_BAROSTATS: 'System has multiple barostats.',
+        UNSUPPORTED_ANISOTROPIC_BAROSTAT: 'MonteCarloAnisotropicBarostat is supported only if the pressure along all '
+                                          'scaled axes is the same and at least one axis is scaled.',
     }
 
     def __init__(self, code, *args):
@@ -65,6 +70,10 @@ class ThermodynamicState:
     A pressure adds what ``MonteCarloBarostat(pressure, temperature)`` adds in the reference (states.py:1761-1771): an
     isotropic Monte Carlo volume move at the state's temperature, attempted every 25 steps (OpenMM's default frequency,
     fixed here).  Only periodic systems take a pressure; surface tensions are not provided.
+
+    A system holding a barostat record makes the state NPT at that barostat's pressure unless ``pressure`` is given.  With
+    a ``MonteCarloAnisotropicBarostat`` the state keeps its scaled axes: ``pressure`` then sets the pressure of all three
+    axes, and ``pressure = None`` removes the barostat.
     """
 
     def __init__(self, system, temperature=None, pressure=None, surface_tension=None):
@@ -75,12 +84,14 @@ class ThermodynamicState:
             raise ThermodynamicsError(ThermodynamicsError.NONE_TEMPERATURE)
         if surface_tension is not None:
             raise NotImplementedError('surface tension (membrane barostats) is outside the replica-exchange hot path')
-        self._standard_system = system.copy()
-        self._standard_system_hash = self._standard_system.standard_hash()
+        baro = _read_barostat(system)
+        self._standard_system = _without_barostats(system)
+        self._barostat_scale = None if baro is None else baro[1]   # anisotropic: (scale_x, scale_y, scale_z)
+        self._rehash()
         self._temperature = None
         self._pressure = None
         self.temperature = temperature
-        self.pressure = pressure
+        self.pressure = baro[0] * unit.bar if pressure is None and baro is not None else pressure
 
     # -- system
     @property
@@ -93,11 +104,33 @@ class ThermodynamicState:
         self.set_system(value)
 
     def set_system(self, system, fix_state=False):
-        self._standard_system = system.copy()
-        self._standard_system_hash = self._standard_system.standard_hash()
+        """A system with a barostat record brings its ensemble along; one without keeps the state's."""
+        baro = _read_barostat(system)
+        self._standard_system = _without_barostats(system)
+        if baro is not None:
+            self._barostat_scale = baro[1]
+            self._rehash()
+            self.pressure = baro[0] * unit.bar
+        else:
+            self._rehash()
 
     def get_system(self, remove_thermostat=False, remove_barostat=False):
-        return self._standard_system.copy()
+        """A copy of the standard system; an anisotropic state's carries its barostat at the state's pressure."""
+        system = self._standard_system.copy()
+        if not remove_barostat and self._barostat_scale is not None and self._pressure is not None:
+            system.addForce(self._anisotropic_barostat())
+        return system
+
+    def _anisotropic_barostat(self):
+        return MonteCarloAnisotropicBarostat(self._pressure * unit.bar, self._temperature * unit.kelvin, *self._barostat_scale)
+
+    def _rehash(self):
+        """The standard system's hash; an anisotropic barostat's kind and scaled axes count, its pressure does not."""
+        system = self._standard_system
+        if self._barostat_scale is not None:
+            system = copy.copy(system)
+            system.forces = [MonteCarloAnisotropicBarostat(1.0 * unit.bar, 300.0 * unit.kelvin, *self._barostat_scale)]
+        self._standard_system_hash = system.standard_hash()
 
     # -- thermodynamic parameters
     @property
@@ -130,6 +163,9 @@ class ThermodynamicState:
     def pressure(self, value):
         if value is None:
             self._pressure = None
+            if self._barostat_scale is not None:   # the anisotropic barostat goes with its pressure
+                self._barostat_scale = None
+                self._rehash()
             return
         if not self.is_periodic:
             raise ThermodynamicsError(ThermodynamicsError.BAROSTATED_NONPERIODIC)
@@ -149,8 +185,9 @@ class ThermodynamicState:
 
     @property
     def barostat(self):
-        """None: the barostat is not an object here (the engine runs it); see ``pressure``."""
-        return None
+        """An anisotropic state's MonteCarloAnisotropicBarostat record (at the state's pressure and temperature); None
+        otherwise: the isotropic barostat is not an object here (the engine runs it), see ``pressure``."""
+        return self._anisotropic_barostat() if self._barostat_scale is not None and self._pressure is not None else None
 
     @property
     def surface_tension(self):
@@ -241,6 +278,35 @@ class ThermodynamicState:
     def __setstate__(self, d):
         self.__dict__.update(d)
         self.__dict__.setdefault('_pressure', None)
+        self.__dict__.setdefault('_barostat_scale', None)
+
+
+def _read_barostat(system):
+    """(pressure in bar, scaled axes or None when isotropic) of the system's barostat record; None without one.  Raises
+    what the reference raises for a system it cannot put in the NPT ensemble (states.py:1656-1693)."""
+    baros = [f for f in getattr(system, 'forces', ()) if isinstance(f, BAROSTATS)]
+    if not baros:
+        return None
+    if len(baros) > 1:
+        raise ThermodynamicsError(ThermodynamicsError.MULTIPLE_BAROSTATS)
+    if not system.usesPeriodicBoundaryConditions():
+        raise ThermodynamicsError(ThermodynamicsError.BAROSTATED_NONPERIODIC)
+    b = baros[0]
+    if b.getFrequency() != 25:
+        raise NotImplementedError('only barostat frequency 25 is provided, got %d' % b.getFrequency())
+    if isinstance(b, MonteCarloBarostat):
+        return b._pressure, None
+    scale = tuple(b._scale)
+    scaled = {p for p, s in zip(b._pressure, scale) if s}   # (the unscaled axes' pressures do not count)
+    if len(scaled) != 1:
+        raise ThermodynamicsError(ThermodynamicsError.UNSUPPORTED_ANISOTROPIC_BAROSTAT)
+    return scaled.pop(), scale
+
+
+def _without_barostats(system):
+    s = system.copy()
+    s.forces = []
+    return s
 
 
 # ------------------------------------------------------------------------------------------------------

@@ -12,6 +12,115 @@ import numpy as np
 LJ, HARMONIC, MOLECULE = 'lj', 'harmonic', 'molecule'
 
 
+def _bar(value, name='pressure'):
+    from . import unit
+    if not (isinstance(value, unit.Quantity) and value.unit.is_compatible(unit.bar)):
+        raise TypeError('%s must be a Quantity with units of pressure (e.g. 1.0 * unit.bar), got %r' % (name, value))
+    return value.value_in_unit(unit.bar)
+
+
+def _kelvin(value):
+    from . import unit
+    return float(unit.to_md(value, unit.kelvin, 'temperature'))
+
+
+class MonteCarloBarostat:
+    """Record of OpenMM's isotropic ``MonteCarloBarostat(defaultPressure, defaultTemperature, frequency=25)``.
+
+    ``ThermodynamicState(system, temperature)`` on a system holding it is NPT at its pressure, exactly as
+    ``ThermodynamicState(system, temperature, pressure)`` on the system without it.  The CUDA engine runs the move."""
+
+    def __init__(self, defaultPressure, defaultTemperature, frequency=25):
+        self.setDefaultPressure(defaultPressure)
+        self.setDefaultTemperature(defaultTemperature)
+        self.setFrequency(frequency)
+
+    def getDefaultPressure(self):
+        from . import unit
+        return self._pressure * unit.bar
+
+    def setDefaultPressure(self, pressure):
+        self._pressure = float(_bar(pressure))
+
+    def getDefaultTemperature(self):
+        from . import unit
+        return self._temperature * unit.kelvin
+
+    def setDefaultTemperature(self, temperature):
+        self._temperature = _kelvin(temperature)
+
+    def getFrequency(self):
+        return self._frequency
+
+    def setFrequency(self, frequency):
+        self._frequency = int(frequency)
+
+    def _hash_key(self):
+        return b'MonteCarloBarostat'
+
+
+class MonteCarloAnisotropicBarostat:
+    """Record of OpenMM's ``MonteCarloAnisotropicBarostat(defaultPressure, defaultTemperature, scaleX, scaleY, scaleZ,
+    frequency=25)``: each attempt scales one box edge, chosen among the scaled axes.  ``defaultPressure`` is a pressure
+    per axis (x, y, z), or one pressure for all three."""
+
+    def __init__(self, defaultPressure, defaultTemperature, scaleX=True, scaleY=True, scaleZ=True, frequency=25):
+        self.setDefaultPressure(defaultPressure)
+        self.setDefaultTemperature(defaultTemperature)
+        self._scale = [bool(scaleX), bool(scaleY), bool(scaleZ)]
+        self.setFrequency(frequency)
+
+    def getDefaultPressure(self):
+        from . import unit
+        return unit.Quantity(np.array(self._pressure), unit.bar)
+
+    def setDefaultPressure(self, pressure):
+        from . import unit
+        if isinstance(pressure, (list, tuple)) and len(pressure) == 3 and all(isinstance(p, unit.Quantity) for p in pressure):
+            p = [_bar(q) for q in pressure]
+        else:
+            p = _bar(pressure)
+        p = np.broadcast_to(np.asarray(p, np.float64), (3,))
+        self._pressure = tuple(float(v) for v in p)
+
+    def getDefaultTemperature(self):
+        from . import unit
+        return self._temperature * unit.kelvin
+
+    def setDefaultTemperature(self, temperature):
+        self._temperature = _kelvin(temperature)
+
+    def getScaleX(self):
+        return self._scale[0]
+
+    def getScaleY(self):
+        return self._scale[1]
+
+    def getScaleZ(self):
+        return self._scale[2]
+
+    def setScaleX(self, scale):
+        self._scale[0] = bool(scale)
+
+    def setScaleY(self, scale):
+        self._scale[1] = bool(scale)
+
+    def setScaleZ(self, scale):
+        self._scale[2] = bool(scale)
+
+    def getFrequency(self):
+        return self._frequency
+
+    def setFrequency(self, frequency):
+        self._frequency = int(frequency)
+
+    def _hash_key(self):
+        return b'MonteCarloAnisotropicBarostat' + repr(tuple(self._scale)).encode()
+
+
+BAROSTATS = (MonteCarloBarostat, MonteCarloAnisotropicBarostat)
+
+
 class System:
     """Parameters of one of the supported systems (md units: nm, ps, dalton, kJ/mol)."""
 
@@ -59,6 +168,8 @@ class System:
         self.gb_parameters = None  # (alpha, beta, gamma, offset, solute dielectric, solvent dielectric, sa_energy, probe radius)
         # -- OpenMM-style global parameters with their defaults (read by GlobalParameterState.from_system)
         self.global_parameters = {}
+        # -- forces added with addForce: barostat records only (the other forces are the parameters above)
+        self.forces = []
 
     # -- OpenMM-flavoured accessors used by user code on this path
     def getNumParticles(self):
@@ -75,6 +186,25 @@ class System:
     def setDefaultPeriodicBoxVectors(self, a, b, c):
         from . import unit
         self.box_vectors = np.array([unit.to_md(a), unit.to_md(b), unit.to_md(c)], dtype=np.float64)
+
+    def addForce(self, force):
+        """Add a barostat record (MonteCarloBarostat or MonteCarloAnisotropicBarostat); returns its index."""
+        if not isinstance(force, BAROSTATS):
+            raise NotImplementedError('only barostat records can be added to a System, got %r' % type(force).__name__)
+        self.forces.append(force)
+        return len(self.forces) - 1
+
+    def getForces(self):
+        return list(self.forces)
+
+    def getNumForces(self):
+        return len(self.forces)
+
+    def getForce(self, index):
+        return self.forces[index]
+
+    def removeForce(self, index):
+        del self.forces[index]
 
     def usesPeriodicBoundaryConditions(self):
         return self.kind == LJ
@@ -138,6 +268,8 @@ class System:
                 for a in (self.gb_radius, self.gb_scale):
                     h.update(np.asarray(a, dtype=np.float64).tobytes())
                 h.update(repr(tuple(float(v) for v in self.gb_parameters)).encode())
+        for f in getattr(self, 'forces', ()):   # a barostat's kind and scaled axes, not its pressure (systems without keep their hash)
+            h.update(f._hash_key())
         return h.hexdigest()
 
     def __getstate__(self):
@@ -146,3 +278,4 @@ class System:
     def __setstate__(self, d):
         self.__dict__.update(d)
         self.__dict__.setdefault('alchemical_regions', None)
+        self.__dict__.setdefault('forces', [])
