@@ -168,6 +168,28 @@ RX_API int rx_set_integrator(rx_engine *h, double timestep, double collision_rat
 RX_API int rx_set_state_integrator(rx_engine *h, int32_t state, double timestep, double collision_rate, int32_t n_steps,
                                    const char *splitting, int32_t reassign_velocities);
 
+/* ---- hybrid Monte Carlo (HMCMove, mcmc.py:1493-1594 -> HMCIntegrator, integrators.py:885-1012) -------------------------
+ * rx_set_hmc_integrator makes the move of every state HMC, in place of rx_set_integrator (which returns to Langevin).  One
+ * rx_propagate is n_steps trials of n_steps velocity-Verlet steps each (BaseIntegratorMove.apply calls step(n_steps) and
+ * HMCIntegrator(nsteps=n_steps) makes one step a whole trial): n_steps^2 force evaluations.  A trial draws v = sqrt(kT/m) g,
+ * takes Eold = KE + U, runs the steps, takes Enew and keeps the new positions iff u <= exp(-(Enew - Eold)/kT); otherwise the
+ * positions go back to the trial's start (NaN where they were not finite) and the velocities stay as the trajectory left
+ * them.  LJ and harmonic engines sum the energies in fixed point (2^-24 kJ/mol, every per-atom term below 2^26 kJ/mol in
+ * magnitude; a trial with a term outside that range is rejected); a molecule's are f64, and its trials constrain the drawn
+ * velocities and every step's positions and velocities as the reference's program does (SHAKE / RATTLE).  Randoms:
+ * Philox4x32-10 keyed as rx_propagate's noise, counter (atom, 0x90000000 + trial, replica, iteration) for the velocities and
+ * (trial, 0xB0000000, replica, iteration) for u.  RX_ERR_UNSUPPORTED at constant pressure and at a launch whose states mix
+ * HMC and Langevin moves (and, as for Langevin moves, per-state moves on a molecule).
+ * rx_set_state_hmc_integrator  the HMC move of one state (after rx_set_hmc_integrator), as rx_set_state_integrator.
+ * rx_get_hmc_statistics / rx_set_hmc_statistics  accepted and attempted trials [K] of the replicas this engine owns
+ *                        (cumulative; a propagation that ends in NaN is not counted; other entries: 0 / ignored).
+ * rx_get_hmc_energies    (Eold, Enew) [K] in kJ/mol of the last trial of every owned replica (NaN: none, or not owned). */
+RX_API int rx_set_hmc_integrator(rx_engine *h, double timestep, int32_t n_steps);
+RX_API int rx_set_state_hmc_integrator(rx_engine *h, int32_t state, double timestep, int32_t n_steps);
+RX_API int rx_get_hmc_statistics(rx_engine *h, int64_t *accepted, int64_t *trials);
+RX_API int rx_set_hmc_statistics(rx_engine *h, const int64_t *accepted, const int64_t *trials);
+RX_API int rx_get_hmc_energies(rx_engine *h, double *e_old, double *e_new);
+
 /* ---- Monte Carlo rigid-body moves (MCDisplacementMove, MCRotationMove: mcmc.py:810-970, 1704-1911) ------------------ */
 /* Up to RX_MAX_MC_MOVES Metropolized moves per thermodynamic state, applied in order to every replica in that state at the
  * start of rx_propagate (before its snapshot, so rx_propagate_retry reruns the dynamics only, from the post-MC state) and of

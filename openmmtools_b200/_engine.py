@@ -178,6 +178,34 @@ class Engine:
         self._check(self._lib.rx_set_state_integrator(self._h, int(state), float(timestep), float(collision_rate), int(n_steps),
                                                       splitting.replace(' ', '').encode(), int(bool(reassign_velocities))))
 
+    # -- hybrid Monte Carlo (rx_set_hmc_integrator)
+    def set_hmc_integrator(self, timestep, n_steps):
+        """HMC for every state: each propagation is n_steps trials of n_steps velocity-Verlet steps of `timestep` ps."""
+        self._check(self._lib.rx_set_hmc_integrator(self._h, float(timestep), int(n_steps)))
+
+    def set_state_hmc_integrator(self, state, timestep, n_steps):
+        """The HMC move of one thermodynamic state (after set_hmc_integrator)."""
+        self._check(self._lib.rx_set_state_hmc_integrator(self._h, int(state), float(timestep), int(n_steps)))
+
+    def get_hmc_statistics(self):
+        """(accepted, trials) int64 [K] of the HMC trials of the replicas this engine owns (zero elsewhere), cumulative over
+        the engine's life.  Diagnostics only: the reference's HMCMove keeps no statistics, so a sampler's storage does not
+        save them and a sampler resumed from storage starts them at zero (set_hmc_statistics can put counts back)."""
+        acc = np.zeros(self.K, np.int64); trials = np.zeros_like(acc)
+        self._check(self._lib.rx_get_hmc_statistics(self._h, _ptr(acc), _ptr(trials)))
+        return acc, trials
+
+    def set_hmc_statistics(self, accepted, trials):
+        acc = np.ascontiguousarray(accepted, np.int64).reshape(self.K)
+        n = np.ascontiguousarray(trials, np.int64).reshape(self.K)
+        self._check(self._lib.rx_set_hmc_statistics(self._h, _ptr(acc), _ptr(n)))
+
+    def get_hmc_energies(self):
+        """(Eold, Enew) float64 [K] in kJ/mol of every owned replica's last HMC trial (NaN: none)."""
+        e0 = np.zeros(self.K); e1 = np.zeros(self.K)
+        self._check(self._lib.rx_get_hmc_energies(self._h, _ptr(e0), _ptr(e1)))
+        return e0, e1
+
     # -- Monte Carlo moves (rx_set_mc_subsets, rx_set_state_mc_moves)
     def set_mc_moves(self, moves):
         """The Monte Carlo moves of every state: moves[l] is a list of up to RX_MAX_MC_MOVES (kind, sigma_nm, atom indices),

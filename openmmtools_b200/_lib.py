@@ -26,6 +26,8 @@ SYMBOLS = [
     'rx_set_alchemical_regions', 'rx_set_states_region2', 'rx_compute_energies_at_region2',
     'rx_set_mc_subsets', 'rx_set_state_mc_moves', 'rx_get_mc_statistics', 'rx_set_mc_statistics', 'rx_get_mc_energy_changes',
     'rx_set_anisotropic_barostat', 'rx_set_barostat_anisotropic', 'rx_get_barostat_anisotropic',
+    'rx_set_hmc_integrator', 'rx_set_state_hmc_integrator', 'rx_get_hmc_statistics', 'rx_set_hmc_statistics',
+    'rx_get_hmc_energies',
 ]
 RX_MAX_MC_MOVES = 4
 RX_MC_DISPLACEMENT, RX_MC_ROTATION = 0, 1
@@ -162,6 +164,10 @@ def load():
     lib.rx_set_mc_statistics.argtypes = [vp, vp, vp]
     lib.rx_get_mc_energy_changes.argtypes = [vp, vp]
     lib.rx_set_anisotropic_barostat.argtypes = [vp, i32]
+    lib.rx_set_hmc_integrator.argtypes = [vp, dbl, i32]
+    lib.rx_set_state_hmc_integrator.argtypes = [vp, i32, dbl, i32]
+    for name in ('rx_get_hmc_statistics', 'rx_set_hmc_statistics', 'rx_get_hmc_energies'):
+        getattr(lib, name).argtypes = [vp, vp, vp]
     for name in ('rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat', 'rx_set_barostat_anisotropic',
                  'rx_get_barostat_anisotropic'):
         getattr(lib, name).argtypes = [vp, i32, i32, vp]

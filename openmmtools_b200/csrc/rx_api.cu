@@ -302,7 +302,109 @@ extern "C" int rx_set_integrator(rx_engine *h, double timestep, double collision
     memset(h->program, 0, sizeof(h->program));
     memcpy(h->program, splitting, n);
     h->have_integrator = true;
+    h->hmc = false;
     h->state_moves.clear();   // one move for every state again
+    return RX_OK;
+}
+
+// The HMC counters and last-trial energies of the owned replicas, allocated (zero) by the first HMC setter.
+static int hmc_buffers(rx_engine *h) {
+    if (h->d_hmc_stats) return RX_OK;
+    const size_t n = (size_t)(h->kloc > 0 ? h->kloc : 1);
+    DevBuf<ulonglong2> stats;
+    DevBuf<double2> energy;
+    RX_CHECK_CUDA(h, stats.alloc(n));
+    RX_CHECK_CUDA(h, energy.alloc(n));
+    RX_CHECK_CUDA(h, cudaMemset(stats, 0, sizeof(ulonglong2) * n));
+    RX_CHECK_CUDA(h, cudaMemset(energy, 0xff, sizeof(double2) * n));   // (NaN: no trial yet)
+    h->d_hmc_stats = std::move(stats); h->d_hmc_energy = std::move(energy);
+    return RX_OK;
+}
+
+static int hmc_check(rx_engine *h, double timestep, int32_t n_steps, const char *who) {
+    if (!(timestep > 0) || !isfinite(timestep) || n_steps < 0) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": need timestep > 0 and n_steps >= 0");
+    if (h->cfg.system_kind == RX_SYSTEM_NONE) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": engine has no particle system");
+    if (h->npt) RX_FAIL(h, RX_ERR_UNSUPPORTED, std::string(who) + ": hybrid Monte Carlo at constant pressure is not provided");
+    return hmc_buffers(h);
+}
+
+extern "C" int rx_set_hmc_integrator(rx_engine *h, double timestep, int32_t n_steps) {
+    ENTER(h);
+    int rc = hmc_check(h, timestep, n_steps, "rx_set_hmc_integrator");
+    if (rc) return rc;
+    h->dt = timestep; h->gamma = 0.0; h->n_steps = n_steps;
+    memset(h->program, 0, sizeof(h->program));
+    memcpy(h->program, "VRV", 3);
+    h->have_integrator = true;
+    h->hmc = true;
+    h->state_moves.clear();
+    return RX_OK;
+}
+
+extern "C" int rx_set_state_hmc_integrator(rx_engine *h, int32_t state, double timestep, int32_t n_steps) {
+    ENTER(h);
+    if (!h->have_integrator || !h->hmc) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_hmc_integrator: rx_set_hmc_integrator must be called first");
+    if (state < 0 || state >= h->cfg.n_states) RX_FAIL(h, RX_ERR_INVALID, "rx_set_state_hmc_integrator: state out of range");
+    int rc = hmc_check(h, timestep, n_steps, "rx_set_state_hmc_integrator");
+    if (rc) return rc;
+    if (h->state_moves.empty()) {   // start from the common move
+        h->state_moves.resize((size_t)h->cfg.n_states);
+        for (auto &m : h->state_moves) {
+            m.dt = h->dt; m.gamma = 0.0; m.n_steps = h->n_steps; m.reassign = 0; m.hmc = true;
+            memcpy(m.program, h->program, sizeof(m.program));
+        }
+    }
+    rx_state_move &m = h->state_moves[(size_t)state];
+    m.dt = timestep; m.gamma = 0.0; m.n_steps = n_steps; m.reassign = 0; m.set = true; m.hmc = true;
+    memset(m.program, 0, sizeof(m.program));
+    memcpy(m.program, "VRV", 3);
+    h->state_moves_dirty = true;
+    return RX_OK;
+}
+
+// Per owned replica: [k0, k0 + kloc) of the [K] arrays; the other entries are left alone.
+extern "C" int rx_get_hmc_statistics(rx_engine *h, int64_t *accepted, int64_t *trials) {
+    ENTER(h);
+    if (!accepted || !trials) RX_FAIL(h, RX_ERR_INVALID, "rx_get_hmc_statistics: null argument");
+    const int K = h->cfg.n_replicas;
+    for (int k = 0; k < K; k++) if (k < h->k0 || k >= h->k0 + h->kloc) accepted[k] = trials[k] = 0;
+    if (!h->d_hmc_stats || h->kloc == 0) {
+        for (int k = h->k0; k < h->k0 + h->kloc; k++) accepted[k] = trials[k] = 0;
+        return RX_OK;
+    }
+    std::vector<ulonglong2> c((size_t)h->kloc);
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpy(c.data(), h->d_hmc_stats, sizeof(ulonglong2) * h->kloc, cudaMemcpyDeviceToHost));
+    for (int r = 0; r < h->kloc; r++) { accepted[h->k0 + r] = (int64_t)c[r].x; trials[h->k0 + r] = (int64_t)c[r].y; }
+    return RX_OK;
+}
+
+extern "C" int rx_set_hmc_statistics(rx_engine *h, const int64_t *accepted, const int64_t *trials) {
+    ENTER(h);
+    if (!accepted || !trials) RX_FAIL(h, RX_ERR_INVALID, "rx_set_hmc_statistics: null argument");
+    if (!h->d_hmc_stats) RX_FAIL(h, RX_ERR_INVALID, "rx_set_hmc_statistics: call rx_set_hmc_integrator first");
+    std::vector<ulonglong2> c((size_t)h->kloc);
+    for (int r = 0; r < h->kloc; r++) {
+        const int64_t a = accepted[h->k0 + r], n = trials[h->k0 + r];
+        if (a < 0 || n < a) RX_FAIL(h, RX_ERR_INVALID, "rx_set_hmc_statistics: need 0 <= accepted <= trials");
+        c[r] = make_ulonglong2((unsigned long long)a, (unsigned long long)n);
+    }
+    if (h->kloc == 0) return RX_OK;
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpy(h->d_hmc_stats, c.data(), sizeof(ulonglong2) * h->kloc, cudaMemcpyHostToDevice));
+    return RX_OK;
+}
+
+extern "C" int rx_get_hmc_energies(rx_engine *h, double *e_old, double *e_new) {
+    ENTER(h);
+    if (!e_old || !e_new) RX_FAIL(h, RX_ERR_INVALID, "rx_get_hmc_energies: null argument");
+    const int K = h->cfg.n_replicas;
+    for (int k = 0; k < K; k++) e_old[k] = e_new[k] = NAN;
+    if (!h->d_hmc_energy || h->kloc == 0) return RX_OK;
+    std::vector<double2> e((size_t)h->kloc);
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpy(e.data(), h->d_hmc_energy, sizeof(double2) * h->kloc, cudaMemcpyDeviceToHost));
+    for (int r = 0; r < h->kloc; r++) { e_old[h->k0 + r] = e[r].x; e_new[h->k0 + r] = e[r].y; }
     return RX_OK;
 }
 
@@ -328,12 +430,12 @@ extern "C" int rx_set_state_integrator(rx_engine *h, int32_t state, double times
     if (h->state_moves.empty()) {   // start from the common move
         h->state_moves.resize((size_t)h->cfg.n_states);
         for (auto &m : h->state_moves) {
-            m.dt = h->dt; m.gamma = h->gamma; m.n_steps = h->n_steps; m.reassign = 0;
+            m.dt = h->dt; m.gamma = h->gamma; m.n_steps = h->n_steps; m.reassign = 0; m.hmc = h->hmc;
             memcpy(m.program, h->program, sizeof(m.program));
         }
     }
     rx_state_move &m = h->state_moves[(size_t)state];
-    m.dt = timestep; m.gamma = collision_rate; m.n_steps = n_steps; m.reassign = reassign_velocities ? 1 : 0; m.set = true;
+    m.dt = timestep; m.gamma = collision_rate; m.n_steps = n_steps; m.reassign = reassign_velocities ? 1 : 0; m.set = true; m.hmc = false;
     memset(m.program, 0, sizeof(m.program));
     memcpy(m.program, splitting, n);
     h->state_moves_dirty = true;

@@ -16,6 +16,7 @@ namespace cg = cooperative_groups;
 #include <math.h>
 #include <string.h>
 #include <stdlib.h>
+#include <type_traits>
 
 // ---------------------------------------------------------------------------------------------------
 // Philox4x32-10 counter-based generator: noise is a pure function of (seed, iteration, replica, atom, step)
@@ -269,7 +270,13 @@ __device__ __forceinline__ void lj_forces(const DynParams &p, const PairCtx &c, 
 // only; nullptr: isotropic) is the per-axis state of rx_set_anisotropic_barostat, read and written inside an attempt only.
 // REG: two alchemical regions (rx_set_alchemical_regions): the parameter records carry each atom's region id instead of the
 // alchemical flag and the pair rule is region_pair's.
-template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false, bool NPT = false, bool REG = false>
+// HMC (NVT only): the move is hybrid Monte Carlo (rx_set_hmc_integrator, DESIGN 4.6): n_steps trials of n_steps
+// velocity-Verlet steps (the program "VRV"), each Metropolized on the cluster-wide fixed-point sum of U + KE.  The two
+// barostat pointers then carry HMC's arrays (so that the parameter list of every other instantiation stays as it was):
+// baro[r] += (accepted, trials) of a launch that ends finite, aniso[r] = (Eold, Enew) of the last trial.
+template <bool HMC> using BaroArg = std::conditional_t<HMC, ulonglong2, rx_barostat_state>;
+template <bool HMC> using AnisoArg = std::conditional_t<HMC, double2, rx_anisotropic_barostat_state>;
+template <bool C6, bool SW, int CL, bool PS = false, bool COMPACT = false, bool NPT = false, bool REG = false, bool HMC = false>
 __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *__restrict__ atom,
                                                     const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                     float4 *__restrict__ pos, float4 *__restrict__ vel, int k0,
@@ -277,8 +284,8 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
                                                     double *__restrict__ pot, double *__restrict__ kin,
                                                     int *__restrict__ nan_flag, const int *__restrict__ only,
                                                     const MoveDev *__restrict__ moves, double4 *__restrict__ box,
-                                                    rx_barostat_state *__restrict__ baro, const double2 *__restrict__ npt,
-                                                    double min_edge, rx_anisotropic_barostat_state *__restrict__ aniso) {
+                                                    BaroArg<HMC> *__restrict__ baro, const double2 *__restrict__ npt,
+                                                    double min_edge, AnisoArg<HMC> *__restrict__ aniso) {
     extern __shared__ float4 s_dyn[];
     // (the whole cluster takes this exit together: `only` is indexed by replica)
     if (only && !only[k0 + blockIdx.x / CL]) return;   // a retry launch propagates the replicas that failed, nothing else
@@ -510,31 +517,33 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         }
     };
 
+    auto cluster_sync = [&]() { if (CL == 1) __syncthreads(); else cg::this_cluster().sync(); };
+    // Cluster-wide sum of the per-atom energies in fixed point (2^-24 kJ/mol): integer additions are associative, so the
+    // total -- and every accept decision of the barostat and of HMC -- is the same bits in every block, at every cluster width
+    // and thread assignment.  False in `fine` when some term is not finite or too large for the format (the move is then
+    // rejected).
+    auto energy_sum = [&](float e, bool &fine) -> long long {
+        unsigned long long *acc = (unsigned long long *)s_red;   // [0] sum, [1] terms out of range (in block 0)
+        if (q == 0 && t < 2) acc[t] = 0ull;
+        cluster_sync();
+        const bool ok = !(fabsf(e) >= 67108864.0f) && !isnan(e);
+        unsigned long long v = ok ? (unsigned long long)__double2ll_rn((double)e * 16777216.0) : 0ull, bad = ok ? 0ull : 1ull;
+        for (int o = 16; o > 0; o >>= 1) { v += __shfl_xor_sync(0xffffffffu, v, o); bad += __shfl_xor_sync(0xffffffffu, bad, o); }
+        unsigned long long *dst = acc;
+        if (CL > 1) dst = cg::this_cluster().map_shared_rank(acc, 0);
+        if ((t & 31) == 0) { atomicAdd(dst, v); if (bad) atomicAdd(dst + 1, bad); }
+        cluster_sync();
+        const long long total = (long long)dst[0];
+        fine = dst[1] == 0ull;
+        cluster_sync();   // every block has read the sums before they are cleared again
+        return total;
+    };
+
     // ---- NPT: the Monte Carlo barostat (DESIGN 4.2) -------------------------------------------------------------
     // (the whole body is a discarded statement in the NVT instantiations, which compile exactly as without it)
     uint32_t n_baro = 0;   // attempts in this launch: the counter of the barostat's Philox stream
     auto barostat = [&]() {
         if constexpr (NPT) {
-            auto cluster_sync = [&]() { if (CL == 1) __syncthreads(); else cg::this_cluster().sync(); };
-            // Cluster-wide sum of the per-atom energies in fixed point (2^-24 kJ/mol): integer additions are associative, so the
-            // total -- and every accept decision -- is the same bits in every block, at every cluster width and thread
-            // assignment.  False in `fine` when some term is not finite or too large for the format (the move is then rejected).
-            auto energy_sum = [&](float e, bool &fine) -> long long {
-                unsigned long long *acc = (unsigned long long *)s_red;   // [0] sum, [1] terms out of range (in block 0)
-                if (q == 0 && t < 2) acc[t] = 0ull;
-                cluster_sync();
-                const bool ok = !(fabsf(e) >= 67108864.0f) && !isnan(e);
-                unsigned long long v = ok ? (unsigned long long)__double2ll_rn((double)e * 16777216.0) : 0ull, bad = ok ? 0ull : 1ull;
-                for (int o = 16; o > 0; o >>= 1) { v += __shfl_xor_sync(0xffffffffu, v, o); bad += __shfl_xor_sync(0xffffffffu, bad, o); }
-                unsigned long long *dst = acc;
-                if (CL > 1) dst = cg::this_cluster().map_shared_rank(acc, 0);
-                if ((t & 31) == 0) { atomicAdd(dst, v); if (bad) atomicAdd(dst + 1, bad); }
-                cluster_sync();
-                const long long total = (long long)dst[0];
-                fine = dst[1] == 0ull;
-                cluster_sync();   // every block has read the sums before they are cleared again
-                return total;
-            };
             auto set_box = [&](double X, double Y, double Z) { bf = box_f(X, Y, Z); pc.box = bf; };
             float e0;
             compute_forces(true, e0);   // (forces already valid come out the same bits: same list, same order)
@@ -615,7 +624,59 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
 
     uint32_t ocount = 0;
     float dummy;
-    for (int s = 0; s < m_steps; s++) {
+    // ---- HMC (DESIGN 4.6): HMCIntegrator's step (integrators.py:959-997) n_steps times ----------------------------------
+    // xold is kept in the replica's row of `pos` (read at the start of the launch, written at its end): with the sorted deal
+    // a list rebuild may hand the thread another atom inside a trial, and the row is indexed by atom.  The row of atom a is
+    // written by its owner at the start of a trial and read by its owner at the end; the energy sums' cluster barriers lie
+    // between the two.
+    unsigned long long hmc_acc = 0;
+    double hmc_h0 = __longlong_as_double(0x7ff8000000000000ll), hmc_h1 = hmc_h0;   // (NaN: no trial)
+    if constexpr (HMC) {
+        // (a thread without an atom adds nothing: the harmonic force path computes a term for it all the same)
+        auto h_i = [&](float e) { return active ? e + 0.5f * (vx * vx + vy * vy + vz * vz) / inv_m : 0.f; };
+        float e_cur = 0.f;      // this thread's U term at the current positions (valid after an accepted trial)
+        bool e_valid = false;
+        for (int s = 0; s < m_steps; s++) {
+            if (active) {   // v = sigma*gaussian; Eold = sum(0.5 m v^2) + energy; xold = x
+                const float3 g = philox_normal3(philox4x32_10(make_uint4(a, 0x90000000u + (uint32_t)s, k, iteration), key));
+                vx = sigma_v * g.x; vy = sigma_v * g.y; vz = sigma_v * g.z;
+                pos[(size_t)r * p.N + a] = make_float4(x, y, z, 0.f);
+            }
+            // (after an accepted trial the positions, the forces, the thread's atom and its term are those of the trial's end)
+            if (!e_valid) { compute_forces(true, e_cur); f_valid = true; }
+            bool fine0;
+            const long long H0 = energy_sum(h_i(e_cur), fine0);
+            float e1 = 0.f;
+            for (int j = 0; j < m_steps; j++) {   // v += dt/2 f/m; x += dt v; v += dt/2 f/m (the last force with the energy)
+                vx += h_V * fx * inv_m; vy += h_V * fy * inv_m; vz += h_V * fz * inv_m;
+                x += h_R * vx; y += h_R * vy; z += h_R * vz;
+                f_valid = false;
+                compute_forces(j == m_steps - 1, e1);
+                f_valid = true;
+                vx += h_V * fx * inv_m; vy += h_V * fy * inv_m; vz += h_V * fz * inv_m;
+            }
+            bool fine1;
+            const long long H1 = energy_sum(h_i(e1), fine1);
+            // accept = step(exp(-(Enew-Eold)/kT) - uniform); x = x*accept + xold*(1-accept)
+            const uint4 rr = philox4x32_10(make_uint4((uint32_t)s, 0xB0000000u, k, iteration), key);
+            const double u = ((double)rr.x + 0.5) * 2.3283064365386963e-10;
+            hmc_h0 = (double)H0 * (1.0 / 16777216.0);
+            hmc_h1 = (double)H1 * (1.0 / 16777216.0);
+            if (fine0 && fine1 && u <= exp(-(hmc_h1 - hmc_h0) / st.kT)) {
+                hmc_acc++;
+                e_cur = e1;
+                e_valid = true;
+            } else {
+                if (active) {   // xold, and NaN where x is not finite (x*0 + xold)
+                    const float4 o = pos[(size_t)r * p.N + a];
+                    x = isfinite(x) ? o.x : x * 0.f; y = isfinite(y) ? o.y : y * 0.f; z = isfinite(z) ? o.z : z * 0.f;
+                }
+                f_valid = false;
+                e_valid = false;
+            }
+        }
+    }
+    for (int s = 0; s < (HMC ? 0 : m_steps); s++) {
         if constexpr (NPT) { if (++bs.step >= 25) { bs.step = 0; barostat(); } }
         for (int q = 0; q < m_nprog; q++) {
             const char op = mv.prog[q];
@@ -671,6 +732,10 @@ __global__ void __launch_bounds__(1024) k_propagate(DynParams p, const float4 *_
         }
         kin[k] = KE;
         nan_flag[k] = (any_bad || !isfinite(U)) ? 1 : 0;
+        if constexpr (HMC) {   // (a launch that ends in NaN is retried from its snapshot: its trials are not counted)
+            if (!nan_flag[k]) { const ulonglong2 c = baro[r]; baro[r] = make_ulonglong2(c.x + hmc_acc, c.y + (unsigned)m_steps); }
+            aniso[r] = make_double2(hmc_h0, hmc_h1);
+        }
     }
     if (active) {
         if (lj) wrap_into(bf, x, y, z);
@@ -1150,6 +1215,19 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         auto kern = gb ? (star ? k_propagate_mol<true, true> : k_propagate_mol<false, true>)
                        : (star ? k_propagate_mol<true, false> : k_propagate_mol<false, false>);
         const int dyn = mol_dyn_bytes(*md, gb, true);
+        if (h->hmc) {
+            auto hk = gb ? (star ? k_propagate_mol_hmc<true, true> : k_propagate_mol_hmc<false, true>)
+                         : (star ? k_propagate_mol_hmc<true, false> : k_propagate_mol_hmc<false, false>);
+            const int rch = smem_opt_in(h, (const void *)hk, dyn);
+            if (rch) return rch;
+            hk<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p.move, (const StateDev *)h->d_states, (const int *)h->d_perm,
+                                                            (double *)h->d_pos.get(), (double *)h->d_vel.get(), h->k0, mkey,
+                                                            (uint32_t)iteration, h->d_pot, h->d_kin, h->d_nan, d_only,
+                                                            gb ? *gb : MolGB{}, h->d_hmc_stats.get(), h->d_hmc_energy.get());
+            RX_CHECK_CUDA(h, cudaGetLastError());
+            (*launches)++;
+            return RX_OK;
+        }
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
         kern<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p.move, (const StateDev *)h->d_states, (const int *)h->d_perm, (double *)h->d_pos.get(),
@@ -1160,6 +1238,10 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         return RX_OK;
     }
     const bool per_state = !h->state_moves.empty();
+    if (h->hmc && h->npt) RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_propagate: hybrid Monte Carlo at constant pressure is not provided");
+    for (const rx_state_move &m : h->state_moves)
+        if (m.hmc != h->hmc)
+            RX_FAIL(h, RX_ERR_UNSUPPORTED, "rx_propagate: the states mix hybrid Monte Carlo and Langevin moves (one launch runs one kind)");
     if (per_state) {
         int rcm = rxi_upload_state_moves(h);
         if (rcm) return rcm;
@@ -1205,6 +1287,16 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
     int rc = RX_OK;
     const bool found = with_flag(p.c_is_6, [&](auto c6) {
         return with_flag(p.use_switch, [&](auto sw) {
+            if (h->hmc)
+                return with_flag(h->two_regions, [&](auto rg) {
+                    return with_layout(PropagateLayouts{}, plan, per_state, rc, [&](auto L) {
+                        return launch_kernel(h, lc, smem > 48 * 1024, k_propagate<c6, sw, L.cl, L.ps, L.compact, false, rg, true>,
+                                             p, (const float4 *)h->d_atom, (const StateDev *)h->d_states, (const int *)h->d_perm,
+                                             h->d_pos.get(), h->d_vel.get(), h->k0, key, it32, h->d_pot.get(), h->d_kin.get(),
+                                             h->d_nan.get(), d_only, (const MoveDev *)h->d_moves, (double4 *)nullptr,
+                                             h->d_hmc_stats.get(), (const double2 *)nullptr, 0.0, h->d_hmc_energy.get());
+                    });
+                });
             return with_flag(npt, [&](auto np) {
                 return with_flag(h->two_regions, [&](auto rg) {
                     return with_layout(PropagateLayouts{}, plan, per_state, rc, [&](auto L) {
@@ -1601,6 +1693,8 @@ static int mol_check_shared(rx_engine *h, const MolDev &m, const MolGB *g, const
     const struct { const void *kern; int dyn; } use[] = {
         {g ? (const void *)k_propagate_mol<true, true> : (const void *)k_propagate_mol<true, false>, mol_dyn_bytes(m, g, true)},
         {g ? (const void *)k_propagate_mol<false, true> : (const void *)k_propagate_mol<false, false>, mol_dyn_bytes(m, g, true)},
+        {g ? (const void *)k_propagate_mol_hmc<true, true> : (const void *)k_propagate_mol_hmc<true, false>, mol_dyn_bytes(m, g, true)},
+        {g ? (const void *)k_propagate_mol_hmc<false, true> : (const void *)k_propagate_mol_hmc<false, false>, mol_dyn_bytes(m, g, true)},
         {g ? (const void *)k_minimize_mol<true> : (const void *)k_minimize_mol<false>, mol_dyn_bytes(m, g, false)},
         {g ? (const void *)k_energy_mol<true> : (const void *)k_energy_mol<false>, mol_dyn_bytes(m, g, false)}};
     size_t need = 0;

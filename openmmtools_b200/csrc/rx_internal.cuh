@@ -108,6 +108,7 @@ struct rx_state_move {
     int n_steps = 0, reassign = 0;
     char program[RX_MAX_PROGRAM] = {0};
     bool set = false;
+    bool hmc = false;   // hybrid Monte Carlo (program "VRV", gamma 0): rx_set_state_hmc_integrator
 };
 
 struct rx_engine {
@@ -155,6 +156,9 @@ struct rx_engine {
     double dt = 0, gamma = 0;
     int n_steps = 0;
     char program[RX_MAX_PROGRAM] = {0};
+    bool hmc = false;                        // the engine's move is hybrid Monte Carlo (rx_set_hmc_integrator)
+    DevBuf<ulonglong2> d_hmc_stats;          // [kloc] (accepted, trials) of HMC, cumulative
+    DevBuf<double2> d_hmc_energy;            // [kloc] (Eold, Enew) of each owned replica's last HMC trial
     RecordPtr<MolTables> mol;                // the molecule of a RX_SYSTEM_MOLECULE engine: device tables, MolDev and MolGB
     std::vector<rx_state_move> state_moves;   // per-state moves (empty: one move for all states)
     bool state_moves_dirty = false;

@@ -779,6 +779,127 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
         for (int c = 0; c < 3; c++) { pos[((size_t)r * n + a) * 3 + c] = X[a][c]; vel[((size_t)r * n + a) * 3 + c] = V[a][c]; }
 }
 
+// Hybrid Monte Carlo on a molecule (rx_set_hmc_integrator; HMCIntegrator, integrators.py:959-997): the block of
+// k_propagate_mol, mv.n_steps trials of mv.n_steps constrained velocity-Verlet steps.  Per trial: v = sqrt(kT/m) g (Philox
+// counter (atom, 0x90000000 + trial, k, iteration)), constrain velocities; Eold = KE + U; xold = x; n_steps x {v += dt/2 f/m;
+// x1 = x + dt v; x = constrain(x1); v += dt/2 f(x)/m + (x - x1)/dt; constrain velocities}; Enew = KE + U; accept iff
+// u <= exp(-(Enew - Eold)/kT) (u: counter (trial, 0xB0000000, k, iteration)), else x = x*0 + xold.  U is mol_energy's (f64,
+// the same function as the energy rows), KE a fixed-tree warp sum in f64, the forces those of k_propagate_mol (f32 terms).
+// No CM-motion removal: the reference removes it before the velocity draw, where it has no effect.  stats[r] += (accepted,
+// trials) of a launch that ends finite; energy[r] = (Eold, Enew) of the last trial.
+template <bool STAR, bool GB>
+__global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol_hmc(MolDev m, const __grid_constant__ MoveDev mv,
+                                                          const StateDev *__restrict__ states, const int *__restrict__ perm,
+                                                          double *__restrict__ pos, double *__restrict__ vel, int k0, uint2 key,
+                                                          uint32_t iteration, double *__restrict__ pot, double *__restrict__ kin,
+                                                          int *__restrict__ nan_flag, const int *__restrict__ only, MolGB g,
+                                                          ulonglong2 *__restrict__ stats, double2 *__restrict__ energy) {
+    __shared__ double X[MOL_MAX_ATOMS][3], XO[MOL_MAX_ATOMS][3], V[MOL_MAX_ATOMS][3];
+    __shared__ int s_accept;
+    extern __shared__ unsigned long long mol_tab[];
+    const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
+    if (only && !only[k]) return;
+    unsigned char *tb = (unsigned char *)mol_tab;
+    mol_stage(tb, m.terms32, m.bytes32);
+    float (*FS)[3] = (float (*)[3])(tb + mol_slots_at(m, true));
+    const MolGBArrays gs((double *)(tb + mol_gb_at(m, true)), n);
+    __syncthreads();
+    const int *g_off = (const int *)(tb + ((const MolTerms *)tb)->o_goff);
+    const bool active = a < n;
+    const StateDev st = states[perm[k]];
+    const double mass = active ? m.mass[a] : 1.0, sg = sqrt(st.kT / mass), inv_mass = 1.0 / mass;
+    if (active) for (int c = 0; c < 3; c++) { X[a][c] = pos[((size_t)r * n + a) * 3 + c]; V[a][c] = vel[((size_t)r * n + a) * 3 + c]; }
+    MolCluster kc;
+    MolStar ks;
+    kc.nc = 0;
+    const bool has_c = a < m.n_clusters;
+    if (has_c) { if (STAR) mol_star_load(m, a, ks); else mol_load_cluster(m, a, kc); }
+    __syncwarp();
+    if (has_c && STAR) mol_star_init(ks, X);
+    __syncwarp();
+    auto rattle = [&]() {
+        __syncwarp();
+        if (has_c) { if (STAR) mol_star_rattle(ks, V); else mol_rattle_cluster(m, a, kc, X, V); }
+        __syncwarp();
+    };
+    double f[3] = {0, 0, 0};
+    auto forces = [&]() {   // every thread of the block (as in k_propagate_mol)
+        __syncthreads();
+        mol_terms<float, false>(m, tb, X, FS);
+        if (GB) mol_gb_integrals<false>(g, X, n, gs);
+        __syncthreads();
+        if (GB) mol_gb_radii_pairs<false>(g, X, m.charge, n, gs);
+        if (active) {
+            float fx = 0.f, fy = 0.f, fz = 0.f;
+            for (int q = g_off[a]; q < g_off[a + 1]; q++) { fx += FS[q][0]; fy += FS[q][1]; fz += FS[q][2]; }
+            f[0] = fx; f[1] = fy; f[2] = fz;
+            if (GB) mol_gb_force(X, a, n, gs, f);
+        }
+        __syncwarp();
+    };
+    auto total = [&]() {   // KE + U (warp 0's; every thread of the block calls it)
+        __syncthreads();
+        const double U = mol_energy<GB>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs);
+        return U + mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
+    };
+    const double dt = mv.dt_d, hdt = 0.5 * dt, inv_dt = 1.0 / dt;
+    const int n_steps = mv.n_steps;
+    unsigned long long n_acc = 0;
+    double e_old = __longlong_as_double(0x7ff8000000000000ll), e_new = e_old;
+    bool f_valid = false;
+    for (int s = 0; s < n_steps; s++) {
+        if (active) {
+            const float3 gv = philox_normal3(philox4x32_10(make_uint4(a, 0x90000000u + (uint32_t)s, k, iteration), key));
+            V[a][0] = sg * gv.x; V[a][1] = sg * gv.y; V[a][2] = sg * gv.z;
+        }
+        rattle();
+        e_old = total();
+        double xold[3] = {0, 0, 0};
+        if (active) for (int c = 0; c < 3; c++) xold[c] = X[a][c];
+        if (!f_valid) forces();
+        for (int j = 0; j < n_steps; j++) {
+            double xu[3] = {0, 0, 0};
+            if (active)
+                for (int c = 0; c < 3; c++) { V[a][c] += hdt * f[c] * inv_mass; XO[a][c] = X[a][c]; X[a][c] += dt * V[a][c]; xu[c] = X[a][c]; }
+            __syncwarp();
+            if (has_c) { if (STAR) mol_star_shake(m, ks, X); else mol_shake_cluster(m, a, kc, XO, X); }
+            forces();
+            if (active) for (int c = 0; c < 3; c++) V[a][c] += hdt * f[c] * inv_mass + (X[a][c] - xu[c]) * inv_dt;
+            rattle();
+        }
+        f_valid = true;
+        e_new = total();
+        if (a == 0) {   // warp 0's energies decide; every warp takes the decision (the force evaluations are block-wide)
+            const uint4 rr = philox4x32_10(make_uint4((uint32_t)s, 0xB0000000u, k, iteration), key);
+            const double u = ((double)rr.x + 0.5) * 2.3283064365386963e-10;
+            s_accept = u <= exp(-(e_new - e_old) / st.kT);   // (NaN: rejected)
+        }
+        __syncthreads();
+        if (s_accept) {
+            n_acc++;
+        } else {
+            if (active) for (int c = 0; c < 3; c++) X[a][c] = isfinite(X[a][c]) ? xold[c] : X[a][c] * 0.0;
+            __syncwarp();
+            if (has_c && STAR) mol_star_init(ks, X);   // (the SHAKE cache is that of the constrained start)
+            f_valid = false;
+        }
+    }
+    __syncthreads();
+    const double U = mol_energy<GB>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs);
+    const double KE = mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
+    const bool bad = active && !(isfinite(X[a][0]) && isfinite(X[a][1]) && isfinite(X[a][2]) && isfinite(V[a][0]) &&
+                                 isfinite(V[a][1]) && isfinite(V[a][2]));
+    const unsigned any_bad = __ballot_sync(0xffffffffu, bad);
+    if (a == 0) {
+        pot[k] = U + states[perm[k]].offset; kin[k] = KE;
+        nan_flag[k] = (any_bad || !isfinite(U)) ? 1 : 0;
+        if (!nan_flag[k]) { const ulonglong2 c = stats[r]; stats[r] = make_ulonglong2(c.x + n_acc, c.y + (unsigned)n_steps); }
+        energy[r] = make_double2(e_old, e_new);
+    }
+    if (active)
+        for (int c = 0; c < 3; c++) { pos[((size_t)r * n + a) * 3 + c] = X[a][c]; vel[((size_t)r * n + a) * 3 + c] = V[a][c]; }
+}
+
 // MultiStateSampler.minimize (multistatesampler.py:611-647) for a molecule: FIRE descent on the constraint manifold.  The
 // force is projected onto the manifold (components along the constrained bonds removed: the RATTLE solve with unit
 // weights, unit-weight sweeps for clusters of more than MOL_MAXC constraints), the move is followed by SHAKE, the FIRE

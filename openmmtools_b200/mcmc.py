@@ -11,7 +11,11 @@ Metropolization (``{ }``), shadow-work and heat bookkeeping need per-substep ene
 Metropolized move, one Langevin move, or a ``SequenceMove`` of up to ``RX_MAX_MC_MOVES`` = 4 Metropolized moves followed
 by at most one Langevin move (none: the replicas take no dynamics steps).  On a periodic box a rotation makes its subset
 whole by minimum image from the subset's first atom and rejects a proposal that would put a rotated atom half a box edge
-or more from that atom.  GHMC/HMC/barostat/weighted moves are other kernels and out of scope.
+or more from that atom.
+
+``HMCMove`` (:1493-1594, ``integrators.HMCIntegrator`` :885-1012) runs inside the same fused propagation kernels
+(rx_set_hmc_integrator) on the LJ fluid, the harmonic oscillator and molecules (constrained); it takes the place of the
+Langevin move, alone or after the Metropolized moves of a ``SequenceMove``.  GHMC/barostat/weighted moves are other kernels and out of scope.
 """
 import copy
 import numpy as np
@@ -85,6 +89,14 @@ class BaseIntegratorMove(MCMCMove):
     # engine-facing description: (timestep ps, collision rate 1/ps, n_steps, splitting)
     def _integrator_parameters(self):
         raise NotImplementedError
+
+    def _set_on_engine(self, engine, state=None):
+        """This move as the engine's move for every state (state None) or for one state."""
+        dt, gamma, n_steps, splitting = self._integrator_parameters()
+        if state is None:
+            engine.set_integrator(dt, gamma, n_steps, splitting)
+        else:
+            engine.set_state_integrator(state, dt, gamma, n_steps, splitting, bool(self.reassign_velocities))
 
     def apply(self, thermodynamic_state, sampler_state, context_cache=None):
         """Propagate one replica (mcmc.py:668-776): builds a single-replica engine, steps, updates the state.
@@ -165,16 +177,67 @@ class LangevinDynamicsMove(BaseIntegratorMove):
             setattr(self, k, s[k])
 
 
+class HMCMove(BaseIntegratorMove):
+    """Hybrid Monte Carlo (mcmc.py:1493-1594 -> integrators.HMCIntegrator, integrators.py:885-1012).
+
+    One trial draws the velocities from the Maxwell-Boltzmann distribution, takes ``n_steps`` velocity-Verlet steps of
+    ``timestep`` and keeps the new positions with probability min(1, exp(-(Enew - Eold)/kT)), E = kinetic + potential;
+    a rejected trial restores the positions and keeps the velocities the trajectory ended with.  As in the reference,
+    ``apply`` runs ``n_steps`` such trials (``BaseIntegratorMove.apply`` calls ``integrator.step(n_steps)`` and one step of
+    ``HMCIntegrator(nsteps=n_steps)`` is a whole trial): n_steps**2 force evaluations, 10**6 at the default n_steps=1000.
+
+    Runs on the LJ fluid, the harmonic oscillator and molecules (positions and velocities constrained as in the reference's
+    program) at constant volume; constant pressure and samplers whose states mix HMC and Langevin moves raise
+    NotImplementedError.  The engine counts accepted and attempted trials per replica (``Engine.get_hmc_statistics``)."""
+
+    def __init__(self, timestep=1.0 * unit.femtosecond, n_steps=1000, **kwargs):
+        super().__init__(n_steps=n_steps, **kwargs)
+        self.timestep = timestep
+
+    def _integrator_parameters(self):
+        return float(unit.to_md(self.timestep, unit.picosecond, 'timestep')), 0.0, int(self.n_steps), 'HMC'
+
+    def _set_on_engine(self, engine, state=None):
+        dt, _, n_steps, _ = self._integrator_parameters()
+        if state is None:
+            engine.set_hmc_integrator(dt, n_steps)
+        else:
+            engine.set_state_hmc_integrator(state, dt, n_steps)
+
+    def __getstate__(self):
+        serialization = super().__getstate__()
+        serialization['timestep'] = self.timestep
+        return serialization
+
+    def __setstate__(self, serialization):
+        super().__setstate__(serialization)
+        self.timestep = serialization['timestep']
+
+
+def check_hmc(integrators, pressure=None):
+    """NotImplementedError for what the HMC kernels do not run: HMC under a barostat, or states that mix HMC and Langevin
+    moves (one fused launch runs one kind of move)."""
+    hmc = [isinstance(m, HMCMove) for m in integrators]
+    if not any(hmc):
+        return
+    if not all(hmc):
+        raise NotImplementedError('the states mix HMCMove and Langevin moves; one launch runs one kind of move: give every '
+                                  'state an HMCMove (timesteps and n_steps may differ) or none')
+    if pressure is not None:
+        raise NotImplementedError('HMCMove at constant pressure (MonteCarloBarostat / MonteCarloAnisotropicBarostat) is '
+                                  'not provided: HMCMove runs at constant volume')
+
+
 def _apply_one_replica(owner, mc_moves, integrator, thermodynamic_state, sampler_state, context_cache):
     """`mc_moves` then `integrator` (None: no dynamics) on one replica in a single-replica engine, as one rx_propagate.
     A NaN retry reruns the dynamics only, from the state the Monte Carlo moves left (the restart loop of the Langevin move
     inside SequenceMove.apply, mcmc.py:420-424, 706-759).  `owner` carries the seed counter."""
     dyn = integrator if integrator is not None else _NO_DYNAMICS
-    dt, gamma, n_steps, splitting = dyn._integrator_parameters()
+    check_hmc([dyn], thermodynamic_state.pressure)
     device = _backend.default_device(context_cache or getattr(owner, 'context_cache', None))
     eng = _backend.build_engine([thermodynamic_state], 1, device=device)
     try:
-        eng.set_integrator(dt, gamma, n_steps, splitting)
+        dyn._set_on_engine(eng)
         if mc_moves:
             eng.set_mc_moves([[m._engine_move(sampler_state.n_particles) for m in mc_moves]])
         has_v = sampler_state._velocities is not None
@@ -418,12 +481,13 @@ class SequenceMove(MCMCMove):
         self._seed_counter = 0
 
 
-_SEQUENCE_RULE = ('a move must be a Metropolized move, a Langevin move, or a SequenceMove of up to %d Metropolized '
-                  'moves followed by at most one Langevin move' % RX_MAX_MC_MOVES)
+_SEQUENCE_RULE = ('a move must be a Metropolized move, a Langevin move, an HMCMove, or a SequenceMove of up to %d '
+                  'Metropolized moves followed by at most one Langevin move or HMCMove' % RX_MAX_MC_MOVES)
 
 
 def split_move(move):
-    """(Metropolized moves, Langevin move or None) of a move; NotImplementedError for the shapes the engine does not run."""
+    """(Metropolized moves, integrator move -- Langevin or HMC -- or None) of a move; NotImplementedError for the shapes the
+    engine does not run."""
     if isinstance(move, MetropolizedMove):
         return [move], None
     if isinstance(move, BaseIntegratorMove):
@@ -448,7 +512,7 @@ def split_move(move):
 
 
 def integrator_part(move):
-    """The Langevin move a move runs (split_move), or the zero-step stand-in of a move without dynamics."""
+    """The integrator move a move runs (split_move), or the zero-step stand-in of a move without dynamics."""
     integrator = split_move(move)[1]
     return _NO_DYNAMICS if integrator is None else integrator
 

@@ -364,16 +364,15 @@ class MultiStateSampler:
         own = moves is None
         moves = self._mcmc_moves if own else moves
         integrators = [mcmc.integrator_part(mv) for mv in moves]
+        mcmc.check_hmc(integrators, self._thermodynamic_states[0].pressure)
         mv0 = integrators[0]
-        dt, gamma, n_steps, splitting = mv0._integrator_parameters()
-        self._engine.set_integrator(dt, gamma, n_steps, splitting)
+        mv0._set_on_engine(self._engine)
         self._reassign = bool(mv0.reassign_velocities)
         if own:
             self._n_restart = mv0.n_restart_attempts
         if any(not mcmc.same_integrator(mv, mv0) for mv in integrators[1:]):
             for l, mv in enumerate(integrators):
-                dt, gamma, n_steps, splitting = mv._integrator_parameters()
-                self._engine.set_state_integrator(l, dt, gamma, n_steps, splitting, bool(mv.reassign_velocities))
+                mv._set_on_engine(self._engine, l)
         mc = [mcmc.split_move(mv)[0] for mv in moves]
         if any(mc) or self._mc_moves is not None:
             n = self._thermodynamic_states[0].n_particles
