@@ -64,9 +64,10 @@ def rattle(cons, mass, x, v, tol):
     return v
 
 
-def trial(x, mass, kT, energy_forces, gauss, u, dt, n_steps, cons=None, tol=1e-10):
+def trial(x, mass, kT, energy_forces, gauss, u, dt, n_steps, cons=None, tol=1e-10, on_step=None):
     """One trial from positions x with standard normals `gauss` [N, 3] and uniform u.  energy_forces(x) -> (U, F); cons:
-    constraints (i, j, d) or None.  Returns (x, v, Eold, Enew, accepted)."""
+    constraints (i, j, d) or None; on_step(x): called with the positions after every step.  Returns (x, v, Eold, Enew,
+    accepted)."""
     mass = np.asarray(mass, np.float64)
     m = mass[:, None]
     cons = [] if cons is None else list(cons)
@@ -83,6 +84,8 @@ def trial(x, mass, kT, energy_forces, gauss, u, dt, n_steps, cons=None, tol=1e-1
         U, f = energy_forces(x)
         v = v + 0.5 * dt * f / m + (x - x1) / dt
         v = rattle(cons, mass, x, v, tol)
+        if on_step is not None:
+            on_step(x)
     e_new = 0.5 * np.sum(m * v * v) + U
     with np.errstate(over='ignore', invalid='ignore'):
         accepted = bool(np.exp(-(e_new - e_old) / kT) - u >= 0.0)   # step(exp(-(Enew-Eold)/kT) - uniform)
@@ -91,11 +94,13 @@ def trial(x, mass, kT, energy_forces, gauss, u, dt, n_steps, cons=None, tol=1e-1
     return x, v, e_old, e_new, accepted
 
 
-def run(x, mass, kT, energy_forces, gauss, u, dt, n_steps, cons=None, tol=1e-10):
-    """len(u) trials.  Returns (x, v, [(Eold, Enew, accepted) per trial])."""
+def run(x, mass, kT, energy_forces, gauss, u, dt, n_steps, cons=None, tol=1e-10, on_step=None):
+    """len(u) trials.  on_step(t, x): called with the trial's index and the positions after every step.  Returns (x, v,
+    [(Eold, Enew, accepted) per trial])."""
     out, v = [], None
     for t in range(len(u)):
-        x, v, e0, e1, acc = trial(x, mass, kT, energy_forces, gauss[t], u[t], dt, n_steps, cons, tol)
+        cb = None if on_step is None else (lambda y, t=t: on_step(t, y))
+        x, v, e0, e1, acc = trial(x, mass, kT, energy_forces, gauss[t], u[t], dt, n_steps, cons, tol, cb)
         out.append((e0, e1, acc))
     return x, v, out
 

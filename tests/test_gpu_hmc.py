@@ -29,12 +29,21 @@ def f32(a):
     return np.asarray(a, np.float32).astype(np.float64)
 
 
-def check_replica(eng, k, x0, mass, kT, ef, dt, n_steps, xg, vg, box=None, tol_x=5e-4, tol_v=5e-3, cons=None):
+def check_replica(eng, k, x0, mass, kT, ef, dt, n_steps, xg, vg, box=None, tol_x=5e-4, tol_v=5e-3, cons=None,
+                  iterations=(IT,)):
     """The device's replica k against the oracle run on the same draws: positions, the velocities the last trajectory ended
     with (kept also after a rejection), the last trial's energies, the number of accepted trials, and the last accept bit
-    as the oracle decides it from the device's dH and uniform."""
-    gauss, u = ho.draws(SEED, IT, k, len(mass), n_steps)
-    x, v, trials = ho.run(f32(x0) if cons is None else np.array(x0, np.float64), mass, kT, ef, gauss, u, dt, n_steps, cons)
+    as the oracle decides it from the device's dH and uniform.  `iterations`: the launches the device ran from x0, in order;
+    the oracle runs on from its own end state (wrapped into the box between launches, as the device wraps it).  Returns
+    the (Eold, Enew, accepted) of every trial in launch order, n_steps per launch."""
+    x = f32(x0) if cons is None else np.array(x0, np.float64)
+    trials = []
+    for q, it in enumerate(iterations):
+        if q and box is not None:
+            x = wrap(x, box)
+        gauss, u = ho.draws(SEED, it, k, len(mass), n_steps)
+        x, v, tr = ho.run(x, mass, kT, ef, gauss, u, dt, n_steps, cons)
+        trials += tr
     d = xg[k] - x if box is None else min_image(xg[k] - wrap(x, box), box)
     assert np.abs(d).max() < tol_x
     assert np.abs(vg[k] - v).max() < tol_v
@@ -42,7 +51,7 @@ def check_replica(eng, k, x0, mass, kT, ef, dt, n_steps, xg, vg, box=None, tol_x
     e0, e1, last = trials[-1]
     assert abs(e_old[k] - e0) < 1e-5 * abs(e0) + 2e-3 and abs(e_new[k] - e1) < 1e-5 * abs(e1) + 2e-3
     acc, n = eng.get_hmc_statistics()
-    assert n[k] == n_steps and acc[k] == sum(t[2] for t in trials)
+    assert n[k] == len(iterations) * n_steps and acc[k] == sum(t[2] for t in trials)
     assert (u[-1] <= np.exp(-(e_new[k] - e_old[k]) / kT)) == last
     return trials
 
