@@ -28,6 +28,8 @@ SYMBOLS = [
     'rx_set_anisotropic_barostat', 'rx_set_barostat_anisotropic', 'rx_get_barostat_anisotropic',
     'rx_set_hmc_integrator', 'rx_set_state_hmc_integrator', 'rx_get_hmc_statistics', 'rx_set_hmc_statistics',
     'rx_get_hmc_energies',
+    'rx_mbar_create', 'rx_mbar_destroy', 'rx_mbar_last_error', 'rx_mbar_evaluate', 'rx_mbar_gram', 'rx_mbar_get_logden',
+    'rx_mbar_set_max_blocks',
 ]
 RX_MAX_MC_MOVES = 4
 RX_MC_DISPLACEMENT, RX_MC_ROTATION = 0, 1
@@ -171,6 +173,15 @@ def load():
     for name in ('rx_set_boxes', 'rx_get_boxes', 'rx_set_barostat', 'rx_get_barostat', 'rx_set_barostat_anisotropic',
                  'rx_get_barostat_anisotropic'):
         getattr(lib, name).argtypes = [vp, i32, i32, vp]
+    lib.rx_mbar_create.argtypes = [i32, i64, vp, vp, C.POINTER(vp)]
+    lib.rx_mbar_destroy.argtypes = [vp]
+    lib.rx_mbar_destroy.restype = None
+    lib.rx_mbar_last_error.argtypes = [vp]
+    lib.rx_mbar_last_error.restype = C.c_char_p
+    lib.rx_mbar_evaluate.argtypes = [vp, vp, vp, vp, vp]
+    lib.rx_mbar_gram.argtypes = [vp, vp, vp, vp]
+    lib.rx_mbar_get_logden.argtypes = [vp, vp]
+    lib.rx_mbar_set_max_blocks.argtypes = [vp, i32]
     if lib.rx_abi_version() != RX_ABI_VERSION:
         raise ImportError('librx_b200.so ABI version mismatch')
     _lib = lib

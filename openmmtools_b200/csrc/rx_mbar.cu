@@ -1,0 +1,333 @@
+// rx_mbar.cu -- the two passes of an MBAR solve over a device-resident reduced-potential matrix (DESIGN §4.7).
+//
+// Shirts & Chodera 2008: with c_k = log N_k + f_k, the density of sample n is log D_n = logsumexp_k (c_k - u_kn) and its
+// weight in state i is W_in = exp(f_i - u_in - log D_n).  Pass 1 (k_mbar_logden) writes log D_n; pass 2 reduces W over
+// the samples: k_mbar_rowsum gives sum_n W_in and sum_n log D_n, k_mbar_gram gives sum_n W_in W_jn.  Every reduction is
+// cut into chunks of samples whose number depends on K and N only; a chunk is summed by one block in a fixed order and
+// the chunks are then added by a fixed pairwise tree (k_mbar_tree), so results do not depend on the grid.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <string.h>
+#include <string>
+#include <vector>
+#include "rx_internal.cuh"
+
+namespace {
+
+constexpr int GT = 64;            // Gram output tile edge (states)
+constexpr int GS = 16;            // samples per shared-memory step of the Gram tile
+constexpr int GTHREADS = 256;     // 16 x 16 threads, 4 x 4 outputs each
+constexpr int RTHREADS = 256;     // k_mbar_rowsum block
+constexpr int ROW_CHUNK = 8192;   // samples per k_mbar_rowsum chunk
+constexpr int GRAM_WORK = 2048;   // k_mbar_gram aims at this many (tile pair, chunk) work items
+
+// u_kn row i, sample n -> W_in; 0 outside the matrix
+__device__ __forceinline__ double weight(const double *__restrict__ u, size_t N, int K, int i, long long n,
+                                         const double *__restrict__ f, const double *__restrict__ logD) {
+    if (i >= K || n >= (long long)N) return 0.0;
+    return exp(f[i] - u[(size_t)i * N + n] - logD[n]);
+}
+
+// Pass 1: one thread per sample, a running log-sum-exp over the states in index order.  States with c_k = -inf (no
+// samples) add nothing and never become the running maximum.
+__global__ void k_mbar_logden(const double *__restrict__ u, size_t N, int K, const double *__restrict__ c,
+                              double *__restrict__ logD) {
+    for (long long n = blockIdx.x * (long long)blockDim.x + threadIdx.x; n < (long long)N;
+         n += (long long)gridDim.x * blockDim.x) {
+        double m = -INFINITY, s = 0.0;
+        for (int k = 0; k < K; ++k) {
+            const double ck = c[k];
+            if (ck == -INFINITY) continue;
+            const double v = ck - u[(size_t)k * N + n];
+            if (v > m) { s = s * exp(m - v) + 1.0; m = v; }
+            else s += exp(v - m);
+        }
+        logD[n] = m + log(s);
+    }
+}
+
+// sum over a block of RTHREADS in a fixed order
+__device__ double block_sum(double v, double *sh) {
+    sh[threadIdx.x] = v;
+    __syncthreads();
+    for (int o = RTHREADS / 2; o > 0; o >>= 1) {
+        if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o];
+        __syncthreads();
+    }
+    const double r = sh[0];
+    __syncthreads();
+    return r;
+}
+
+// Pass 2a: work item (row r, chunk c) -> part[c * (K + 1) + r] = sum over the chunk's samples of W_rn (r < K) or of
+// log D_n (r = K).  Each thread sums a strided subsequence of the chunk in order, then the block adds the threads.
+__global__ void k_mbar_rowsum(const double *__restrict__ u, size_t N, int K, const double *__restrict__ f,
+                              const double *__restrict__ logD, int n_chunks, double *__restrict__ part) {
+    __shared__ double sh[RTHREADS];
+    const long long items = (long long)(K + 1) * n_chunks;
+    for (long long w = blockIdx.x; w < items; w += gridDim.x) {
+        const int r = (int)(w % (K + 1)), c = (int)(w / (K + 1));
+        const long long n0 = (long long)c * ROW_CHUNK, n1 = min(n0 + ROW_CHUNK, (long long)N);
+        double s = 0.0;
+        for (long long n = n0 + threadIdx.x; n < n1; n += RTHREADS)
+            s += r < K ? exp(f[r] - u[(size_t)r * N + n] - logD[n]) : logD[n];
+        s = block_sum(s, sh);
+        if (threadIdx.x == 0) part[(size_t)c * (K + 1) + r] = s;
+    }
+}
+
+// Pass 2b: work item (tile pair p = (I, J) with I <= J, chunk c) -> the 64 x 64 block G[I-tile][J-tile] summed over the
+// chunk's samples, at part[(c * n_pairs + p) * 4096].  Per step of GS samples the block stages W of both row tiles,
+// transposed (sample-major), in shared memory; thread (tx, ty) owns rows ty + 16 a and columns tx + 16 b (a, b < 4), so
+// a warp reads its J-row operands from consecutive addresses and its I-row operands as broadcasts.
+__global__ void __launch_bounds__(GTHREADS) k_mbar_gram(const double *__restrict__ u, size_t N, int K,
+                                                        const double *__restrict__ f, const double *__restrict__ logD,
+                                                        int n_tiles, int n_pairs, int n_chunks, long long chunk,
+                                                        double *__restrict__ part) {
+    __shared__ double sA[GS][GT + 1], sB[GS][GT + 1];
+    const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;
+    const long long items = (long long)n_pairs * n_chunks;
+    for (long long w = blockIdx.x; w < items; w += gridDim.x) {
+        int p = (int)(w % n_pairs), I = 0;
+        const int c = (int)(w / n_pairs);
+        while (p >= n_tiles - I) { p -= n_tiles - I; ++I; }   // p-th pair of the upper triangle, row-major
+        const int J = I + p;
+        const long long n0 = c * chunk, n1 = min(n0 + chunk, (long long)N);
+        double acc[4][4] = {};
+        for (long long s0 = n0; s0 < n1; s0 += GS) {
+            // 64 rows x GS samples per tile: thread t stages row t / 4, samples 4 (t % 4) .. + 3
+            const int row = threadIdx.x / 4, col = 4 * (threadIdx.x % 4);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const long long n = s0 + col + q;
+                const bool in = n < n1;
+                sA[col + q][row] = in ? weight(u, N, K, I * GT + row, n, f, logD) : 0.0;
+                if (I != J) sB[col + q][row] = in ? weight(u, N, K, J * GT + row, n, f, logD) : 0.0;
+            }
+            __syncthreads();
+            const double(*B)[GT + 1] = I == J ? sA : sB;
+#pragma unroll
+            for (int s = 0; s < GS; ++s) {
+                double a[4], b[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) { a[q] = sA[s][ty + 16 * q]; b[q] = B[s][tx + 16 * q]; }
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) acc[i][j] = fma(a[i], b[j], acc[i][j]);
+            }
+            __syncthreads();
+        }
+        double *out = part + ((size_t)c * n_pairs + (I * n_tiles - I * (I - 1) / 2 + (J - I))) * (GT * GT);
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) out[(ty + 16 * i) * GT + tx + 16 * j] = acc[i][j];
+    }
+}
+
+// One level of the fixed pairwise tree over chunk records of len doubles: rec[c] += rec[c + half] for c < n - half.
+__global__ void k_mbar_tree(double *__restrict__ rec, size_t len, int n, int half) {
+    const size_t total = (size_t)(n - half) * len;
+    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x)
+        rec[e] += rec[e + (size_t)half * len];
+}
+
+}  // namespace
+
+struct rx_mbar {
+    int K = 0;
+    size_t N = 0;
+    int device = 0;              // the current device at rx_mbar_create
+    int n_sm = 0;
+    int max_blocks = 0;          // rx_mbar_set_max_blocks (0: from the device)
+    std::vector<double> logN;    // log N_k, -inf for N_k = 0
+    std::vector<double> Nk;
+    int row_chunks = 0;          // k_mbar_rowsum chunks
+    int n_tiles = 0, n_pairs = 0, gram_chunks = 0;
+    long long gram_chunk = 0;    // samples per k_mbar_gram chunk (a multiple of GS)
+    DevBuf<double> d_u, d_logD, d_c, d_f, d_rows, d_gram;
+    std::vector<double> h_rows, h_gram;
+    cudaStream_t stream = nullptr;
+    std::string err;
+    ~rx_mbar() { if (stream) cudaStreamDestroy(stream); }
+};
+
+namespace {
+
+thread_local std::string g_mbar_create_error;
+
+int blocks_for(const rx_mbar *h, long long items, int per_sm) {
+    long long b = h->max_blocks > 0 ? h->max_blocks : (long long)h->n_sm * per_sm;
+    return (int)std::max(1LL, std::min(items, b));
+}
+
+// sums n_chunks records of len doubles in place into rec[0]
+int tree(rx_mbar *h, double *rec, size_t len, int n) {
+    while (n > 1) {
+        const int half = (n + 1) / 2;
+        const long long work = (long long)(n - half) * (long long)len;
+        k_mbar_tree<<<blocks_for(h, (work + 255) / 256, 16), 256, 0, h->stream>>>(rec, len, n, half);
+        RX_CHECK_CUDA(h, cudaGetLastError());
+        n = half;
+    }
+    return RX_OK;
+}
+
+// log D at f, then sum_n W_in and sum_n log D_n (h_rows) and, when gram, sum_n W_in W_jn (h_gram, upper tile pairs)
+int run(rx_mbar *h, const double *f, bool gram) {
+    const int K = h->K;
+    RX_CHECK_CUDA(h, cudaSetDevice(h->device));
+    std::vector<double> c(K);
+    for (int k = 0; k < K; ++k) {
+        if (!isfinite(f[k])) RX_FAIL(h, RX_ERR_INVALID, "f_k must be finite");
+        c[k] = h->logN[k] + f[k];
+    }
+    RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_c, c.data(), K * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpyAsync(h->d_f, f, K * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    k_mbar_logden<<<blocks_for(h, ((long long)h->N + 255) / 256, 16), 256, 0, h->stream>>>(h->d_u, h->N, K, h->d_c,
+                                                                                              h->d_logD);
+    RX_CHECK_CUDA(h, cudaGetLastError());
+    k_mbar_rowsum<<<blocks_for(h, (long long)(K + 1) * h->row_chunks, 8), RTHREADS, 0, h->stream>>>(
+        h->d_u, h->N, K, h->d_f, h->d_logD, h->row_chunks, h->d_rows);
+    RX_CHECK_CUDA(h, cudaGetLastError());
+    int rc = tree(h, h->d_rows, K + 1, h->row_chunks);
+    if (rc) return rc;
+    RX_CHECK_CUDA(h, cudaMemcpyAsync(h->h_rows.data(), h->d_rows, (K + 1) * sizeof(double), cudaMemcpyDeviceToHost,
+                                     h->stream));
+    if (gram) {
+        k_mbar_gram<<<blocks_for(h, (long long)h->n_pairs * h->gram_chunks, 8), GTHREADS, 0, h->stream>>>(
+            h->d_u, h->N, K, h->d_f, h->d_logD, h->n_tiles, h->n_pairs, h->gram_chunks, h->gram_chunk, h->d_gram);
+        RX_CHECK_CUDA(h, cudaGetLastError());
+        rc = tree(h, h->d_gram, (size_t)h->n_pairs * GT * GT, h->gram_chunks);
+        if (rc) return rc;
+        RX_CHECK_CUDA(h, cudaMemcpyAsync(h->h_gram.data(), h->d_gram, h->h_gram.size() * sizeof(double),
+                                         cudaMemcpyDeviceToHost, h->stream));
+    }
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    return RX_OK;
+}
+
+// the full K x K Gram matrix from the upper tile pairs of h_gram
+void unpack_gram(const rx_mbar *h, double *G) {
+    const int K = h->K, T = h->n_tiles;
+    for (int i = 0; i < K; ++i)
+        for (int j = i; j < K; ++j) {
+            const int I = i / GT, J = j / GT;
+            const size_t p = (size_t)I * T - (size_t)I * (I - 1) / 2 + (J - I);
+            const double v = h->h_gram[p * GT * GT + (i % GT) * GT + (j % GT)];
+            G[(size_t)i * K + j] = v;
+            G[(size_t)j * K + i] = v;
+        }
+}
+
+}  // namespace
+
+extern "C" const char *rx_mbar_last_error(const rx_mbar *h) { return h ? h->err.c_str() : g_mbar_create_error.c_str(); }
+
+extern "C" int rx_mbar_create(int32_t K, int64_t N, const double *u_kn, const int64_t *N_k, rx_mbar **out) {
+#define MBAR_CREATE_FAIL(code, msg) do { g_mbar_create_error = (msg); return (code); } while (0)
+    if (!out) MBAR_CREATE_FAIL(RX_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (K < 1 || N < 1 || !u_kn || !N_k) MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create: need K >= 1, N >= 1, u_kn and N_k");
+    long long total = 0;
+    for (int k = 0; k < K; ++k) {
+        if (N_k[k] < 0) MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create: N_k must be non-negative");
+        total += N_k[k];
+    }
+    if (total != N) MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create: sum of N_k must equal N");
+    auto h = std::make_unique<rx_mbar>();
+    h->K = K;
+    h->N = (size_t)N;
+    h->row_chunks = (int)((N + ROW_CHUNK - 1) / ROW_CHUNK);
+    h->n_tiles = (K + GT - 1) / GT;
+    h->n_pairs = h->n_tiles * (h->n_tiles + 1) / 2;
+    // chunks of the Gram pass: about GRAM_WORK work items, at least 2 * GS samples each
+    long long want = std::max(1, GRAM_WORK / h->n_pairs);
+    want = std::min(want, std::max(1LL, (long long)N / (2 * GS)));
+    h->gram_chunk = ((N + want - 1) / want + GS - 1) / GS * GS;
+    h->gram_chunks = (int)((N + h->gram_chunk - 1) / h->gram_chunk);
+    const size_t bytes = (size_t)K * N * sizeof(double) + (size_t)N * sizeof(double) +
+                         (size_t)h->row_chunks * (K + 1) * sizeof(double) +
+                         (size_t)h->gram_chunks * h->n_pairs * GT * GT * sizeof(double);
+    if (cudaGetDevice(&h->device) != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: no CUDA device");
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: cudaMemGetInfo failed");
+    // the size is checked before u_kn is read
+    if (bytes > free_b)
+        MBAR_CREATE_FAIL(RX_ERR_UNSUPPORTED, "rx_mbar_create: u_kn and its reduction buffers need " + std::to_string(bytes) +
+                                                 " bytes, the device has " + std::to_string(free_b) + " free");
+    if (cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, h->device) != cudaSuccess)
+        MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: cudaDeviceGetAttribute failed");
+    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess)
+        MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: cudaStreamCreate failed");
+    cudaError_t e = h->d_u.alloc((size_t)K * N);
+    if (e == cudaSuccess) e = h->d_logD.alloc(N);
+    if (e == cudaSuccess) e = h->d_c.alloc(K);
+    if (e == cudaSuccess) e = h->d_f.alloc(K);
+    if (e == cudaSuccess) e = h->d_rows.alloc((size_t)h->row_chunks * (K + 1));
+    if (e == cudaSuccess) e = h->d_gram.alloc((size_t)h->gram_chunks * h->n_pairs * GT * GT);
+    if (e == cudaErrorMemoryAllocation) {
+        cudaGetLastError();
+        MBAR_CREATE_FAIL(RX_ERR_UNSUPPORTED, "rx_mbar_create: out of device memory for u_kn and its reduction buffers");
+    }
+    if (e != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, std::string("rx_mbar_create: ") + cudaGetErrorString(e));
+    if (cudaMemcpy(h->d_u, u_kn, (size_t)K * N * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess)
+        MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: upload of u_kn failed");
+    h->logN.resize(K);
+    h->Nk.resize(K);
+    for (int k = 0; k < K; ++k) {
+        h->Nk[k] = (double)N_k[k];
+        h->logN[k] = N_k[k] > 0 ? log((double)N_k[k]) : -INFINITY;
+    }
+    h->h_rows.resize(K + 1);
+    h->h_gram.resize((size_t)h->n_pairs * GT * GT);
+    *out = h.release();
+    return RX_OK;
+#undef MBAR_CREATE_FAIL
+}
+
+extern "C" void rx_mbar_destroy(rx_mbar *h) { delete h; }
+
+extern "C" int rx_mbar_set_max_blocks(rx_mbar *h, int32_t max_blocks) {
+    if (!h || max_blocks < 0) return RX_ERR_INVALID;
+    h->max_blocks = max_blocks;
+    return RX_OK;
+}
+
+extern "C" int rx_mbar_evaluate(rx_mbar *h, const double *f_k, double *logden_sum, double *grad, double *hess) {
+    if (!h) return RX_ERR_INVALID;
+    if (!f_k) RX_FAIL(h, RX_ERR_INVALID, "f_k is NULL");
+    const int rc = run(h, f_k, hess != nullptr);
+    if (rc) return rc;
+    const int K = h->K;
+    if (logden_sum) *logden_sum = h->h_rows[K];
+    if (grad)
+        for (int i = 0; i < K; ++i) grad[i] = h->Nk[i] - h->Nk[i] * h->h_rows[i];
+    if (hess) {
+        unpack_gram(h, hess);
+        for (int i = 0; i < K; ++i) {
+            for (int j = 0; j < K; ++j) hess[(size_t)i * K + j] *= h->Nk[i] * h->Nk[j];
+            hess[(size_t)i * K + i] -= h->Nk[i] * h->h_rows[i];
+        }
+    }
+    return RX_OK;
+}
+
+extern "C" int rx_mbar_gram(rx_mbar *h, const double *f_k, double *G, double *wsum) {
+    if (!h) return RX_ERR_INVALID;
+    if (!f_k || !G) RX_FAIL(h, RX_ERR_INVALID, "f_k and G must not be NULL");
+    const int rc = run(h, f_k, true);
+    if (rc) return rc;
+    unpack_gram(h, G);
+    if (wsum) memcpy(wsum, h->h_rows.data(), h->K * sizeof(double));
+    return RX_OK;
+}
+
+extern "C" int rx_mbar_get_logden(rx_mbar *h, double *logD) {
+    if (!h) return RX_ERR_INVALID;
+    if (!logD) RX_FAIL(h, RX_ERR_INVALID, "logD is NULL");
+    RX_CHECK_CUDA(h, cudaSetDevice(h->device));
+    RX_CHECK_CUDA(h, cudaMemcpy(logD, h->d_logD, h->N * sizeof(double), cudaMemcpyDeviceToHost));
+    return RX_OK;
+}

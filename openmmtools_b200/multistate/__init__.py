@@ -5,3 +5,4 @@ from .paralleltempering import ParallelTemperingSampler
 from .sams import SAMSSampler
 from .utils import SimulationNaNError
 from .multistatereporter import MultiStateReporter
+from .multistateanalyzer import MultiStateSamplerAnalyzer, ReplicaExchangeAnalyzer, SAMSAnalyzer, MultiPhaseAnalyzer
