@@ -462,6 +462,30 @@ RX_API int rx_mbar_gram(rx_mbar *h, const double *f_k, double *G, double *wsum);
 RX_API int rx_mbar_get_logden(rx_mbar *h, double *logD);
 RX_API int rx_mbar_set_max_blocks(rx_mbar *h, int32_t max_blocks);
 
+/* ---- energy history: the energy matrices of a run, kept on the device for MBAR ------------------------------------
+ * Row t is iteration t: [K][M + U] doubles, the K x M matrix of rx_compute_energies followed by the K x U block of the
+ * last rx_compute_energies_at* call (U unsampled states, 0 or more).  Capacity grows geometrically; a growth is checked
+ * against the free device memory first and returns RX_ERR_UNSUPPORTED when it does not fit, leaving the history as it
+ * was.  8 K (M + U) bytes per iteration.  In a multi-GPU run the matrices are all-gathered, so one rank can keep it.
+ *
+ * rx_history_append   row `iteration` (<= the current length; later rows are dropped; 0 starts a new history) from the
+ *                     current matrices, by device-to-device copies on the engine's stream.  RX_ERR_INVALID when U > 0 and
+ *                     the last rx_compute_energies_at* call did not compute U states.
+ * rx_history_truncate keeps iterations 0..iteration (-1: none).
+ * rx_history_load     replaces the history by n_iterations rows from the host: u [n][K][M], u_unsampled [n][K][U].
+ * rx_history_reserve  capacity for n_iterations rows of U unsampled states.
+ * rx_history_length   the number of rows and U.
+ * rx_mbar_create_from_history  rx_mbar_create with u_kn gathered on the device from the history of engine h: row i of
+ *                     u_kn is history column columns[i] (< M + U), and column r n_sel + j is replica r at iteration
+ *                     iterations[j] (replica-major).  RX_ERR_INVALID when an element is not finite. */
+RX_API int rx_history_append(rx_engine *h, int64_t iteration, int32_t n_unsampled);
+RX_API int rx_history_truncate(rx_engine *h, int64_t iteration);
+RX_API int rx_history_load(rx_engine *h, int64_t n_iterations, int32_t n_unsampled, const double *u, const double *u_unsampled);
+RX_API int rx_history_reserve(rx_engine *h, int64_t n_iterations, int32_t n_unsampled);
+RX_API int rx_history_length(rx_engine *h, int64_t *n_iterations, int32_t *n_unsampled);
+RX_API int rx_mbar_create_from_history(rx_engine *h, int32_t K, int64_t n_sel, const int64_t *iterations,
+                                       const int32_t *columns, const int64_t *N_k, rx_mbar **out);
+
 #ifdef __cplusplus
 }
 #endif

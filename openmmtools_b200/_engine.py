@@ -434,6 +434,34 @@ class Engine:
         self._check(self._lib.rx_get_energies(self._h, _ptr(u)))
         return u
 
+    # -- energy history (rx_history_*): row t holds iteration t's (K, M) matrix and (K, U) unsampled block on the device
+    def history_append(self, iteration, n_unsampled=0):
+        """Row `iteration` from the current matrix and, with n_unsampled > 0, the last compute_energies_at block."""
+        self._check(self._lib.rx_history_append(self._h, int(iteration), int(n_unsampled)))
+
+    def history_truncate(self, iteration):
+        """Keep iterations 0..iteration."""
+        self._check(self._lib.rx_history_truncate(self._h, int(iteration)))
+
+    def history_load(self, u, u_unsampled=None):
+        """Replace the history by u (T, K, M) and u_unsampled (T, K, U)."""
+        u = _c64(u)
+        T = u.shape[0]
+        uu = np.zeros((T, self.K, 0)) if u_unsampled is None else _c64(u_unsampled)
+        if u.shape != (T, self.K, self.M) or uu.shape[:2] != (T, self.K):
+            raise ValueError('expected (T, %d, %d) and (T, %d, U) energies, got %s and %s' % (self.K, self.M, self.K, u.shape,
+                                                                                            uu.shape))
+        self._check(self._lib.rx_history_load(self._h, T, uu.shape[2], _ptr(u), _ptr(uu)))
+
+    def history_reserve(self, n_iterations, n_unsampled=0):
+        self._check(self._lib.rx_history_reserve(self._h, int(n_iterations), int(n_unsampled)))
+
+    def history_length(self):
+        """(iterations held, unsampled states per row)."""
+        n, u = C.c_int64(), C.c_int32()
+        self._check(self._lib.rx_history_length(self._h, C.byref(n), C.byref(u)))
+        return n.value, u.value
+
     def mix_seed(self, seed, stream=_lib.RX_STREAM_NUMBA):
         self._check(self._lib.rx_mix_seed(self._h, stream, int(seed) & 0xFFFFFFFF))
 

@@ -30,6 +30,8 @@ SYMBOLS = [
     'rx_get_hmc_energies',
     'rx_mbar_create', 'rx_mbar_destroy', 'rx_mbar_last_error', 'rx_mbar_evaluate', 'rx_mbar_gram', 'rx_mbar_get_logden',
     'rx_mbar_set_max_blocks',
+    'rx_history_append', 'rx_history_truncate', 'rx_history_load', 'rx_history_reserve', 'rx_history_length',
+    'rx_mbar_create_from_history',
 ]
 RX_MAX_MC_MOVES = 4
 RX_MC_DISPLACEMENT, RX_MC_ROTATION = 0, 1
@@ -182,6 +184,12 @@ def load():
     lib.rx_mbar_gram.argtypes = [vp, vp, vp, vp]
     lib.rx_mbar_get_logden.argtypes = [vp, vp]
     lib.rx_mbar_set_max_blocks.argtypes = [vp, i32]
+    lib.rx_history_append.argtypes = [vp, i64, i32]
+    lib.rx_history_truncate.argtypes = [vp, i64]
+    lib.rx_history_load.argtypes = [vp, i64, i32, vp, vp]
+    lib.rx_history_reserve.argtypes = [vp, i64, i32]
+    lib.rx_history_length.argtypes = [vp, C.POINTER(i64), C.POINTER(i32)]
+    lib.rx_mbar_create_from_history.argtypes = [vp, i32, i64, vp, vp, vp, C.POINTER(vp)]
     if lib.rx_abi_version() != RX_ABI_VERSION:
         raise ImportError('librx_b200.so ABI version mismatch')
     _lib = lib

@@ -975,10 +975,15 @@ static int energies_at(rx_engine *h, const rx_state_params *st, const double *la
     }
     const int K = h->cfg.n_replicas;
     DevBuf<StateDev> d_st;
-    DevBuf<double> d_out;
     DevBuf<double2> d_tab;
     RX_CHECK_CUDA(h, d_st.alloc(n));
-    RX_CHECK_CUDA(h, d_out.alloc((size_t)K * n));
+    // the result stays in d_u_at, where rx_history_append finds the unsampled block
+    h->u_at_cols = 0;
+    if ((size_t)K * n > h->u_at_cap) {
+        RX_CHECK_CUDA(h, h->d_u_at.alloc((size_t)K * n));
+        h->u_at_cap = (size_t)K * n;
+    }
+    double *d_out = h->d_u_at;
     if (pressure) RX_CHECK_CUDA(h, d_tab.alloc(n));
     int launches = 0;
     cudaMemcpyAsync(d_st, hs.data(), sizeof(StateDev) * n, cudaMemcpyHostToDevice, h->stream);
@@ -994,7 +999,108 @@ static int energies_at(rx_engine *h, const rx_state_params *st, const double *la
     cudaStreamSynchronize(h->stream);   // (before the buffers are freed)
     if (rc) return rc;
     h->phase_launches[2] += launches;
-    return check_device_error(h);
+    rc = check_device_error(h);
+    if (!rc) h->u_at_cols = n;
+    return rc;
+}
+
+// ---- energy history -------------------------------------------------------------------------------------------------
+// Capacity for `rows` rows of M + U doubles per replica, grown geometrically.  The growth is checked against the free
+// device memory first, and a growth that fails leaves the history as it was.
+static int history_reserve(rx_engine *h, long long rows, int U, const char *who) {
+    const size_t row = (size_t)h->cfg.n_replicas * (h->cfg.n_states + U);
+    if (rows < 0 || U < 0) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": negative size");
+    if (h->hist_len > 0 && U != h->hist_u)
+        RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": the history holds " + std::to_string(h->hist_u) + " unsampled states");
+    if ((size_t)rows * row <= h->hist_cap) return RX_OK;
+    const size_t want = std::max((size_t)rows * row, std::max((size_t)16 * row, 2 * h->hist_cap));
+    size_t free_b = 0, total_b = 0;
+    RX_CHECK_CUDA(h, cudaMemGetInfo(&free_b, &total_b));
+    if (rows > (long long)(SIZE_MAX / 16 / row) || want * sizeof(double) > free_b)
+        RX_FAIL(h, RX_ERR_UNSUPPORTED, std::string(who) + ": an energy history of " + std::to_string(rows) +
+                                           " iterations needs " + std::to_string(want * sizeof(double)) + " bytes, the device has " +
+                                           std::to_string(free_b) + " free");
+    DevBuf<double> grown;
+    const cudaError_t e = grown.alloc(want);
+    if (e == cudaErrorMemoryAllocation) {
+        cudaGetLastError();
+        RX_FAIL(h, RX_ERR_UNSUPPORTED, std::string(who) + ": out of device memory for the energy history");
+    }
+    RX_CHECK_CUDA(h, e);
+    if (h->hist_len > 0)
+        RX_CHECK_CUDA(h, cudaMemcpyAsync(grown, h->d_hist, (size_t)h->hist_len * row * sizeof(double), cudaMemcpyDeviceToDevice,
+                                         h->stream));
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    h->d_hist = std::move(grown);
+    h->hist_cap = want;
+    return RX_OK;
+}
+
+extern "C" int rx_history_reserve(rx_engine *h, int64_t n_iterations, int32_t n_unsampled) {
+    ENTER(h);
+    return history_reserve(h, n_iterations, n_unsampled, "rx_history_reserve");
+}
+
+extern "C" int rx_history_append(rx_engine *h, int64_t iteration, int32_t n_unsampled) {
+    ENTER(h);
+    if (iteration < 0 || iteration > h->hist_len)
+        RX_FAIL(h, RX_ERR_INVALID, "rx_history_append: iteration " + std::to_string(iteration) + " does not follow the " +
+                                       std::to_string(h->hist_len) + " iterations of the history");
+    if (n_unsampled > 0 && h->u_at_cols != n_unsampled)
+        RX_FAIL(h, RX_ERR_INVALID, "rx_history_append: the last rx_compute_energies_at call did not compute " +
+                                       std::to_string(n_unsampled) + " states");
+    const long long len = h->hist_len;
+    if (iteration == 0) h->hist_len = 0;    // a new history may change the number of unsampled states
+    int rc = history_reserve(h, iteration + 1, n_unsampled, "rx_history_append");
+    if (rc) { h->hist_len = len; return rc; }
+    const int K = h->cfg.n_replicas, M = h->cfg.n_states, W = M + n_unsampled;
+    double *row = h->d_hist + (size_t)iteration * K * W;
+    RX_CHECK_CUDA(h, cudaMemcpy2DAsync(row, W * sizeof(double), h->d_u, M * sizeof(double), M * sizeof(double), K,
+                                       cudaMemcpyDeviceToDevice, h->stream));
+    if (n_unsampled > 0)
+        RX_CHECK_CUDA(h, cudaMemcpy2DAsync(row + M, W * sizeof(double), h->d_u_at, n_unsampled * sizeof(double),
+                                           n_unsampled * sizeof(double), K, cudaMemcpyDeviceToDevice, h->stream));
+    h->hist_len = iteration + 1;
+    h->hist_u = n_unsampled;
+    return RX_OK;
+}
+
+extern "C" int rx_history_truncate(rx_engine *h, int64_t iteration) {
+    ENTER(h);
+    if (iteration < -1) RX_FAIL(h, RX_ERR_INVALID, "rx_history_truncate: iteration must be >= -1");
+    h->hist_len = std::min(h->hist_len, (long long)iteration + 1);
+    return RX_OK;
+}
+
+extern "C" int rx_history_load(rx_engine *h, int64_t n_iterations, int32_t n_unsampled, const double *u,
+                               const double *u_unsampled) {
+    ENTER(h);
+    if (n_iterations < 0 || n_unsampled < 0 || (n_iterations > 0 && !u) || (n_iterations > 0 && n_unsampled > 0 && !u_unsampled))
+        RX_FAIL(h, RX_ERR_INVALID, "rx_history_load: bad arguments");
+    const long long len = h->hist_len;
+    h->hist_len = 0;     // (the old rows are not kept)
+    int rc = history_reserve(h, n_iterations, n_unsampled, "rx_history_load");
+    if (rc) { h->hist_len = len; return rc; }
+    const int M = h->cfg.n_states, W = M + n_unsampled;
+    const size_t height = (size_t)n_iterations * h->cfg.n_replicas;
+    RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (height > 0) {
+        RX_CHECK_CUDA(h, cudaMemcpy2D(h->d_hist, W * sizeof(double), u, M * sizeof(double), M * sizeof(double), height,
+                                      cudaMemcpyHostToDevice));
+        if (n_unsampled > 0)
+            RX_CHECK_CUDA(h, cudaMemcpy2D(h->d_hist + M, W * sizeof(double), u_unsampled, n_unsampled * sizeof(double),
+                                          n_unsampled * sizeof(double), height, cudaMemcpyHostToDevice));
+    }
+    h->hist_len = n_iterations;
+    h->hist_u = n_unsampled;
+    return RX_OK;
+}
+
+extern "C" int rx_history_length(rx_engine *h, int64_t *n_iterations, int32_t *n_unsampled) {
+    ENTER(h);
+    if (n_iterations) *n_iterations = h->hist_len;
+    if (n_unsampled) *n_unsampled = h->hist_u;
+    return RX_OK;
 }
 
 extern "C" int rx_compute_energies_at(rx_engine *h, const rx_state_params *st, int32_t n, double *u_out) {

@@ -203,6 +203,15 @@ struct rx_engine {
     // anisotropic barostat (rx_set_anisotropic_barostat): per owned replica per-axis state; the step counter stays in d_baro
     bool aniso = false;
     DevBuf<rx_anisotropic_barostat_state> d_aniso, d_aniso_snap;
+    // energies of the last rx_compute_energies_at* call, [K][u_at_cols] after the all-gather
+    DevBuf<double> d_u_at;
+    size_t u_at_cap = 0;
+    int u_at_cols = 0;
+    // energy history (rx_history_*): row t is iteration t, [K][M + hist_u] (the sampled states, then the unsampled ones)
+    DevBuf<double> d_hist;
+    size_t hist_cap = 0;          // doubles
+    long long hist_len = 0;       // rows
+    int hist_u = 0;
     // nccl
     void *nccl_lib = nullptr;
     void *nccl_comm = nullptr;

@@ -126,6 +126,36 @@ __global__ void __launch_bounds__(GTHREADS) k_mbar_gram(const double *__restrict
     }
 }
 
+// u_kn from the engine's energy history (rx_mbar_create_from_history): u[i][r n_sel + j] = hist[iter[j]][r][cols[i]].  A
+// block transposes a tile of TT samples (one replica, TT consecutive selected iterations) x TT rows of u_kn through shared
+// memory: a warp reads TT states of one history row and writes TT consecutive samples of one u_kn row.  Any non-finite
+// element sets *bad.
+constexpr int TT = 32, TROWS = 8;
+__global__ void __launch_bounds__(TT * TROWS) k_mbar_gather(const double *__restrict__ hist, int R, int W,
+                                                            const long long *__restrict__ iter, int n_sel, int j_tiles,
+                                                            const int *__restrict__ cols, int K, double *__restrict__ u,
+                                                            int *__restrict__ bad) {
+    __shared__ double t[TT][TT + 1];
+    const int r = blockIdx.x / j_tiles, j0 = (blockIdx.x % j_tiles) * TT, i0 = blockIdx.y * TT;
+    const size_t N = (size_t)R * n_sel;
+    bool finite = true;
+    const int i = i0 + threadIdx.x;
+    const int col = i < K ? cols[i] : 0;
+    for (int s = threadIdx.y; s < TT; s += TROWS) {
+        const int j = j0 + s;
+        if (i < K && j < n_sel) {
+            const double v = hist[((size_t)iter[j] * R + r) * W + col];
+            finite &= isfinite(v);
+            t[s][threadIdx.x] = v;
+        }
+    }
+    __syncthreads();
+    const int j = j0 + threadIdx.x;
+    for (int s = threadIdx.y; s < TT; s += TROWS)
+        if (i0 + s < K && j < n_sel) u[(size_t)(i0 + s) * N + (size_t)r * n_sel + j] = t[threadIdx.x][s];
+    if (!finite) atomicExch(bad, 1);
+}
+
 // One level of the fixed pairwise tree over chunk records of len doubles: rec[c] += rec[c + half] for c < n - half.
 __global__ void k_mbar_tree(double *__restrict__ rec, size_t len, int n, int half) {
     const size_t total = (size_t)(n - half) * len;
@@ -225,11 +255,11 @@ void unpack_gram(const rx_mbar *h, double *G) {
 
 extern "C" const char *rx_mbar_last_error(const rx_mbar *h) { return h ? h->err.c_str() : g_mbar_create_error.c_str(); }
 
-extern "C" int rx_mbar_create(int32_t K, int64_t N, const double *u_kn, const int64_t *N_k, rx_mbar **out) {
 #define MBAR_CREATE_FAIL(code, msg) do { g_mbar_create_error = (msg); return (code); } while (0)
-    if (!out) MBAR_CREATE_FAIL(RX_ERR_INVALID, "out is NULL");
-    *out = nullptr;
-    if (K < 1 || N < 1 || !u_kn || !N_k) MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create: need K >= 1, N >= 1, u_kn and N_k");
+
+// A handle with every device buffer allocated on the current device; u_kn still to be filled.  `extra` bytes of the
+// caller's are part of the free-memory check.
+static int mbar_alloc(int32_t K, int64_t N, const int64_t *N_k, size_t extra, std::unique_ptr<rx_mbar> &out) {
     long long total = 0;
     for (int k = 0; k < K; ++k) {
         if (N_k[k] < 0) MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create: N_k must be non-negative");
@@ -249,7 +279,7 @@ extern "C" int rx_mbar_create(int32_t K, int64_t N, const double *u_kn, const in
     h->gram_chunks = (int)((N + h->gram_chunk - 1) / h->gram_chunk);
     const size_t bytes = (size_t)K * N * sizeof(double) + (size_t)N * sizeof(double) +
                          (size_t)h->row_chunks * (K + 1) * sizeof(double) +
-                         (size_t)h->gram_chunks * h->n_pairs * GT * GT * sizeof(double);
+                         (size_t)h->gram_chunks * h->n_pairs * GT * GT * sizeof(double) + extra;
     if (cudaGetDevice(&h->device) != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: no CUDA device");
     size_t free_b = 0, total_b = 0;
     if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: cudaMemGetInfo failed");
@@ -272,8 +302,6 @@ extern "C" int rx_mbar_create(int32_t K, int64_t N, const double *u_kn, const in
         MBAR_CREATE_FAIL(RX_ERR_UNSUPPORTED, "rx_mbar_create: out of device memory for u_kn and its reduction buffers");
     }
     if (e != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, std::string("rx_mbar_create: ") + cudaGetErrorString(e));
-    if (cudaMemcpy(h->d_u, u_kn, (size_t)K * N * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess)
-        MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: upload of u_kn failed");
     h->logN.resize(K);
     h->Nk.resize(K);
     for (int k = 0; k < K; ++k) {
@@ -282,10 +310,71 @@ extern "C" int rx_mbar_create(int32_t K, int64_t N, const double *u_kn, const in
     }
     h->h_rows.resize(K + 1);
     h->h_gram.resize((size_t)h->n_pairs * GT * GT);
+    out = std::move(h);
+    return RX_OK;
+}
+
+extern "C" int rx_mbar_create_from_history(rx_engine *e, int32_t K, int64_t n_sel, const int64_t *iterations,
+                                           const int32_t *columns, const int64_t *N_k, rx_mbar **out) {
+    if (!out) MBAR_CREATE_FAIL(RX_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (!e || K < 1 || n_sel < 1 || !iterations || !columns || !N_k)
+        MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create_from_history: need an engine, K >= 1, n_sel >= 1, iterations, "
+                                         "columns and N_k");
+    const int R = e->cfg.n_replicas, W = e->cfg.n_states + e->hist_u;
+    for (int64_t j = 0; j < n_sel; ++j)
+        if (iterations[j] < 0 || iterations[j] >= e->hist_len)
+            MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create_from_history: iteration " + std::to_string(iterations[j]) +
+                                                 " is not in the history of " + std::to_string(e->hist_len));
+    for (int i = 0; i < K; ++i)
+        if (columns[i] < 0 || columns[i] >= W)
+            MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create_from_history: column " + std::to_string(columns[i]) +
+                                                 " is not in a history row of " + std::to_string(W));
+    const int64_t N = (int64_t)R * n_sel;
+    const int j_tiles = (int)((n_sel + TT - 1) / TT);
+    if ((long long)R * j_tiles > INT32_MAX || (K + TT - 1) / TT > 65535)
+        MBAR_CREATE_FAIL(RX_ERR_UNSUPPORTED, "rx_mbar_create_from_history: too many samples or states for one gather");
+    if (cudaSetDevice(e->cfg.device) != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create_from_history: cudaSetDevice failed");
+    std::unique_ptr<rx_mbar> h;
+    int rc = mbar_alloc(K, N, N_k, n_sel * sizeof(long long) + K * sizeof(int) + sizeof(int), h);
+    if (rc) return rc;
+    DevBuf<long long> d_iter;
+    DevBuf<int> d_cols, d_bad;
+    cudaError_t c = d_iter.alloc(n_sel);
+    if (c == cudaSuccess) c = d_cols.alloc(K);
+    if (c == cudaSuccess) c = d_bad.alloc(1);
+    // the engine's appends are queued on its stream
+    if (c == cudaSuccess) c = cudaStreamSynchronize(e->stream);
+    if (c == cudaSuccess) c = cudaMemcpyAsync(d_iter, iterations, n_sel * sizeof(long long), cudaMemcpyHostToDevice, h->stream);
+    if (c == cudaSuccess) c = cudaMemcpyAsync(d_cols, columns, K * sizeof(int), cudaMemcpyHostToDevice, h->stream);
+    if (c == cudaSuccess) c = cudaMemsetAsync(d_bad, 0, sizeof(int), h->stream);
+    if (c == cudaSuccess) {
+        k_mbar_gather<<<dim3(R * j_tiles, (K + TT - 1) / TT), dim3(TT, TROWS), 0, h->stream>>>(
+            e->d_hist, R, W, d_iter, (int)n_sel, j_tiles, d_cols, K, h->d_u, d_bad);
+        c = cudaGetLastError();
+    }
+    int bad = 0;
+    if (c == cudaSuccess) c = cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+    if (c == cudaSuccess) c = cudaStreamSynchronize(h->stream);
+    if (c != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, std::string("rx_mbar_create_from_history: ") + cudaGetErrorString(c));
+    if (bad) MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create_from_history: u_kn must be finite");
     *out = h.release();
     return RX_OK;
-#undef MBAR_CREATE_FAIL
 }
+
+extern "C" int rx_mbar_create(int32_t K, int64_t N, const double *u_kn, const int64_t *N_k, rx_mbar **out) {
+    if (!out) MBAR_CREATE_FAIL(RX_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (K < 1 || N < 1 || !u_kn || !N_k) MBAR_CREATE_FAIL(RX_ERR_INVALID, "rx_mbar_create: need K >= 1, N >= 1, u_kn and N_k");
+    std::unique_ptr<rx_mbar> h;
+    int rc = mbar_alloc(K, N, N_k, 0, h);
+    if (rc) return rc;
+    if (cudaMemcpy(h->d_u, u_kn, (size_t)K * N * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess)
+        MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: upload of u_kn failed");
+    *out = h.release();
+    return RX_OK;
+}
+#undef MBAR_CREATE_FAIL
 
 extern "C" void rx_mbar_destroy(rx_mbar *h) { delete h; }
 

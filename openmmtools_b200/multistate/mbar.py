@@ -70,6 +70,29 @@ class MBAR:
         h = C.c_void_p()
         K, N = self.u_kn.shape
         _check(self._lib, None, self._lib.rx_mbar_create(K, N, _ptr(self.u_kn), _ptr(self.N_k), C.byref(h)))
+        self._start(h, initial_f_k, maximum_iterations, relative_tolerance)
+
+    @classmethod
+    def from_history(cls, engine, iterations, columns, N_k, initial_f_k=None, maximum_iterations=10000,
+                     relative_tolerance=1.0e-12):
+        """MBAR of u_kn gathered on the device from ``engine``'s energy history (Engine.history_append), with no host
+        copy: row i of u_kn is history column ``columns[i]`` (the sampled states 0..M-1, then the unsampled ones), and
+        column r * n + j is replica r at iteration ``iterations[j]``, n = len(iterations).  ``u_kn`` is None."""
+        self = cls.__new__(cls)
+        self.u_kn = None
+        it = np.ascontiguousarray(iterations, dtype=np.int64)
+        cols = np.ascontiguousarray(columns, dtype=np.int32)
+        self.N_k = np.asarray(N_k, dtype=np.int64).copy()
+        if it.ndim != 1 or cols.ndim != 1 or self.N_k.shape != cols.shape:
+            raise ValueError('iterations and columns must be 1-D, and N_k as long as columns')
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        _check(self._lib, None, self._lib.rx_mbar_create_from_history(engine._h, len(cols), len(it), _ptr(it), _ptr(cols),
+                                                                       _ptr(self.N_k), C.byref(h)))
+        self._start(h, initial_f_k, maximum_iterations, relative_tolerance)
+        return self
+
+    def _start(self, h, initial_f_k, maximum_iterations, relative_tolerance):
         self._h = h
         self.n_iterations = 0
         try:

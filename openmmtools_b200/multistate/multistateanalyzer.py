@@ -26,6 +26,36 @@ class MixingStatistics(NamedTuple):
     statistical_inefficiency: float
 
 
+# The analysis steps below are shared by MultiStateSamplerAnalyzer, which reads a stored run, and the sampler's periodic
+# offline pass (MultiStateSampler._offline_analysis), which keeps the same inputs in memory: the same operations in the
+# same order give both the same bits.
+def effective_energy_timeseries(u_kt, replica_state_indices=None, log_weights=None, f_l=None):
+    """u_n = sum over replicas of u_kt [replica, iteration], each replica's reduced potential in the state it visits; with
+    the [state, iteration] log weights of a SAMS run and its latest f_l = -logZ, corrected for the changing weights
+    (:1414-1477)."""
+    u_n = np.ascontiguousarray(u_kt, dtype=np.float64).sum(0)
+    if log_weights is not None:
+        for it in range(len(u_n)):
+            st = replica_state_indices[:, it]
+            u_n[it] += -np.sum(log_weights[st, it]) + logsumexp(-f_l + log_weights[:, it])
+    return u_n
+
+
+def equilibration_data(u_n, t0, max_subset):
+    """(iterations discarded to equilibration, statistical inefficiency, effective samples) of the timeseries u_n, with
+    the origins from t0 on (:2026-2093)."""
+    i_t, g_i, n_effective_i = utils.get_equilibration_data_per_sample(u_n[t0:], max_subset=max_subset)
+    i_max = n_effective_i.argmax()
+    return i_t[i_max] + t0, g_i[i_max], n_effective_i.max()
+
+
+def decorrelated_iterations(n_equilibration, statistical_inefficiency, max_n_iterations):
+    """The production iterations n_equilibration..max_n_iterations, subsampled by the statistical inefficiency
+    (:2211-2219)."""
+    production = np.arange(n_equilibration, max_n_iterations + 1)
+    return production[utils.subsample_correlated_data(production, statistical_inefficiency)]
+
+
 class MultiStateSamplerAnalyzer:
     """MBAR analysis of a run stored by a MultiStateReporter.
 
@@ -175,15 +205,13 @@ class MultiStateSamplerAnalyzer:
         elif (energies is None) != (replica_state_indices is None):
             raise ValueError('energies and replica_state_indices must be given together')
         n_replicas, _, n_iterations = energies.shape
-        u_n = energies[np.arange(n_replicas)[:, None], replica_state_indices, np.arange(n_iterations)[None, :]].sum(0)
+        u_kt = energies[np.arange(n_replicas)[:, None], replica_state_indices, np.arange(n_iterations)[None, :]]
+        log_weights = f_l = None
         if self.has_log_weights:
             data = self._reporter.read_online_analysis_data(slice(None), 'log_weights', 'logZ')
             log_weights = np.moveaxis(np.asarray(data['log_weights']), 0, -1)
             f_l = -np.asarray(data['logZ'])[-1]
-            for it in range(n_iterations):
-                st = replica_state_indices[:, it]
-                u_n[it] += -np.sum(log_weights[st, it]) + logsumexp(-f_l + log_weights[:, it])
-        return u_n
+        return effective_energy_timeseries(u_kt, replica_state_indices, log_weights, f_l)
 
     def _get_equilibration_data(self, energies=None, neighborhoods=None, replica_state_indices=None):
         """(iterations discarded to equilibration, statistical inefficiency, effective samples) (:2026-2093)."""
@@ -200,11 +228,9 @@ class MultiStateSamplerAnalyzer:
                 t0 = max(t0, int(np.asarray(self._reporter.read_online_analysis_data(None, 't0')['t0']).ravel()[0]))
             except (KeyError, OSError, IndexError, ValueError):
                 pass
-            i_t, g_i, n_effective_i = utils.get_equilibration_data_per_sample(u_n[t0:], max_subset=self._max_subset)
-            i_max = n_effective_i.argmax()
-            n_effective_max = n_effective_i.max()
-            n_equilibration = i_t[i_max] + t0
-            g_t = self._statistical_inefficiency if self._statistical_inefficiency is not None else g_i[i_max]
+            n_equilibration, g_t, n_effective_max = equilibration_data(u_n, t0, self._max_subset)
+            if self._statistical_inefficiency is not None:
+                g_t = self._statistical_inefficiency
         return n_equilibration, g_t, n_effective_max
 
     @property
@@ -233,8 +259,7 @@ class MultiStateSamplerAnalyzer:
         """Indices of the iterations MBAR uses, up to max_n_iterations (:2211-2219)."""
         if self.use_full_trajectory:
             return np.arange(self.max_n_iterations + 1, dtype=int)
-        production = np.arange(self.n_equilibration_iterations, self.max_n_iterations + 1)
-        return production[utils.subsample_correlated_data(production, self.statistical_inefficiency)]
+        return decorrelated_iterations(self.n_equilibration_iterations, self.statistical_inefficiency, self.max_n_iterations)
 
     @staticmethod
     def reformat_energies_for_mbar(u_kln, n_k=None):

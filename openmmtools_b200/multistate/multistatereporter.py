@@ -20,6 +20,7 @@ Only rank 0 writes (as in the reference, multistatesampler.py:1169-1187).
 """
 import json
 import os
+import re
 import shutil
 import pickle
 import numpy as np
@@ -47,6 +48,7 @@ class MultiStateReporter:
         self._open_mode = None
         self._meta = None
         self._dirty = set()
+        self._overwrite_statistics = False
         if open_mode is not None:
             self.open(open_mode)
 
@@ -99,6 +101,7 @@ class MultiStateReporter:
                 os.makedirs(os.path.join(self._storage, sub))
             self._meta = {'convention': convention, 'dicts': {}}
             self._write_meta()
+            self._overwrite_statistics = True    # a fresh run starts a new real-time statistics file
         else:
             if not self.storage_exists():
                 raise IOError('storage {} does not exist'.format(self._storage))
@@ -294,6 +297,27 @@ class MultiStateReporter:
         """multistatereporter.py:1341-1351"""
         self.write_online_analysis_data(None, **kwargs)
         self.write_online_analysis_data(iteration, **kwargs)
+
+    @property
+    def real_time_statistics_path(self):
+        """``<storage stem>_real_time_analysis.yaml`` next to the storage (multistatereporter.py:1353-1379)."""
+        directory, name = os.path.split(os.path.normpath(self._storage))
+        return os.path.join(directory, os.path.splitext(name)[0] + '_real_time_analysis.yaml')
+
+    def write_current_statistics(self, data):
+        """Append one entry to the real-time statistics file, a YAML list with one entry per offline analysis pass
+        (multistatereporter.py:1353-1379); the first write of a fresh run truncates it.  Each entry is one line
+        ``- {json}``, which is YAML; non-finite numbers are written as YAML's .inf / -.inf / .nan."""
+        path = self.real_time_statistics_path
+        if self._overwrite_statistics:
+            if os.path.exists(path):
+                os.remove(path)
+            self._overwrite_statistics = False
+        line = json.dumps(_jsonable(data), allow_nan=True)
+        line = re.sub(r'(?<![\w."])(-?)Infinity\b', r'\1.inf', line)
+        line = re.sub(r'(?<![\w."])NaN\b', '.nan', line)
+        with open(path, 'a') as f:
+            f.write('- ' + line + '\n')
 
     def read_online_analysis_data(self, iteration, *keys):
         out = {}

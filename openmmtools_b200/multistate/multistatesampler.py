@@ -9,8 +9,9 @@ replicas, the K x M energy matrix, the replica->state map, the swap statistics),
 kernel launches, and ``sampler_states`` are materialised on the host only when asked for (or every iteration with
 ``host_resident_states=True``, which reproduces the reference's per-iteration host round trip).  Storage goes
 through :class:`MultiStateReporter` (a netCDF4-free container with the reference's variable names; checkpoints also
-carry the RNG positions, so a resumed run is bit-identical to an uninterrupted one).  Online MBAR analysis and
-minimisation are outside the hot path (SURVEY.md section 8f).
+carry the RNG positions, so a resumed run is bit-identical to an uninterrupted one).  Minimisation is outside the hot
+path (SURVEY.md section 8f).  The periodic offline MBAR pass of a run with storage reads the energy matrices from a
+history the engine keeps on the device (DESIGN §4.8), not from storage.
 
 Multi-GPU: one process per GPU (torchrun style: RANK / WORLD_SIZE / LOCAL_RANK); replicas are sharded in contiguous
 blocks, energy rows are all-gathered with NCCL, mixing is replicated from identical generator state.
@@ -19,6 +20,7 @@ import collections
 import copy
 import logging
 import os
+import struct
 import time
 import numpy as np
 from .. import unit, mcmc, states, _backend, _lib
@@ -26,6 +28,8 @@ from .._engine import EngineError, scale_mask
 from ..cache import ContextCache
 from .utils import SimulationNaNError
 from .multistatereporter import MultiStateReporter
+from .mbar import MBAR, MBARConvergenceError
+from .multistateanalyzer import effective_energy_timeseries, equilibration_data, decorrelated_iterations
 
 logger = logging.getLogger(__name__)
 
@@ -70,6 +74,9 @@ class MultiStateSampler:
         self.locality = locality
         self._last_mbar_f_k = None
         self._last_err_free_energy = None
+        self._last_mbar_f_k_offline = None
+        self._offline_inputs = None        # rank 0: the host inputs of the offline pass, one entry per iteration
+        self._offline_stopped = False      # the energy history could not grow: no more offline passes in this run
         self.host_resident_states = host_resident_states
         self.energy_context_cache = ContextCache()
         self.sampler_context_cache = ContextCache()
@@ -187,9 +194,19 @@ class MultiStateSampler:
         iteration = reporter.read_last_iteration(last_checkpoint=False)
         n_it = options.get('number_of_iterations')
         n_it = np.inf if n_it == 'inf' else n_it
+        target = options.get('online_analysis_target_error', 0.0)
+        target_error = last_err = None
+        # the error of the last offline pass counts only when online analysis runs and the target is a stopping condition
+        if options.get('online_analysis_interval') is not None and target != 0.0:
+            target_error = target
+            try:
+                last_err = float(reporter.read_online_analysis_data(None, 'free_energy')['free_energy'][1])
+            except (KeyError, OSError, IndexError, ValueError):
+                last_err = np.inf
         if not was_open:
             reporter.close()
-        return cls.Status(iteration=iteration, target_error=None, is_completed=(n_it is not None and iteration >= n_it))
+        is_completed = n_it is not None and cls._is_completed_static(n_it, iteration, last_err, target)
+        return cls.Status(iteration=iteration, target_error=target_error, is_completed=is_completed)
 
     def _restore_sampler_from_reporter(self, reporter):
         metadata = reporter.read_dict('metadata')
@@ -246,6 +263,37 @@ class MultiStateSampler:
             if n:
                 self._engine.mix_skip(n, stream)
         self._equil_counter = int(extra.get('equil_counter', 0))
+        self._restore_offline_analysis(reporter, int(checkpoint))
+
+    def _restore_offline_analysis(self, reporter, checkpoint):
+        """The offline pass of the checkpoint iteration's state: its error and the last f_k_offline up to the checkpoint
+        (where the reference restarts from zeros; these keep the stored free energies of a resumed run bit-identical to an
+        uninterrupted run's), and on rank 0 its inputs: the stored energies of iterations 0..checkpoint, read once."""
+        try:
+            self._last_err_free_energy = float(reporter.read_online_analysis_data(checkpoint, 'free_energy')['free_energy'][1])
+        except (KeyError, IndexError, OSError):
+            self._last_err_free_energy = None
+        try:
+            f = np.asarray(reporter.read_online_analysis_data(slice(0, checkpoint + 1), 'f_k_offline')['f_k_offline'])
+            done = np.flatnonzero(np.any(f != 0, axis=1))      # (iterations without a pass hold zeros)
+            self._last_mbar_f_k_offline = f[done[-1]].copy() if len(done) else None
+        except (KeyError, OSError):
+            self._last_mbar_f_k_offline = None
+        if not self._keeps_offline_inputs:
+            return
+        e, _, unsampled = reporter.read_energies(slice(0, checkpoint + 1))
+        st = reporter.read_replica_thermodynamic_states(slice(0, checkpoint + 1))
+        try:
+            lw = np.asarray(reporter.read_online_analysis_data(slice(0, checkpoint + 1), 'log_weights')['log_weights'])
+        except (KeyError, OSError):
+            lw = None
+        try:
+            self._engine.history_load(e, unsampled if unsampled.shape[-1] else None)
+        except EngineError as err:
+            self._stop_offline_analysis(err)
+            return
+        diag = e[np.arange(len(e))[:, None], np.arange(e.shape[1])[None, :], st]
+        self._offline_inputs = {'u': list(diag), 'states': list(st), 'log_weights': None if lw is None else list(lw)}
 
     # ------------------------------------------------------------------ create (multistatesampler.py:537-609)
     def create(self, thermodynamic_states, sampler_states, storage=None, initial_thermodynamic_states=None,
@@ -594,6 +642,7 @@ class MultiStateSampler:
             if self._reporter is not None and self._rank == 0:      # multistatesampler.py:741-746
                 self._reporter.write_energies(self._energy_thermodynamic_states, self._neighborhoods,
                                               self._energy_unsampled_states, 0)
+            self._record_offline_inputs()
             self._check_nan_energy()
         iteration_limit = self.number_of_iterations if n_iterations is None else \
             min(self._iteration + n_iterations, self.number_of_iterations)
@@ -609,6 +658,7 @@ class MultiStateSampler:
             self._compute_energies()
             t3 = time.time()
             self._report_iteration()
+            self._record_offline_inputs()
             self._update_analysis()
             self._update_timing(t3 - t0, time.time() - timer_start, run_initial_iteration, iteration_limit,
                                 phases=(t1 - t0, t2 - t1, t3 - t2))
@@ -928,17 +978,144 @@ class MultiStateSampler:
         return self._last_err_free_energy
 
     def _update_analysis(self):
-        """multistatesampler.py:1676-1695.  The cheap online estimate runs every iteration; the periodic offline MBAR
-        pass of the reference (MultiStateSamplerAnalyzer, every ``online_analysis_interval`` iterations) is outside
-        the hot path and not run, so the error estimate stays +inf and never ends a run early."""
+        """multistatesampler.py:1676-1695.  The online estimate runs every iteration and sets the error to +inf; every
+        ``online_analysis_interval`` iterations of a run with storage, the offline MBAR pass sets it to the standard error
+        of the free energy between the end states, so a run can stop only at those iterations.  Rank 0 runs the pass and
+        every rank gets its error, so that all stop at the same iteration.  Runs with ``locality`` have no pass (MBAR of
+        them is not implemented)."""
         if self.online_analysis_interval is None:
             return
         self._last_err_free_energy = self._online_analysis()
+        if self._iteration % self.online_analysis_interval != 0 or self._reporter is None or self.locality is not None:
+            return
+        err = self._offline_analysis() if self._rank == 0 and self._offline_inputs is not None else None
+        if self._world_size > 1:
+            err = self._bcast_error(err)
+        if err is not None:
+            self._last_err_free_energy = err
+
+    @property
+    def _keeps_offline_inputs(self):
+        return (self._rank == 0 and self._reporter is not None and self.locality is None
+                and self.online_analysis_interval is not None and not self._offline_stopped)
+
+    def _log_weights_and_logZ(self):
+        """Hook: (log weights, logZ) of a sampler whose state weights change during the run (SAMS), else None."""
+        return None
+
+    def _stop_offline_analysis(self, err):
+        if err.code != _lib.RX_ERR_UNSUPPORTED:
+            raise err
+        logger.warning('offline free-energy analysis stops for the rest of this run: %s', err.message)
+        self._offline_stopped = True
+        self._offline_inputs = None
+
+    def _record_offline_inputs(self):
+        """What the offline pass needs of the iteration just reported (rank 0 of a run with storage): the energy matrices
+        go to the engine's device history; the host keeps u[r, s_r(t)] of the K replicas, their states and, for SAMS, the
+        log weights."""
+        if not self._keeps_offline_inputs:
+            return
+        it = self._iteration
+        rec = self._offline_inputs
+        if it == 0 or rec is None:
+            rec = self._offline_inputs = {'u': [], 'states': [], 'log_weights': None}
+        if it > len(rec['u']):
+            # iterations ran without reports (run_fused): the history has a gap the analyzer of the storage would not see
+            logger.warning('offline free-energy analysis stops for the rest of this run: iterations %d..%d were not '
+                           'reported', len(rec['u']), it - 1)
+            self._offline_stopped = True
+            self._offline_inputs = None
+            return
+        try:
+            self._engine.history_append(it, len(self._unsampled_states))
+        except EngineError as err:
+            self._stop_offline_analysis(err)
+            return
+        st = np.array(self._replica_thermodynamic_states, dtype=np.int64)
+        del rec['u'][it:], rec['states'][it:]
+        rec['u'].append(self._energy_thermodynamic_states[np.arange(len(st)), st])
+        rec['states'].append(st)
+        lw = self._log_weights_and_logZ()
+        if lw is not None:
+            if rec['log_weights'] is None:
+                rec['log_weights'] = []
+            del rec['log_weights'][it:]
+            rec['log_weights'].append(np.array(lw[0], dtype=np.float64))
+
+    def _offline_analysis(self):
+        """The reference's offline pass (multistatesampler.py:1526-1620): the decisions of MultiStateSamplerAnalyzer
+        (effective-energy timeseries, equilibration, subsampling, initial_f_k = the previous pass's f_k) on iterations
+        0..t, from the inputs kept in memory; MBAR's u_kn is gathered on the device from the engine's energy history.
+        Returns the standard error of Delta f between the end states (NaN becomes +inf), or None when MBAR fails (then
+        nothing is written and the previous error stands)."""
+        rec = self._offline_inputs
+        it = self._iteration
+        M, U = self.n_states, len(self._unsampled_states)
+        if self._last_mbar_f_k_offline is None:
+            self._last_mbar_f_k_offline = np.zeros(M + U)
+        try:
+            states = np.stack(rec['states'], axis=1)
+            log_weights, f_l = None, None
+            lw = self._log_weights_and_logZ()
+            if lw is not None:
+                log_weights, f_l = np.stack(rec['log_weights'], axis=1), -np.asarray(lw[1], dtype=np.float64)
+            u_n = effective_energy_timeseries(np.stack(rec['u'], axis=1), states, log_weights, f_l)
+            # t0 = 1: iteration 0 is discarded.  SAMS stores its t0 per iteration, not as the static record the analyzer
+            # looks for, so the analyzer starts at 1 as well.
+            n_equilibration, g_t, n_effective = equilibration_data(u_n, 1, 100)
+            selected = decorrelated_iterations(n_equilibration, g_t, it)
+            first = U // 2          # the unsampled states at both ends, as MultiStateSamplerAnalyzer lays out u_kn
+            columns = np.zeros(M + U, dtype=np.int32)
+            columns[first:first + M] = np.arange(M)
+            if U > 0:
+                columns[[0, -1]] = (M, M + U - 1)
+            N_k = np.zeros(M + U, dtype=np.int64)
+            visited, counts = np.unique(states[:, selected], return_counts=True)
+            N_k[first + visited] = counts
+            mbar = MBAR.from_history(self._engine, selected, columns, N_k, initial_f_k=self._last_mbar_f_k_offline)
+            try:
+                r = mbar.compute_free_energy_differences()
+            finally:
+                mbar.close()
+        except (MBARConvergenceError, ValueError) as err:
+            logger.debug('offline free-energy analysis at iteration %d failed: %s', it, err)
+            return None
+        self._last_mbar_f_k_offline = mbar.f_k
+        free_energy, err = float(r['Delta_f'][0, -1]), float(r['dDelta_f'][0, -1])
+        if np.isnan(err):
+            err = np.inf
+        self._reporter.write_online_data_dynamic_and_static(it, f_k_offline=self._last_mbar_f_k_offline,
+                                                            free_energy=np.array([free_energy, err]))
+        self._reporter.write_current_statistics({
+            'iteration': it, 'percent_complete': it * 100 / self.number_of_iterations,
+            'mbar_analysis': {'free_energy_in_kT': free_energy, 'standard_error_in_kT': err,
+                              'number_of_uncorrelated_samples': float(n_effective),
+                              'n_equilibrium_iterations': int(n_equilibration),
+                              'statistical_inefficiency': float(g_t)},
+            'timing_data': self._timing_data})
+        return err
+
+    def _bcast_error(self, err):
+        comm = self._communicator
+        if comm is None:
+            from .._dist import default_communicator
+            comm = self._communicator = default_communicator()
+        data = struct.pack('<d', np.nan if err is None else err) if self._rank == 0 else None
+        v = struct.unpack('<d', comm.bcast_bytes(data, 8))[0]
+        return None if np.isnan(v) else v
 
     def _is_completed(self, iteration_limit=None):
         if iteration_limit is None:
             iteration_limit = self.number_of_iterations
-        return self._iteration is not None and self._iteration >= iteration_limit
+        return self._iteration is not None and self._is_completed_static(
+            iteration_limit, self._iteration, self._last_err_free_energy, self.online_analysis_target_error)
+
+    @staticmethod
+    def _is_completed_static(iteration_limit, iteration, last_err_free_energy, online_analysis_target_error):
+        """multistatesampler.py:1722-1739: the iteration limit is reached, or the last error is at or below the target."""
+        return iteration >= iteration_limit or (
+            last_err_free_energy is not None and last_err_free_energy <= online_analysis_target_error)
 
     def _check_nan_energy(self):
         """multistatesampler.py:1049-1081"""

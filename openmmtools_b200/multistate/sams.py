@@ -260,6 +260,9 @@ class SAMSSampler(MultiStateSampler):
                                                       stage=np.array([self._stage]), t0=np.array([self._t0]),
                                                       histogram=self._cached_state_histogram)
 
+    def _log_weights_and_logZ(self):
+        return self.log_weights, self._logZ
+
     def _checkpoint_extra(self):
         e = super()._checkpoint_extra()
         st = self._rng.get_state()

@@ -43,4 +43,12 @@ ss_ = multistate.SAMSSampler(mcmc_moves=mcmc.LangevinSplittingDynamicsMove(n_ste
                              flatness_criteria='minimum-visits', device_weight_update=True)
 ss_.create([states.ThermodynamicState(ho.system, T * unit.kelvin) for T in (300, 310, 320)], [states.SamplerState(ho.positions)] * 2)
 ss_.run(6); ss_.run_fused(4)
+# energy history and the u_kn gather (k_mbar_gather): partial tiles in both directions, two unsampled columns
+from openmmtools_b200.multistate.mbar import MBAR
+e = Engine(0, 7, 40)
+rng = np.random.default_rng(0)
+e.history_load(rng.normal(size=(50, 7, 40)), rng.normal(size=(50, 7, 2)))
+N_k = np.zeros(42, np.int64); N_k[1:8] = 37
+MBAR.from_history(e, np.arange(3, 40), np.r_[40, np.arange(40), 41], N_k).close()
+e.close()
 print('sanitize workload done')
