@@ -440,17 +440,23 @@ RX_API int rx_comm_init(rx_engine *h, const char *nccl_library_path, const void 
  * Independent of any engine: the two passes of each Newton iteration of an MBAR solve (multistateanalyzer.py:1038-1058
  * hands u_kn to pymbar.MBAR there).  With c_k = log N_k + f_k (c_k = -inf for N_k = 0):
  *   log D_n = logsumexp_k (c_k - u_kn),  W_in = exp(f_i - u_in - log D_n).
- * Results are reduced in chunks fixed by K and N and added by a fixed pairwise tree: the same inputs give the same bits
- * on every call and for every rx_mbar_set_max_blocks.  Calls use the device that was current at rx_mbar_create.
+ * At creation every sample is shifted on the device by m_n = min over the sampled states of u_kn; f, W and every output
+ * below are those of the unshifted u_kn, computed without the rounding of large |u|.  Sums over samples of W are taken
+ * in log space, so they are exact to rounding at any energy scale.
+ * Results are reduced in chunks fixed by K and N and combined by a fixed pairwise tree: the same inputs give the same
+ * bits on every call and for every rx_mbar_set_max_blocks.  Calls use the device that was current at rx_mbar_create.
  *
  * rx_mbar_create    uploads u_kn (f64, row-major [K][N]) and N_k [K] (sum N_k = N, zeros allowed).  The size of the
  *                   device buffers is checked before u_kn is read: RX_ERR_UNSUPPORTED when they do not fit in the free
  *                   device memory.
  * rx_mbar_evaluate  at f_k [K]: logden_sum = sum_n log D_n; grad[i] = N_i - N_i sum_n W_in (the gradient of the
- *                   log-likelihood sum_k N_k f_k - sum_n log D_n); hess [K][K] = N_i N_j sum_n W_in W_jn
- *                   - delta_ij N_i sum_n W_in (its Hessian).  Any output may be NULL; hess = NULL skips the K x K pass.
+ *                   log-likelihood sum_k N_k f_k - sum_n log D_n), computed as -N_i expm1(log sum_n W_in);
+ *                   hess [K][K] = N_i N_j sum_n W_in W_jn - delta_ij N_i sum_n W_in (its Hessian).  grad and the rows
+ *                   and columns of hess of states with N_i = 0 are 0.  Any output may be NULL; hess = NULL skips the
+ *                   K x K pass.
  * rx_mbar_gram      G [K][K] = sum_n W_in W_jn at f_k (W^T W of the N x K weight matrix) and, unless NULL,
- *                   wsum [K] = sum_n W_in.
+ *                   wsum [K] = sum_n W_in = exp(log sum_n W_in) (0 or inf where that is out of range).
+ * rx_mbar_get_log_wsum  log sum_n W_in [K] of the last evaluate or gram call: finite for every state at any f_k.
  * rx_mbar_get_logden  log D_n [N] of the last evaluate or gram call.
  * rx_mbar_set_max_blocks  caps the blocks of every launch (0: chosen from the device); results do not change. */
 typedef struct rx_mbar rx_mbar;
@@ -460,6 +466,7 @@ RX_API const char *rx_mbar_last_error(const rx_mbar *h);   /* h = NULL: the last
 RX_API int rx_mbar_evaluate(rx_mbar *h, const double *f_k, double *logden_sum, double *grad, double *hess);
 RX_API int rx_mbar_gram(rx_mbar *h, const double *f_k, double *G, double *wsum);
 RX_API int rx_mbar_get_logden(rx_mbar *h, double *logD);
+RX_API int rx_mbar_get_log_wsum(rx_mbar *h, double *log_wsum);
 RX_API int rx_mbar_set_max_blocks(rx_mbar *h, int32_t max_blocks);
 
 /* ---- energy history: the energy matrices of a run, kept on the device for MBAR ------------------------------------

@@ -29,7 +29,7 @@ SYMBOLS = [
     'rx_set_hmc_integrator', 'rx_set_state_hmc_integrator', 'rx_get_hmc_statistics', 'rx_set_hmc_statistics',
     'rx_get_hmc_energies',
     'rx_mbar_create', 'rx_mbar_destroy', 'rx_mbar_last_error', 'rx_mbar_evaluate', 'rx_mbar_gram', 'rx_mbar_get_logden',
-    'rx_mbar_set_max_blocks',
+    'rx_mbar_set_max_blocks', 'rx_mbar_get_log_wsum',
     'rx_history_append', 'rx_history_truncate', 'rx_history_load', 'rx_history_reserve', 'rx_history_length',
     'rx_mbar_create_from_history',
 ]
@@ -184,6 +184,7 @@ def load():
     lib.rx_mbar_gram.argtypes = [vp, vp, vp, vp]
     lib.rx_mbar_get_logden.argtypes = [vp, vp]
     lib.rx_mbar_set_max_blocks.argtypes = [vp, i32]
+    lib.rx_mbar_get_log_wsum.argtypes = [vp, vp]
     lib.rx_history_append.argtypes = [vp, i64, i32]
     lib.rx_history_truncate.argtypes = [vp, i64]
     lib.rx_history_load.argtypes = [vp, i64, i32, vp, vp]

@@ -1,10 +1,13 @@
 // rx_mbar.cu -- the two passes of an MBAR solve over a device-resident reduced-potential matrix (DESIGN §4.7).
 //
 // Shirts & Chodera 2008: with c_k = log N_k + f_k, the density of sample n is log D_n = logsumexp_k (c_k - u_kn) and its
-// weight in state i is W_in = exp(f_i - u_in - log D_n).  Pass 1 (k_mbar_logden) writes log D_n; pass 2 reduces W over
-// the samples: k_mbar_rowsum gives sum_n W_in and sum_n log D_n, k_mbar_gram gives sum_n W_in W_jn.  Every reduction is
-// cut into chunks of samples whose number depends on K and N only; a chunk is summed by one block in a fixed order and
-// the chunks are then added by a fixed pairwise tree (k_mbar_tree), so results do not depend on the grid.
+// weight in state i is W_in = exp(f_i - u_in - log D_n).  At creation k_mbar_shift subtracts m_n = min over the sampled
+// states of u_kn from every sample: W is unchanged, and exp's argument no longer carries the rounding of |u| ~ 1e5 kT.
+// Pass 1 (k_mbar_logden) writes log D_n of the shifted u; pass 2 reduces W over the samples: k_mbar_rowsum gives
+// log sum_n W_in (a log-sum-exp, so it neither underflows nor overflows at any energy scale) and sum_n log D_n,
+// k_mbar_gram gives sum_n W_in W_jn.  Every reduction is cut into chunks of samples whose number depends on K and N only;
+// a chunk is summed by one block in a fixed order and the chunks are then combined by a fixed pairwise tree
+// (k_mbar_tree, k_mbar_tree_rows), so results do not depend on the grid.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <string.h>
@@ -46,6 +49,12 @@ __global__ void k_mbar_logden(const double *__restrict__ u, size_t N, int K, con
     }
 }
 
+// (m, s) += (m2, s2) for running log-sum-exps m + log s; (-inf, 0) is the empty sum.  One exp per call.
+__device__ __forceinline__ void lse_add(double &m, double &s, double m2, double s2) {
+    if (m2 > m) { s = s * exp(m - m2) + s2; m = m2; }   // s = 0 while m = -inf, so exp(-inf) = 0 adds nothing
+    else if (m2 != -INFINITY) s += s2 * exp(m2 - m);
+}
+
 // sum over a block of RTHREADS in a fixed order
 __device__ double block_sum(double v, double *sh) {
     sh[threadIdx.x] = v;
@@ -59,20 +68,57 @@ __device__ double block_sum(double v, double *sh) {
     return r;
 }
 
-// Pass 2a: work item (row r, chunk c) -> part[c * (K + 1) + r] = sum over the chunk's samples of W_rn (r < K) or of
-// log D_n (r = K).  Each thread sums a strided subsequence of the chunk in order, then the block adds the threads.
+// (m, s) log-sum-exp over a block of RTHREADS in the same fixed order; the result is in (m, s) of thread 0
+__device__ void block_lse(double &m, double &s, double *shm, double *shs) {
+    shm[threadIdx.x] = m;
+    shs[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = RTHREADS / 2; o > 0; o >>= 1) {
+        if (threadIdx.x < o) {
+            double a = shm[threadIdx.x], b = shs[threadIdx.x];
+            lse_add(a, b, shm[threadIdx.x + o], shs[threadIdx.x + o]);
+            shm[threadIdx.x] = a;
+            shs[threadIdx.x] = b;
+        }
+        __syncthreads();
+    }
+    m = shm[0];
+    s = shs[0];
+    __syncthreads();
+}
+
+// Pass 2a: work item (row r, chunk c) -> the record pair part[c * 2 (K + 1) + 2 r ..] = (m, s) with
+// m + log s = log sum over the chunk's samples of W_rn (r < K), or (sum of log D_n - m_n, 0) for r = K.  Each thread
+// runs over a strided subsequence of the chunk in order, then the block combines the threads.
 __global__ void k_mbar_rowsum(const double *__restrict__ u, size_t N, int K, const double *__restrict__ f,
-                              const double *__restrict__ logD, int n_chunks, double *__restrict__ part) {
-    __shared__ double sh[RTHREADS];
+                              const double *__restrict__ logD, const double *__restrict__ shift, int n_chunks,
+                              double *__restrict__ part) {
+    __shared__ double shm[RTHREADS], shs[RTHREADS];
     const long long items = (long long)(K + 1) * n_chunks;
     for (long long w = blockIdx.x; w < items; w += gridDim.x) {
         const int r = (int)(w % (K + 1)), c = (int)(w / (K + 1));
         const long long n0 = (long long)c * ROW_CHUNK, n1 = min(n0 + ROW_CHUNK, (long long)N);
-        double s = 0.0;
-        for (long long n = n0 + threadIdx.x; n < n1; n += RTHREADS)
-            s += r < K ? exp(f[r] - u[(size_t)r * N + n] - logD[n]) : logD[n];
-        s = block_sum(s, sh);
-        if (threadIdx.x == 0) part[(size_t)c * (K + 1) + r] = s;
+        double m, s;
+        if (r < K) {
+            m = -INFINITY;
+            s = 0.0;
+            const double fr = f[r];
+            for (long long n = n0 + threadIdx.x; n < n1; n += RTHREADS) {
+                const double v = fr - u[(size_t)r * N + n] - logD[n];
+                if (v > m) { s = s * exp(m - v) + 1.0; m = v; }
+                else s += exp(v - m);
+            }
+            block_lse(m, s, shm, shs);
+        } else {
+            m = 0.0;
+            for (long long n = n0 + threadIdx.x; n < n1; n += RTHREADS) m += logD[n] - shift[n];
+            m = block_sum(m, shm);
+            s = 0.0;
+        }
+        if (threadIdx.x == 0) {
+            part[((size_t)c * (K + 1) + r) * 2] = m;
+            part[((size_t)c * (K + 1) + r) * 2 + 1] = s;
+        }
     }
 }
 
@@ -163,6 +209,35 @@ __global__ void k_mbar_tree(double *__restrict__ rec, size_t len, int n, int hal
         rec[e] += rec[e + (size_t)half * len];
 }
 
+// The same tree over k_mbar_rowsum's records of K + 1 pairs: pair r < K of rec[c] is log-sum-exp combined with that of
+// rec[c + half], pair K is added.
+__global__ void k_mbar_tree_rows(double *__restrict__ rec, int K, int n, int half) {
+    const size_t total = (size_t)(n - half) * (K + 1), len = 2 * (size_t)(K + 1);
+    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const size_t c = e / (K + 1), r = e % (K + 1);
+        double *a = rec + c * len + 2 * r;
+        const double *b = a + (size_t)half * len;
+        if (r < (size_t)K) lse_add(a[0], a[1], b[0], b[1]);
+        else a[0] += b[0];
+    }
+}
+
+// One thread per sample: m_n = min over the sampled states (c_k = log N_k > -inf) of u_kn, then u_kn -= m_n for every
+// state, sampled or not.  MBAR's f and W are unchanged by any per-sample shift; this one makes the sampled states' u
+// at least 0 and 0 for one of them, so log D_n and exp's arguments are of the order of the spread across states
+// instead of |u|.
+__global__ void k_mbar_shift(double *__restrict__ u, size_t N, int K, const double *__restrict__ c,
+                             double *__restrict__ shift) {
+    for (long long n = blockIdx.x * (long long)blockDim.x + threadIdx.x; n < (long long)N;
+         n += (long long)gridDim.x * blockDim.x) {
+        double m = INFINITY;
+        for (int k = 0; k < K; ++k)
+            if (c[k] != -INFINITY) m = fmin(m, u[(size_t)k * N + n]);
+        for (int k = 0; k < K; ++k) u[(size_t)k * N + n] -= m;
+        shift[n] = m;
+    }
+}
+
 }  // namespace
 
 struct rx_mbar {
@@ -176,8 +251,9 @@ struct rx_mbar {
     int row_chunks = 0;          // k_mbar_rowsum chunks
     int n_tiles = 0, n_pairs = 0, gram_chunks = 0;
     long long gram_chunk = 0;    // samples per k_mbar_gram chunk (a multiple of GS)
-    DevBuf<double> d_u, d_logD, d_c, d_f, d_rows, d_gram;
-    std::vector<double> h_rows, h_gram;
+    DevBuf<double> d_u, d_logD, d_shift, d_c, d_f, d_rows, d_gram;
+    std::vector<double> h_rows, h_gram;   // h_rows: (m, s) of log sum_n W_in for i < K, then (sum_n log D_n, 0)
+    std::vector<double> log_wsum;         // log sum_n W_in of the last run
     cudaStream_t stream = nullptr;
     std::string err;
     ~rx_mbar() { if (stream) cudaStreamDestroy(stream); }
@@ -204,7 +280,20 @@ int tree(rx_mbar *h, double *rec, size_t len, int n) {
     return RX_OK;
 }
 
-// log D at f, then sum_n W_in and sum_n log D_n (h_rows) and, when gram, sum_n W_in W_jn (h_gram, upper tile pairs)
+// The K + 1 row records: (m, s) pairs of k_mbar_rowsum, combined into rec[0] by the tree.
+int tree_rows(rx_mbar *h, double *rec, int n) {
+    const int K = h->K;
+    while (n > 1) {
+        const int half = (n + 1) / 2;
+        const long long work = (long long)(n - half) * (K + 1);
+        k_mbar_tree_rows<<<blocks_for(h, (work + 255) / 256, 16), 256, 0, h->stream>>>(rec, K, n, half);
+        RX_CHECK_CUDA(h, cudaGetLastError());
+        n = half;
+    }
+    return RX_OK;
+}
+
+// log D at f, then log sum_n W_in and sum_n log D_n (h_rows, log_wsum) and, when gram, sum_n W_in W_jn (h_gram, upper tile pairs)
 int run(rx_mbar *h, const double *f, bool gram) {
     const int K = h->K;
     RX_CHECK_CUDA(h, cudaSetDevice(h->device));
@@ -219,12 +308,12 @@ int run(rx_mbar *h, const double *f, bool gram) {
                                                                                               h->d_logD);
     RX_CHECK_CUDA(h, cudaGetLastError());
     k_mbar_rowsum<<<blocks_for(h, (long long)(K + 1) * h->row_chunks, 8), RTHREADS, 0, h->stream>>>(
-        h->d_u, h->N, K, h->d_f, h->d_logD, h->row_chunks, h->d_rows);
+        h->d_u, h->N, K, h->d_f, h->d_logD, h->d_shift, h->row_chunks, h->d_rows);
     RX_CHECK_CUDA(h, cudaGetLastError());
-    int rc = tree(h, h->d_rows, K + 1, h->row_chunks);
+    int rc = tree_rows(h, h->d_rows, h->row_chunks);
     if (rc) return rc;
-    RX_CHECK_CUDA(h, cudaMemcpyAsync(h->h_rows.data(), h->d_rows, (K + 1) * sizeof(double), cudaMemcpyDeviceToHost,
-                                     h->stream));
+    RX_CHECK_CUDA(h, cudaMemcpyAsync(h->h_rows.data(), h->d_rows, 2 * (K + 1) * sizeof(double),
+                                     cudaMemcpyDeviceToHost, h->stream));
     if (gram) {
         k_mbar_gram<<<blocks_for(h, (long long)h->n_pairs * h->gram_chunks, 8), GTHREADS, 0, h->stream>>>(
             h->d_u, h->N, K, h->d_f, h->d_logD, h->n_tiles, h->n_pairs, h->gram_chunks, h->gram_chunk, h->d_gram);
@@ -235,6 +324,8 @@ int run(rx_mbar *h, const double *f, bool gram) {
                                          cudaMemcpyDeviceToHost, h->stream));
     }
     RX_CHECK_CUDA(h, cudaStreamSynchronize(h->stream));
+    // every row has N >= 1 samples, so m is finite and s >= 1
+    for (int i = 0; i < K; ++i) h->log_wsum[i] = h->h_rows[2 * i] + log(h->h_rows[2 * i + 1]);
     return RX_OK;
 }
 
@@ -277,8 +368,8 @@ static int mbar_alloc(int32_t K, int64_t N, const int64_t *N_k, size_t extra, st
     want = std::min(want, std::max(1LL, (long long)N / (2 * GS)));
     h->gram_chunk = ((N + want - 1) / want + GS - 1) / GS * GS;
     h->gram_chunks = (int)((N + h->gram_chunk - 1) / h->gram_chunk);
-    const size_t bytes = (size_t)K * N * sizeof(double) + (size_t)N * sizeof(double) +
-                         (size_t)h->row_chunks * (K + 1) * sizeof(double) +
+    const size_t bytes = (size_t)K * N * sizeof(double) + 2 * (size_t)N * sizeof(double) +
+                         (size_t)h->row_chunks * 2 * (K + 1) * sizeof(double) +
                          (size_t)h->gram_chunks * h->n_pairs * GT * GT * sizeof(double) + extra;
     if (cudaGetDevice(&h->device) != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: no CUDA device");
     size_t free_b = 0, total_b = 0;
@@ -293,9 +384,10 @@ static int mbar_alloc(int32_t K, int64_t N, const int64_t *N_k, size_t extra, st
         MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: cudaStreamCreate failed");
     cudaError_t e = h->d_u.alloc((size_t)K * N);
     if (e == cudaSuccess) e = h->d_logD.alloc(N);
+    if (e == cudaSuccess) e = h->d_shift.alloc(N);
     if (e == cudaSuccess) e = h->d_c.alloc(K);
     if (e == cudaSuccess) e = h->d_f.alloc(K);
-    if (e == cudaSuccess) e = h->d_rows.alloc((size_t)h->row_chunks * (K + 1));
+    if (e == cudaSuccess) e = h->d_rows.alloc((size_t)h->row_chunks * 2 * (K + 1));
     if (e == cudaSuccess) e = h->d_gram.alloc((size_t)h->gram_chunks * h->n_pairs * GT * GT);
     if (e == cudaErrorMemoryAllocation) {
         cudaGetLastError();
@@ -308,10 +400,21 @@ static int mbar_alloc(int32_t K, int64_t N, const int64_t *N_k, size_t extra, st
         h->Nk[k] = (double)N_k[k];
         h->logN[k] = N_k[k] > 0 ? log((double)N_k[k]) : -INFINITY;
     }
-    h->h_rows.resize(K + 1);
+    h->h_rows.resize(2 * (K + 1));
+    h->log_wsum.assign(K, NAN);
     h->h_gram.resize((size_t)h->n_pairs * GT * GT);
     out = std::move(h);
     return RX_OK;
+}
+
+// u_kn -= m_n on the handle's stream (k_mbar_shift); d_c holds log N_k until the first run
+static cudaError_t mbar_shift(rx_mbar *h) {
+    cudaError_t c = cudaMemcpyAsync(h->d_c, h->logN.data(), h->K * sizeof(double), cudaMemcpyHostToDevice, h->stream);
+    if (c != cudaSuccess) return c;
+    const long long b = std::min(((long long)h->N + 255) / 256, (long long)h->n_sm * 16);
+    k_mbar_shift<<<(int)b, 256, 0, h->stream>>>(h->d_u, h->N, h->K, h->d_c, h->d_shift);
+    c = cudaGetLastError();
+    return c == cudaSuccess ? cudaStreamSynchronize(h->stream) : c;
 }
 
 extern "C" int rx_mbar_create_from_history(rx_engine *e, int32_t K, int64_t n_sel, const int64_t *iterations,
@@ -353,6 +456,7 @@ extern "C" int rx_mbar_create_from_history(rx_engine *e, int32_t K, int64_t n_se
             e->d_hist, R, W, d_iter, (int)n_sel, j_tiles, d_cols, K, h->d_u, d_bad);
         c = cudaGetLastError();
     }
+    if (c == cudaSuccess) c = mbar_shift(h.get());
     int bad = 0;
     if (c == cudaSuccess) c = cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
     if (c == cudaSuccess) c = cudaStreamSynchronize(h->stream);
@@ -371,6 +475,7 @@ extern "C" int rx_mbar_create(int32_t K, int64_t N, const double *u_kn, const in
     if (rc) return rc;
     if (cudaMemcpy(h->d_u, u_kn, (size_t)K * N * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess)
         MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: upload of u_kn failed");
+    if (mbar_shift(h.get()) != cudaSuccess) MBAR_CREATE_FAIL(RX_ERR_CUDA, "rx_mbar_create: shift of u_kn failed");
     *out = h.release();
     return RX_OK;
 }
@@ -390,14 +495,18 @@ extern "C" int rx_mbar_evaluate(rx_mbar *h, const double *f_k, double *logden_su
     const int rc = run(h, f_k, hess != nullptr);
     if (rc) return rc;
     const int K = h->K;
-    if (logden_sum) *logden_sum = h->h_rows[K];
+    const std::vector<double> &Nk = h->Nk, &lw = h->log_wsum;
+    if (logden_sum) *logden_sum = h->h_rows[2 * K];
+    // N_i - N_i sum_n W_in = -N_i expm1(log sum_n W_in): no cancellation when the sum is far from 1.  Rows and columns of
+    // states without samples are 0 (their W at f_i = 0 may be inf).
     if (grad)
-        for (int i = 0; i < K; ++i) grad[i] = h->Nk[i] - h->Nk[i] * h->h_rows[i];
+        for (int i = 0; i < K; ++i) grad[i] = Nk[i] > 0 ? -Nk[i] * expm1(lw[i]) : 0.0;
     if (hess) {
         unpack_gram(h, hess);
         for (int i = 0; i < K; ++i) {
-            for (int j = 0; j < K; ++j) hess[(size_t)i * K + j] *= h->Nk[i] * h->Nk[j];
-            hess[(size_t)i * K + i] -= h->Nk[i] * h->h_rows[i];
+            for (int j = 0; j < K; ++j)
+                hess[(size_t)i * K + j] = Nk[i] > 0 && Nk[j] > 0 ? hess[(size_t)i * K + j] * Nk[i] * Nk[j] : 0.0;
+            if (Nk[i] > 0) hess[(size_t)i * K + i] -= Nk[i] * exp(lw[i]);
         }
     }
     return RX_OK;
@@ -409,7 +518,15 @@ extern "C" int rx_mbar_gram(rx_mbar *h, const double *f_k, double *G, double *ws
     const int rc = run(h, f_k, true);
     if (rc) return rc;
     unpack_gram(h, G);
-    if (wsum) memcpy(wsum, h->h_rows.data(), h->K * sizeof(double));
+    if (wsum)
+        for (int i = 0; i < h->K; ++i) wsum[i] = exp(h->log_wsum[i]);
+    return RX_OK;
+}
+
+extern "C" int rx_mbar_get_log_wsum(rx_mbar *h, double *log_wsum) {
+    if (!h) return RX_ERR_INVALID;
+    if (!log_wsum) RX_FAIL(h, RX_ERR_INVALID, "log_wsum is NULL");
+    memcpy(log_wsum, h->log_wsum.data(), h->K * sizeof(double));
     return RX_OK;
 }
 
@@ -417,6 +534,10 @@ extern "C" int rx_mbar_get_logden(rx_mbar *h, double *logD) {
     if (!h) return RX_ERR_INVALID;
     if (!logD) RX_FAIL(h, RX_ERR_INVALID, "logD is NULL");
     RX_CHECK_CUDA(h, cudaSetDevice(h->device));
+    // the device holds log D_n of the shifted u_kn, log D_n + m_n
+    std::vector<double> m(h->N);
     RX_CHECK_CUDA(h, cudaMemcpy(logD, h->d_logD, h->N * sizeof(double), cudaMemcpyDeviceToHost));
+    RX_CHECK_CUDA(h, cudaMemcpy(m.data(), h->d_shift, h->N * sizeof(double), cudaMemcpyDeviceToHost));
+    for (size_t n = 0; n < h->N; ++n) logD[n] -= m[n];
     return RX_OK;
 }

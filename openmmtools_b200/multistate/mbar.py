@@ -6,12 +6,16 @@ For K states with N_k samples each, and u_kn the reduced potential of sample n i
 
 equivalently they maximise the concave log-likelihood  L(f) = sum_k N_k f_k - sum_n log D_n,  whose gradient
 g_i = N_i - N_i sum_n W_in and Hessian H_ij = N_i N_j sum_n W_in W_jn - delta_ij N_i sum_n W_in use the weights
-W_in = exp(f_i - u_in) / D_n.  The device evaluates log D_n, g and H; the host takes self-consistent steps
-(f_i <- f_i - log sum_n W_in) until the relative gradient is small, then Newton steps (a K x K solve in numpy), and stops
-when max_i |g_i| / N_i <= relative_tolerance.  The gauge is f_0 = 0.
+W_in = exp(f_i - u_in) / D_n.  The device evaluates log D_n, log sum_n W_in, g and H; the host takes self-consistent
+steps (f_i <- f_i - log sum_n W_in) until the relative gradient is small, then Newton steps (a K x K solve in numpy), and
+stops when max_i |g_i| / N_i = max_i |expm1(log sum_n W_in)| <= relative_tolerance, or <= 16 eps max_i |f_i|, the
+rounding floor of that residual, where this is larger (f spread over more than ~300 kT).  A Newton step that the
+Hessian cannot give or that no backtracking makes ascend is replaced by a self-consistent step.  The gauge is f_0 = 0.  The sums of
+W are taken in log space and every sample is shifted by its lowest sampled energy on the device, so states tens to
+thousands of kT apart and energies of |u| ~ 1e5 kT solve as well as energies of order 1 kT.
 
 States without samples (N_k = 0) take no part in D_n; their f_k follow from the converged f of the others by the
-equation above.  The asymptotic covariance of f comes from the weight matrix W (N x K) through its SVD W = U S V^T,
+equation above, from the log sums at f_k = 0.  The asymptotic covariance of f comes from the weight matrix W (N x K) through its SVD W = U S V^T,
 with V and S from the eigendecomposition of the device Gram matrix W^T W = V S^2 V^T:
 
     Theta = W^T (I - W diag(N) W^T)^+ W = V S (I - S V^T diag(N) V S)^+ S V^T,
@@ -113,14 +117,16 @@ class MBAR:
 
     # -- device calls
     def _evaluate(self, f, hessian):
+        """(sum_n log D_n, gradient, Hessian or None, log sum_n W_in) at f."""
         K = len(f)
         f = np.ascontiguousarray(f, dtype=np.float64)
         s = C.c_double()
-        g = np.empty(K)
+        g, lw = np.empty(K), np.empty(K)
         H = np.empty((K, K)) if hessian else None
         _check(self._lib, self._h, self._lib.rx_mbar_evaluate(self._h, _ptr(f), C.byref(s), _ptr(g),
                                                                _ptr(H) if hessian else None))
-        return s.value, g, H
+        _check(self._lib, self._h, self._lib.rx_mbar_get_log_wsum(self._h, _ptr(lw)))
+        return s.value, g, H, lw
 
     def _gram(self, f):
         K = len(f)
@@ -141,47 +147,65 @@ class MBAR:
             f -= f[gauge]
         f[self.N_k == 0] = 0.0
 
-        def residual(g):
-            return np.max(np.abs(g[sampled]) / N[sampled])
+        def residual(lw):
+            # |g_i| / N_i = |1 - sum_n W_in|, without the cancellation of 1 - sum when the sum is far from 1
+            return np.max(np.abs(np.expm1(lw[sampled])))
+
+        def floor(f):
+            # exp's arguments f_i - u_in - log D_n are of the size of f, so each weight, and the residual, carries a
+            # rounding error of about eps max|f|: a tolerance below that can only be met by chance
+            return max(tol, 16.0 * np.finfo(np.float64).eps * np.max(np.abs(f[sampled])))
 
         # self-consistent iterations until the gradient is small enough for Newton steps
         it = 0
         while it < min(maximum_iterations, 50):
-            logden, g, _ = self._evaluate(f, False)
+            logden, g, _, lw = self._evaluate(f, False)
             it += 1
-            r = residual(g)
-            if r <= tol or r < 1.0e-2:
+            r = residual(lw)
+            if r <= floor(f) or r < 1.0e-2:
                 break
-            f[sampled] -= np.log1p(-g[sampled] / N[sampled])
+            f[sampled] -= lw[sampled]
             f[sampled] -= f[gauge]
         # Newton iterations on the log-likelihood, backtracking when a step lowers it
-        logden, g, H = self._evaluate(f, True)
+        logden, g, H, lw = self._evaluate(f, True)
         it += 1
         like = N @ f - logden
-        while residual(g) > tol:
+        while residual(lw) > floor(f):
             if it >= maximum_iterations:
                 raise MBARConvergenceError('MBAR did not converge in %d iterations: relative gradient %.3g > %.3g'
-                                           % (it, residual(g), tol))
+                                           % (it, residual(lw), floor(f)))
             if len(free) == 0:
                 break
-            step = np.linalg.solve(H[np.ix_(free, free)], -g[free])
+            try:
+                step = np.linalg.solve(H[np.ix_(free, free)], -g[free])
+            except np.linalg.LinAlgError:
+                step = np.full(len(free), np.nan)
             t = 1.0
-            while True:
+            while np.all(np.isfinite(step)):
                 trial = f.copy()
                 trial[free] += t * step
-                logden_t, g_t, H_t = self._evaluate(trial, True)
+                logden_t, g_t, H_t, lw_t = self._evaluate(trial, True)
                 it += 1
                 like_t = N @ trial - logden_t
-                if like_t >= like - 1e-12 * abs(like) or t < 1e-6 or it >= maximum_iterations:
+                if like_t >= like - 1e-12 * abs(like) or it >= maximum_iterations:
                     break
                 t *= 0.5
-            f, g, H, like = trial, g_t, H_t, like_t
+                if t < 1e-6:
+                    step = step * np.nan
+            if not np.all(np.isfinite(step)):
+                # far from the solution a state whose weights all underflow makes H singular: a self-consistent
+                # step, which is exact in log space at any distance, moves it instead
+                trial = f.copy()
+                trial[sampled] -= lw[sampled]
+                trial[sampled] -= trial[gauge]
+                logden_t, g_t, H_t, lw_t = self._evaluate(trial, True)
+                it += 1
+                like_t = N @ trial - logden_t
+            f, g, H, like, lw = trial, g_t, H_t, like_t, lw_t
         self.n_iterations = it
-        # states without samples: f_i = -log sum_n exp(-u_in) / D_n, at f_i = 0
+        # states without samples: f_i = -log sum_n exp(-u_in) / D_n, from the last evaluation, which was at f_i = 0
         unsampled = self.N_k == 0
-        if unsampled.any():
-            _, wsum = self._gram(f)
-            f[unsampled] = -np.log(wsum[unsampled])
+        f[unsampled] = -lw[unsampled]
         return f - f[0]
 
     # -- uncertainty

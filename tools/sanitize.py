@@ -50,5 +50,9 @@ rng = np.random.default_rng(0)
 e.history_load(rng.normal(size=(50, 7, 40)), rng.normal(size=(50, 7, 2)))
 N_k = np.zeros(42, np.int64); N_k[1:8] = 37
 MBAR.from_history(e, np.arange(3, 40), np.r_[40, np.arange(40), 41], N_k).close()
+# the per-sample shift (k_mbar_shift) and the log-space row sums over several chunks (k_mbar_rowsum, k_mbar_tree_rows)
+# on a host-built u_kn with a partial last chunk, states 800 kT apart and unsampled ends
+u = rng.normal(size=(5, 3 * 8192 + 5)) + np.array([-900.0, 0.0, 400.0, 800.0, 1700.0])[:, None] - 1.0e5
+MBAR(u, [0, 8192, 8192, 8197, 0]).close()
 e.close()
 print('sanitize workload done')
