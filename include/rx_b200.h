@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define RX_ABI_VERSION 1
+#define RX_ABI_VERSION 2
 #if defined(__GNUC__)
 #define RX_API __attribute__((visibility("default")))
 #else
@@ -79,6 +79,7 @@ typedef struct {
     double energy_offset;    /* kJ/mol added to U in this state (dispersion corrections, U0)              */
     double ho_K;             /* kJ/mol/nm^2 */
     double ho_x0[3];         /* nm */
+    double lambda_electrostatics;   /* AlchemicalState.lambda_electrostatics; read for alchemical molecules only     */
 } rx_state_params;
 
 /* ---- lifecycle ------------------------------------------------------------------------------------ */
@@ -109,6 +110,13 @@ typedef struct {
     const double *bonds, *angles, *torsions;
     const int64_t *exclusions;
     const double *exceptions, *constraints;
+    /* One alchemical region (AbsoluteAlchemicalFactory, alchemy.py:1539-2038 with NoCutoff; NULL: none).  A pair or 1-4
+     * exception with one alchemical atom becomes
+     *   lambda_electrostatics 138.935456 qq / r + lambda_sterics^a 4 eps x (x - 1),  x = (alpha (1 - lambda_sterics)^b + (r/sigma)^c)^(-6/c)
+     * with the soft-core constants of rx_config; one with two alchemical atoms the same with each lambda replaced by 1 unless
+     * the matching annihilate flag is set.  Exclusions stay exclusions.  The states' lambdas are those of rx_state_params. */
+    const uint8_t *alchemical;   /* [n_atoms] 0/1 */
+    int32_t annihilate_sterics, annihilate_electrostatics;
 } rx_molecule;
 
 /* ---- static tables -------------------------------------------------------------------------------- */
@@ -152,6 +160,12 @@ typedef struct {
     double alpha, beta, gamma, offset;
     double solute_dielectric, solvent_dielectric;
     double sa_energy, probe_radius;   /* kJ/mol/nm^2, nm */
+    /* An alchemical molecule (rx_molecule.alchemical): atom j's descreening of i and the charges of the pair term are scaled
+     * by w_j = lambda_electrostatics alch_j + (1 - alch_j), each atom's self and non-polar terms by w_i
+     * (alchemy.py:2144-2300).  alchemical_obc2: the literal constants of the reference's alchemical OBC2 expression
+     * instead -- 138.935485 for 138.935456, 28.3919551 (radius + 0.14)^2 for the non-polar prefactor -- and its engulfment
+     * term 1/2 C, C = 2 (1/rt_i - 1/L) for sr_j - r > rt_i. */
+    int32_t alchemical_obc2;
 } rx_gbsa;
 RX_API int rx_set_implicit_solvent(rx_engine *h, const rx_gbsa *gbsa);
 /* LangevinSplittingDynamicsMove parameters (mcmc.py:1280-1291) / LangevinIntegrator (integrators.py:1071-1158):

@@ -148,7 +148,7 @@ def engine_tables(thermodynamic_states):
     """Per-state arrays for Engine.set_states."""
     sys0 = check_compatible(thermodynamic_states)
     M = len(thermodynamic_states)
-    T = np.zeros(M); lam = np.ones(M); off = np.zeros(M); hoK = np.zeros(M); hox0 = np.zeros((M, 3))
+    T = np.zeros(M); lam = np.ones(M); lam_e = np.ones(M); off = np.zeros(M); hoK = np.zeros(M); hox0 = np.zeros((M, 3))
     two = sys0.kind == LJ and sys0.alchemical_regions is not None
     lam2 = np.ones(M) if two else None
     base_lrc = lj_dispersion_correction(sys0) if sys0.kind == LJ else 0.0
@@ -167,13 +167,16 @@ def engine_tables(thermodynamic_states):
                 cache[lam[l]] = alchemical_dispersion_correction(sys0, lam[l])
             off[l] = base_lrc + cache[lam[l]]
         elif sys0.kind == MOLECULE:
-            pass      # the states of a molecule differ in temperature only
+            if sys0.is_alchemical:   # (other molecules' states differ in temperature only)
+                lam[l], lam_e[l] = p['lambda_sterics'], p['lambda_electrostatics']
         else:
             so = s._standard_system
             hoK[l] = so.ho_K
             hox0[l] = so.ho_x0
             off[l] = so.ho_U0
     tab = dict(temperature=T, lambda_sterics=lam, energy_offset=off, ho_K=hoK, ho_x0=hox0)
+    if sys0.kind == MOLECULE and sys0.is_alchemical:
+        tab['lambda_electrostatics'] = lam_e
     if two:
         tab['lambda_sterics_2'] = lam2
     return sys0, tab
@@ -243,7 +246,9 @@ def build_engine(thermodynamic_states, n_replicas, device=0, rank=0, world_size=
     elif sys0.kind == MOLECULE:
         if N > 32:
             raise NotImplementedError('molecules above 32 atoms are not provided (one lane per atom): %d atoms' % N)
-        eng = Engine(_lib.RX_SYSTEM_MOLECULE, n_replicas, M, N, device=device, rank=rank, world_size=world_size)
+        eng = Engine(_lib.RX_SYSTEM_MOLECULE, n_replicas, M, N, device=device, rank=rank, world_size=world_size,
+                     softcore_alpha=sys0.softcore_alpha, softcore_a=sys0.softcore_a, softcore_b=sys0.softcore_b,
+                     softcore_c=sys0.softcore_c)
         eng.set_molecule(sys0)
     else:
         eng = Engine(_lib.RX_SYSTEM_HARMONIC, n_replicas, M, N, device=device, rank=rank, world_size=world_size)

@@ -82,7 +82,7 @@ class Engine:
         self._two_regions = False
 
     @staticmethod
-    def _state_table(temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None):
+    def _state_table(temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None, lambda_electrostatics=None):
         M = len(temperature)
         arr = (_lib.RxStateParams * M)()
         for l in range(M):
@@ -90,17 +90,20 @@ class Engine:
             arr[l].lambda_sterics = 1.0 if lambda_sterics is None else float(lambda_sterics[l])
             arr[l].energy_offset = 0.0 if energy_offset is None else float(energy_offset[l])
             arr[l].ho_K = 0.0 if ho_K is None else float(ho_K[l])
+            arr[l].lambda_electrostatics = 1.0 if lambda_electrostatics is None else float(lambda_electrostatics[l])
             x0 = (0.0, 0.0, 0.0) if ho_x0 is None else ho_x0[l]
             for q in range(3):
                 arr[l].ho_x0[q] = float(x0[q])
         return arr
 
-    def set_states(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None, lambda_sterics_2=None):
-        """lambda_sterics_2: the second alchemical region's lambda of every state (rx_set_states_region2)."""
+    def set_states(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None, lambda_sterics_2=None,
+                   lambda_electrostatics=None):
+        """lambda_sterics_2: the second alchemical region's lambda of every state (rx_set_states_region2);
+        lambda_electrostatics: read for alchemical molecules only."""
         if len(temperature) != self.M:
             raise ValueError('expected %d states' % self.M)
         self._check_region2(lambda_sterics_2)
-        arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0)
+        arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0, lambda_electrostatics)
         self._check(self._lib.rx_set_states(self._h, C.cast(arr, C.c_void_p)))
         if lambda_sterics_2 is not None:
             self._check(self._lib.rx_set_states_region2(self._h, _ptr(_c64(lambda_sterics_2, (self.M,)))))
@@ -123,12 +126,12 @@ class Engine:
         self._two_regions = True
 
     def compute_energies_at(self, temperature, lambda_sterics=None, energy_offset=None, ho_K=None, ho_x0=None, pressure=None,
-                            dispersion=None, lambda_sterics_2=None):
+                            dispersion=None, lambda_sterics_2=None, lambda_electrostatics=None):
         """u[K][n] of every replica at n other states (unsampled states); the resident matrix is untouched.  An NPT engine
         takes those states' pressures (kJ/mol/nm^3) and dispersion coefficients (kJ/mol nm^3) as well; a two-region engine
         their second-region lambdas."""
         self._check_region2(lambda_sterics_2)
-        arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0)
+        arr = self._state_table(temperature, lambda_sterics, energy_offset, ho_K, ho_x0, lambda_electrostatics)
         n = len(temperature)
         out = np.zeros((self.K, n))
         if lambda_sterics_2 is not None:
@@ -160,17 +163,22 @@ class Engine:
                             float(constraint_tolerance), *[arrs[k].ctypes.data for k in
                                                            ('mass', 'charge', 'sigma', 'epsilon', 'bonds', 'angles', 'torsions',
                                                             'exclusions', 'exceptions', 'constraints')])
+        if system.is_alchemical:
+            alch = np.ascontiguousarray(system.alchemical_mask(), np.uint8)
+            m.alchemical, m.annihilate_sterics = alch.ctypes.data, int(bool(system.annihilate_sterics))
+            m.annihilate_electrostatics = int(bool(system.annihilate_electrostatics))
         self._check(self._lib.rx_set_molecule(self._h, C.byref(m)))
         if getattr(system, 'gb_radius', None) is not None:
-            self.set_implicit_solvent(system.gb_radius, system.gb_scale, *system.gb_parameters)
+            self.set_implicit_solvent(system.gb_radius, system.gb_scale, *system.gb_parameters,
+                                      alchemical_obc2=system.is_alchemical and system.alchemical_obc2)
 
     def set_implicit_solvent(self, radius, scale, alpha, beta, gamma, offset, solute_dielectric, solvent_dielectric, sa_energy,
-                             probe_radius):
+                             probe_radius, alchemical_obc2=False):
         """OBC implicit solvent for the molecule of the last set_molecule (rx_set_implicit_solvent)."""
         radius = np.ascontiguousarray(radius, np.float64)
         scale = np.ascontiguousarray(scale, np.float64)
         g = _lib.RxGbsa(radius.ctypes.data, scale.ctypes.data, alpha, beta, gamma, offset, solute_dielectric, solvent_dielectric,
-                        sa_energy, probe_radius)
+                        sa_energy, probe_radius, int(bool(alchemical_obc2)))
         self._check(self._lib.rx_set_implicit_solvent(self._h, C.byref(g)))
 
     def set_state_integrator(self, state, timestep, collision_rate, n_steps, splitting='V R O R V', reassign_velocities=False):

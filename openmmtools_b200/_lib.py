@@ -9,7 +9,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('RX_B200_LIB') or os.path.join(_HERE, 'csrc', 'librx_b200.so')   # override: A/B builds
 
-RX_ABI_VERSION = 1
+RX_ABI_VERSION = 2
 RX_OK, RX_ERR_INVALID, RX_ERR_CUDA, RX_ERR_NAN, RX_ERR_UNSUPPORTED, RX_ERR_COMM, RX_ERR_CAPACITY = 0, -1, -2, -3, -4, -5, -6
 RX_SYSTEM_NONE, RX_SYSTEM_LJ_ALCH, RX_SYSTEM_HARMONIC, RX_SYSTEM_MOLECULE = 0, 1, 2, 3
 RX_STREAM_NUMBA, RX_STREAM_NUMPY = 0, 1
@@ -48,7 +48,7 @@ class RxConfig(C.Structure):
 
 class RxStateParams(C.Structure):
     _fields_ = [('temperature', C.c_double), ('lambda_sterics', C.c_double), ('energy_offset', C.c_double),
-                ('ho_K', C.c_double), ('ho_x0', C.c_double * 3)]
+                ('ho_K', C.c_double), ('ho_x0', C.c_double * 3), ('lambda_electrostatics', C.c_double)]
 
 
 class RxSamsConfig(C.Structure):
@@ -84,7 +84,8 @@ class RxMolecule(C.Structure):
                 ('constraint_tolerance', C.c_double),
                 ('mass', C.c_void_p), ('charge', C.c_void_p), ('sigma', C.c_void_p), ('epsilon', C.c_void_p),
                 ('bonds', C.c_void_p), ('angles', C.c_void_p), ('torsions', C.c_void_p), ('exclusions', C.c_void_p),
-                ('exceptions', C.c_void_p), ('constraints', C.c_void_p)]
+                ('exceptions', C.c_void_p), ('constraints', C.c_void_p), ('alchemical', C.c_void_p),
+                ('annihilate_sterics', C.c_int32), ('annihilate_electrostatics', C.c_int32)]
 
 
 class RxMcMove(C.Structure):
@@ -95,7 +96,7 @@ class RxMcMove(C.Structure):
 class RxGbsa(C.Structure):
     _fields_ = [('radius', C.c_void_p), ('scale', C.c_void_p), ('alpha', C.c_double), ('beta', C.c_double), ('gamma', C.c_double),
                 ('offset', C.c_double), ('solute_dielectric', C.c_double), ('solvent_dielectric', C.c_double),
-                ('sa_energy', C.c_double), ('probe_radius', C.c_double)]
+                ('sa_energy', C.c_double), ('probe_radius', C.c_double), ('alchemical_obc2', C.c_int32)]
 
 
 _lib = None

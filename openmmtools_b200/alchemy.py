@@ -1,4 +1,4 @@
-"""Alchemical modification of the Lennard-Jones test system and the AlchemicalState that controls it.
+"""Alchemical modification of the Lennard-Jones test system and of small molecules, and the AlchemicalState that controls it.
 
 Mirrors /root/reference/openmmtools/alchemy/alchemy.py for the pieces the replica-exchange path exercises:
 ``AlchemicalState`` (:90-410), ``AlchemicalRegion`` (:417-427) and
@@ -6,8 +6,8 @@ Mirrors /root/reference/openmmtools/alchemy/alchemy.py for the pieces the replic
 fluid (:1539-2038) is restated as parameters of the CUDA energy function: non-alchemical pairs keep plain LJ
 (NonbondedForce with the alchemical epsilons zeroed, :1903-1909), alchemical/non-alchemical pairs use soft-core
 sterics controlled by ``lambda_sterics`` (:1383-1388, interaction group :1915), alchemical/alchemical pairs use
-the same expression with lambda fixed to 1 unless ``annihilate_sterics`` (:1776-1777, group :1919).  Bonded,
-electrostatic and GB branches need a molecular force field and are out of scope.
+the same expression with lambda fixed to 1 unless ``annihilate_sterics`` (:1776-1777, group :1919).  Small molecules:
+see below; alchemical bonds, angles and torsions are not provided.
 
 Two alchemical regions (a list of two ``AlchemicalRegion``, e.g. ``name=None`` or ``'A'`` plus ``'B'``) are the
 dual-topology / separated-topology set-up: the epsilons of both regions are zeroed in the NonbondedForce, each region r
@@ -24,11 +24,24 @@ gets its own environment x r and r x r groups driven by ``lambda_sterics<suffix_
 
 Up to two regions; both must use the same soft-core constants (OpenMM keeps one value per global parameter name,
 :2009-2017), their ``annihilate_sterics`` may differ.
+
+A small molecule (``MOLECULE`` systems: TolueneVacuum, TolueneImplicit, AlanineDipeptide*, in vacuum or OBC1/OBC2 implicit
+solvent) takes one region.  Its pairs and 1-4 exceptions with one alchemical atom get soft-core sterics driven by
+``lambda_sterics`` and Coulomb scaled by ``lambda_electrostatics`` (:1380-1450, 1840-1880; NoCutoff, so the soft-core
+electrostatic radius is r); pairs of two alchemical atoms the same with each lambda fixed to 1 unless
+``annihilate_sterics`` / ``annihilate_electrostatics``.  The OBC terms are scaled by w_i = lambda_electrostatics alch_i +
+(1 - alch_i) as the reference rewrites them (OBC1: :2223-2300; OBC2: :2144-2221, with that expression's own constants)::
+
+    toluene = testsystems.TolueneImplicit()
+    system = AbsoluteAlchemicalFactory().create_alchemical_system(toluene.system, AlchemicalRegion(alchemical_atoms=range(15)))
+    protocol = {'lambda_electrostatics': [1.0, 0.5, 0.0, 0.0, 0.0], 'lambda_sterics': [1.0, 1.0, 1.0, 0.5, 0.0]}
 """
 import collections
+import numpy as np
 from . import unit
 from .states import GlobalParameterState, GlobalParameterError   # noqa: F401
-from .system import System, LJ
+from .system import System, LJ, MOLECULE
+from .amber import OBC_MODELS
 
 
 class AlchemicalStateError(GlobalParameterError):
@@ -75,7 +88,8 @@ _SOFTCORE_FIELDS = ('softcore_alpha', 'softcore_a', 'softcore_b', 'softcore_c', 
 
 
 class AbsoluteAlchemicalFactory:
-    """Factory of alchemically modified systems (alchemy.py:430-754), LJ-sterics subset."""
+    """Factory of alchemically modified systems (alchemy.py:430-754): the LJ fluid's sterics, small molecules' sterics,
+    electrostatics and OBC terms."""
 
     def __init__(self, consistent_exceptions=False, switch_width=1.0 * unit.angstroms,
                  alchemical_pme_treatment='exact', alchemical_rf_treatment='switched',
@@ -90,10 +104,12 @@ class AbsoluteAlchemicalFactory:
     def create_alchemical_system(self, reference_system, alchemical_regions, alchemical_regions_interactions=frozenset()):
         if alchemical_regions_interactions != frozenset():       # alchemy.py:661-662
             raise NotImplementedError('Interactions between alchemical regions is untested')
-        if not isinstance(reference_system, System) or reference_system.kind != LJ:
-            raise NotImplementedError('only the Lennard-Jones test system can be alchemically modified on this path')
+        if not isinstance(reference_system, System) or reference_system.kind not in (LJ, MOLECULE):
+            raise NotImplementedError('only the Lennard-Jones fluid and small molecules can be alchemically modified on this path')
         if isinstance(alchemical_regions, AlchemicalRegion):
             alchemical_regions = [alchemical_regions]
+        if reference_system.kind == MOLECULE:
+            return self._alchemically_modify_molecule(reference_system, list(alchemical_regions))
         regions = list(alchemical_regions)
         if len(regions) == 0:
             raise ValueError('alchemical_atoms must be specified')
@@ -142,6 +158,48 @@ class AbsoluteAlchemicalFactory:
             suffix = '' if r.name is None else '_' + r.name                  # alchemy.py:1695-1700
             system.global_parameters['lambda_sterics' + suffix] = 1.0
             system.global_parameters['lambda_electrostatics' + suffix] = 1.0
+        return system
+
+    # the literals of the reference's alchemical OBC2 expression (alchemy.py:2184-2203): offset, probe radius and the
+    # surface-area energy whose 4 pi multiple is its 28.3919551
+    _OBC2_LITERALS = (0.009, 0.14, 28.3919551 / (4.0 * np.pi))
+
+    def _alchemically_modify_molecule(self, reference_system, regions):
+        if len(regions) == 0:
+            raise ValueError('alchemical_atoms must be specified')
+        if len(regions) > 1:      # both GB paths refuse them (alchemy.py:2167-2168, 2258-2259); vacuum follows suit
+            raise NotImplementedError('a molecule takes one alchemical region')
+        region = regions[0]
+        if region.alchemical_atoms is None or len(list(region.alchemical_atoms)) == 0:
+            raise ValueError('alchemical_atoms must be specified')
+        atoms = sorted(set(int(a) for a in region.alchemical_atoms))
+        if atoms[0] < 0 or atoms[-1] >= reference_system.n_particles:
+            raise ValueError('alchemical atom index out of range')
+        if any(x not in (None, False, [], ()) for x in (region.alchemical_bonds, region.alchemical_angles, region.alchemical_torsions)):
+            raise NotImplementedError('alchemical bonds, angles and torsions are not provided for molecules')
+        if (region.softcore_beta, region.softcore_d, region.softcore_e, region.softcore_f) != (0.0, 1, 1, 2):
+            raise NotImplementedError('soft-core electrostatics (softcore_beta/d/e/f other than 0, 1, 1, 2) are not provided')
+        if self.consistent_exceptions:
+            raise NotImplementedError('consistent_exceptions is not provided for molecules')
+        if reference_system.is_alchemical:
+            raise ValueError('the system is already alchemically modified')
+        gb = reference_system.gb_parameters
+        obc2 = gb is not None and tuple(gb[:3]) == OBC_MODELS['OBC2']
+        if obc2 and not np.allclose((gb[3], gb[7], gb[6]), self._OBC2_LITERALS, rtol=1e-9, atol=0.0):
+            raise NotImplementedError('the alchemical OBC2 expression has offset 0.009 nm, probe radius 0.14 nm and '
+                                      'surface-area energy 2.25936 kJ/mol/nm^2 built in; this system has %r' % (tuple(gb),))
+        system = reference_system.copy()
+        system.alchemical_atoms = tuple(atoms)
+        system.annihilate_sterics = bool(region.annihilate_sterics)
+        system.annihilate_electrostatics = bool(region.annihilate_electrostatics)
+        system.softcore_alpha = float(region.softcore_alpha)
+        system.softcore_a = float(region.softcore_a)
+        system.softcore_b = float(region.softcore_b)
+        system.softcore_c = float(region.softcore_c)
+        system.alchemical_obc2 = obc2
+        system.global_parameters = dict(reference_system.global_parameters)
+        system.global_parameters['lambda_sterics'] = 1.0
+        system.global_parameters['lambda_electrostatics'] = 1.0
         return system
 
     @staticmethod

@@ -231,6 +231,9 @@ static int convert_states(rx_engine *h, const rx_state_params *s, int n, std::ve
         if (!(s[l].temperature > 0)) RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": temperature must be > 0");
         if (h->cfg.system_kind == RX_SYSTEM_LJ_ALCH && !(s[l].lambda_sterics >= 0.0 && s[l].lambda_sterics <= 1.0))
             RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": lambda_sterics must be in [0, 1]");
+        if (h->cfg.system_kind == RX_SYSTEM_MOLECULE &&
+            !(s[l].lambda_sterics >= 0.0 && s[l].lambda_sterics <= 1.0 && s[l].lambda_electrostatics >= 0.0 && s[l].lambda_electrostatics <= 1.0))
+            RX_FAIL(h, RX_ERR_INVALID, std::string(who) + ": lambda_sterics and lambda_electrostatics must be in [0, 1]");
         StateDev &d = out[l];
         d.kT = RX_KB * s[l].temperature;
         d.beta = 1.0 / d.kT;
@@ -241,6 +244,7 @@ static int convert_states(rx_engine *h, const rx_state_params *s, int n, std::ve
         d.ho_K = s[l].ho_K;
         for (int q = 0; q < 3; q++) d.ho_x0[q] = s[l].ho_x0[q];
         d.lambda2 = 1.0; d.la2 = 1.0; d.ob2 = 0.0;
+        d.lambda_e = s[l].lambda_electrostatics;
     }
     return RX_OK;
 }

@@ -17,6 +17,7 @@ namespace cg = cooperative_groups;
 #include <string.h>
 #include <stdlib.h>
 #include <type_traits>
+#include <array>
 
 // ---------------------------------------------------------------------------------------------------
 // Philox4x32-10 counter-based generator: noise is a pure function of (seed, iteration, replica, atom, step)
@@ -993,6 +994,8 @@ struct MolTables {
 };
 void RecordDelete::operator()(MolTables *m) const { delete m; }
 static const MolGB *mol_gb_of(const rx_engine *h) { return h->mol->gb.on ? &h->mol->gb : nullptr; }   // nullptr: vacuum
+// An alchemical molecule runs the ALCH = true instantiations; any other the kernels it ran before they existed.
+static bool mol_alch(const rx_engine *h) { return h->mol->dev.alch != 0; }
 
 // A block may take 48 KB of shared memory, static and dynamic together, unless the kernel has opted in to more (up to
 // cudaDevAttrMaxSharedMemoryPerBlockOptin, which mol_check_shared checks).  The molecule's tables grow with its terms, the
@@ -1212,12 +1215,12 @@ int rxi_propagate(rx_engine *h, uint64_t seed, uint64_t iteration, int reassign,
         const MolGB *gb = mol_gb_of(h);
         const bool no_star = getenv("RX_MOL_NO_STAR") != nullptr;   // cross-check: the general cluster path for every molecule
         const bool star = md->max_cluster <= 3 && !no_star;
-        auto kern = gb ? (star ? k_propagate_mol<true, true> : k_propagate_mol<false, true>)
-                       : (star ? k_propagate_mol<true, false> : k_propagate_mol<false, false>);
+        auto kern = with_flag(star, [&](auto s) { return with_flag(gb != nullptr, [&](auto g) { return with_flag(mol_alch(h), [&](auto al) {
+            return k_propagate_mol<s, g, al>; }); }); });
         const int dyn = mol_dyn_bytes(*md, gb, true);
         if (h->hmc) {
-            auto hk = gb ? (star ? k_propagate_mol_hmc<true, true> : k_propagate_mol_hmc<false, true>)
-                         : (star ? k_propagate_mol_hmc<true, false> : k_propagate_mol_hmc<false, false>);
+            auto hk = with_flag(star, [&](auto s) { return with_flag(gb != nullptr, [&](auto g) { return with_flag(mol_alch(h), [&](auto al) {
+                return k_propagate_mol_hmc<s, g, al>; }); }); });
             const int rch = smem_opt_in(h, (const void *)hk, dyn);
             if (rch) return rch;
             hk<<<h->kloc, 32 * MOL_WARPS, dyn, h->stream>>>(*md, p.move, (const StateDev *)h->d_states, (const int *)h->d_perm,
@@ -1511,12 +1514,12 @@ int rxi_minimize(rx_engine *h, double tolerance, int max_iterations, double *d_r
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
         const MolDev *m = &h->mol->dev;
         const MolGB *gb = mol_gb_of(h);
-        auto kern = gb ? k_minimize_mol<true> : k_minimize_mol<false>;
+        auto kern = with_flag(gb != nullptr, [&](auto g) { return with_flag(mol_alch(h), [&](auto al) { return k_minimize_mol<g, al>; }); });
         const int dyn = mol_dyn_bytes(*m, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
         kern<<<h->kloc, 32, dyn, h->stream>>>(*m, (double *)h->d_pos.get(), h->k0, tolerance, max_iterations > 0 ? max_iterations : 100000,
-                                              d_rms, d_iters, gb ? *gb : MolGB{});
+                                              d_rms, d_iters, gb ? *gb : MolGB{}, (const StateDev *)h->d_states, (const int *)h->d_perm);
         RX_CHECK_CUDA(h, cudaGetLastError());
         return RX_OK;
     }
@@ -1595,7 +1598,7 @@ int rxi_compute_energy_rows_at(rx_engine *h, const StateDev *d_states, int n_sta
     if (c.system_kind == RX_SYSTEM_MOLECULE) {
         const MolDev *m = &h->mol->dev;
         const MolGB *gb = mol_gb_of(h);
-        auto kern = gb ? k_energy_mol<true> : k_energy_mol<false>;
+        auto kern = with_flag(gb != nullptr, [&](auto g) { return with_flag(mol_alch(h), [&](auto al) { return k_energy_mol<g, al>; }); });
         const int dyn = mol_dyn_bytes(*m, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;
@@ -1643,6 +1646,7 @@ struct MolTermList {   // every term once with the slots of its contributions; p
     std::vector<TAngle<double>> a;
     std::vector<TTors<double>> t;
     std::vector<TPair<double>> p;   // the plain pairs (the first n_plain), then the exceptions
+    std::vector<TAPair<double>> ap;   // the alchemical pairs (eps: the pair's own)
     int n_plain = 0;
     std::vector<int> goff;
 };
@@ -1659,6 +1663,8 @@ static std::vector<unsigned char> mol_pack(const MolTermList &L, const std::vect
     std::vector<TAngle<T>> a;
     std::vector<TTors<T>> t;
     std::vector<TPair<T>> p;
+    std::vector<TAPair<T>> ap;
+    for (const auto &x : L.ap) ap.push_back({x.i, x.j, x.si, x.sj, x.ls, x.le, {0, 0}, (T)x.qq, (T)x.sig, (T)x.eps});
     for (const auto &x : L.b) b.push_back({x.i, x.j, x.si, x.sj, (T)x.K, (T)x.r0});
     for (const auto &x : L.a) a.push_back({x.i, x.j, x.k, x.si, x.sj, x.sk, (T)x.K, (T)x.t0});
     for (const auto &x : L.t) t.push_back({x.i, x.j, x.k, x.l, x.si, x.sj, x.sk, x.sl, (T)x.n, (T)x.phase, (T)x.kk});
@@ -1676,10 +1682,11 @@ static std::vector<unsigned char> mol_pack(const MolTermList &L, const std::vect
     hd.o_tors = (int)off; off += up(sizeof(TTors<T>) * t.size());
     hd.o_pair = (int)off; off += up(sizeof(TPair<T>) * p.size());
     hd.o_goff = (int)off; off += up(sizeof(int) * L.goff.size());
+    hd.o_apair = (int)off; off += up(sizeof(TAPair<T>) * ap.size());
     std::vector<unsigned char> blob(off, 0);
     memcpy(blob.data(), &hd, sizeof(hd));
     auto put = [&](int o, const auto &v) { if (!v.empty()) memcpy(blob.data() + o, v.data(), sizeof(v[0]) * v.size()); };
-    put(hd.o_bond, b); put(hd.o_angle, a); put(hd.o_tors, t); put(hd.o_pair, p); put(hd.o_goff, L.goff);
+    put(hd.o_bond, b); put(hd.o_angle, a); put(hd.o_tors, t); put(hd.o_pair, p); put(hd.o_goff, L.goff); put(hd.o_apair, ap);
     return blob;
 }
 
@@ -1690,13 +1697,17 @@ static int mol_check_shared(rx_engine *h, const MolDev &m, const MolGB *g, const
     int dev = 0, optin = 0;
     RX_CHECK_CUDA(h, cudaGetDevice(&dev));
     RX_CHECK_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    const bool al = m.alch != 0;
+    auto pick = [&](auto g_, auto al_) {
+        constexpr bool G = decltype(g_)::value, A = decltype(al_)::value;
+        return std::array<const void *, 6>{(const void *)k_propagate_mol<true, G, A>, (const void *)k_propagate_mol<false, G, A>,
+                                           (const void *)k_propagate_mol_hmc<true, G, A>, (const void *)k_propagate_mol_hmc<false, G, A>,
+                                           (const void *)k_minimize_mol<G, A>, (const void *)k_energy_mol<G, A>};
+    };
+    const std::array<const void *, 6> k = with_flag(g != nullptr, [&](auto g_) { return with_flag(al, [&](auto al_) { return pick(g_, al_); }); });
     const struct { const void *kern; int dyn; } use[] = {
-        {g ? (const void *)k_propagate_mol<true, true> : (const void *)k_propagate_mol<true, false>, mol_dyn_bytes(m, g, true)},
-        {g ? (const void *)k_propagate_mol<false, true> : (const void *)k_propagate_mol<false, false>, mol_dyn_bytes(m, g, true)},
-        {g ? (const void *)k_propagate_mol_hmc<true, true> : (const void *)k_propagate_mol_hmc<true, false>, mol_dyn_bytes(m, g, true)},
-        {g ? (const void *)k_propagate_mol_hmc<false, true> : (const void *)k_propagate_mol_hmc<false, false>, mol_dyn_bytes(m, g, true)},
-        {g ? (const void *)k_minimize_mol<true> : (const void *)k_minimize_mol<false>, mol_dyn_bytes(m, g, false)},
-        {g ? (const void *)k_energy_mol<true> : (const void *)k_energy_mol<false>, mol_dyn_bytes(m, g, false)}};
+        {k[0], mol_dyn_bytes(m, g, true)}, {k[1], mol_dyn_bytes(m, g, true)}, {k[2], mol_dyn_bytes(m, g, true)},
+        {k[3], mol_dyn_bytes(m, g, true)}, {k[4], mol_dyn_bytes(m, g, false)}, {k[5], mol_dyn_bytes(m, g, false)}};
     size_t need = 0;
     for (const auto &u : use) {
         cudaFuncAttributes fa;
@@ -1756,14 +1767,32 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
         const int i = (int)q[0], j = (int)q[1];
         nb_mask[i] &= ~(1u << j); nb_mask[j] &= ~(1u << i);
     }
+    // an alchemical region (alchemy.py:1539-2038, one region, NoCutoff): a pair or exception with one alchemical atom follows
+    // both lambdas, one with two follows those the annihilate flags name; one that follows neither keeps its plain term (the
+    // soft-core expression at lambda 1 is plain Lennard-Jones)
+    unsigned alch = 0;
+    if (mol->alchemical)
+        for (int i = 0; i < n; i++) alch |= mol->alchemical[i] ? 1u << i : 0u;
+    auto lambdas = [&](int i, int j, short &ls, short &le) {
+        const int na = (int)((alch >> i) & 1u) + (int)((alch >> j) & 1u);
+        ls = na == 1 || (na == 2 && mol->annihilate_sterics); le = na == 1 || (na == 2 && mol->annihilate_electrostatics);
+        return ls || le;
+    };
     auto add_pair = [&](const TPair<double> &p) {
+        short ls, le;
+        if (lambdas(p.i, p.j, ls, le)) {
+            L.ap.push_back({p.i, p.j, 0, 0, ls, le, {0, 0}, p.qq, p.sig, p.eps});
+            per_atom[p.i].push_back({4, (int)L.ap.size() - 1, 0}); per_atom[p.j].push_back({4, (int)L.ap.size() - 1, 1});
+            return;
+        }
         L.p.push_back(p);
         per_atom[p.i].push_back({3, (int)L.p.size() - 1, 0}); per_atom[p.j].push_back({3, (int)L.p.size() - 1, 1});
     };
     for (int i = 0; i < n; i++)
         for (int j = i + 1; j < n; j++)
-            if ((nb_mask[i] >> j) & 1u)   // (epsilon: mol_pack)
-                add_pair({(short)i, (short)j, 0, 0, MOL_ONE_4PI_EPS0 * charge[i] * charge[j], 0.5 * (sigma[i] + sigma[j]), 0.0});
+            if ((nb_mask[i] >> j) & 1u)   // (epsilon: mol_pack; an alchemical pair's here)
+                add_pair({(short)i, (short)j, 0, 0, MOL_ONE_4PI_EPS0 * charge[i] * charge[j], 0.5 * (sigma[i] + sigma[j]),
+                          sqrt(eps[i]) * sqrt(eps[j])});
     L.n_plain = (int)L.p.size();
     for (int e = 0; e < mol->n_exceptions; e++) {
         const double *q = mol->exceptions + 5 * e;
@@ -1777,7 +1806,8 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
             if (c.kind == 0) dst = c.role == 0 ? &L.b[c.term].si : &L.b[c.term].sj;
             else if (c.kind == 1) dst = c.role == 0 ? &L.a[c.term].si : (c.role == 1 ? &L.a[c.term].sj : &L.a[c.term].sk);
             else if (c.kind == 2) dst = c.role == 0 ? &L.t[c.term].si : (c.role == 1 ? &L.t[c.term].sj : (c.role == 2 ? &L.t[c.term].sk : &L.t[c.term].sl));
-            else dst = c.role == 0 ? &L.p[c.term].si : &L.p[c.term].sj;
+            else if (c.kind == 3) dst = c.role == 0 ? &L.p[c.term].si : &L.p[c.term].sj;
+            else dst = c.role == 0 ? &L.ap[c.term].si : &L.ap[c.term].sj;
             *dst = (short)slot++;
         }
         L.goff.push_back(slot);
@@ -1814,6 +1844,7 @@ int rxi_set_molecule(rx_engine *h, const rx_molecule *mol) {
     const std::vector<unsigned char> t32 = mol_pack<float>(L, eps), t64 = mol_pack<double>(L, eps);
     m->bytes32 = (int)t32.size(); m->bytes64 = (int)t64.size();
     m->n_tb = (int)L.b.size(); m->n_ta = (int)L.a.size(); m->n_tt = (int)L.t.size(); m->n_tp = (int)L.p.size(); m->n_slots = slot;
+    m->n_tap = (int)L.ap.size(); m->alch = alch; m->sc_c = h->cfg.softcore_c; m->c6 = h->cfg.softcore_c == 6.0;
     int rc = mol_check_shared(h, *m, nullptr, "rx_set_molecule: the term tables");
     if (rc) return rc;
     MolTables &t = *tables;
@@ -1834,6 +1865,7 @@ int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s) {
     const MolDev *m = &h->mol->dev;
     const int n = m->n;
     if (!s->radius || !s->scale) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: null per-atom arrays");
+    if (s->alchemical_obc2 && !m->alch) RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: alchemical_obc2 needs an alchemical molecule");
     if (!(s->offset >= 0) || !(s->solute_dielectric > 0) || !(s->solvent_dielectric > 0) || !(s->sa_energy >= 0) ||
         !(s->probe_radius >= 0) || !isfinite(s->alpha) || !isfinite(s->beta) || !isfinite(s->gamma))
         RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: need offset >= 0, dielectrics > 0, sa_energy >= 0, probe_radius >= 0");
@@ -1844,13 +1876,15 @@ int rxi_set_implicit_solvent(rx_engine *h, const rx_gbsa *s) {
             RX_FAIL(h, RX_ERR_INVALID, "rx_set_implicit_solvent: need radius > offset, radius > 0 and scale >= 0 for every atom");
         const double rt = rho - s->offset;
         tab[4 * i] = rt; tab[4 * i + 1] = sc * rt; tab[4 * i + 2] = rho;
-        tab[4 * i + 3] = 4.0 * M_PI * s->sa_energy * (rho + s->probe_radius) * (rho + s->probe_radius);
+        tab[4 * i + 3] = s->alchemical_obc2 ? 28.3919551 * (rho + 0.14) * (rho + 0.14)
+                                            : 4.0 * M_PI * s->sa_energy * (rho + s->probe_radius) * (rho + s->probe_radius);
     }
     MolGB g;
     memset(&g, 0, sizeof(g));
     g.alpha = s->alpha; g.beta = s->beta; g.gamma = s->gamma;
-    g.pre = -MOL_ONE_4PI_EPS0 * (1.0 / s->solute_dielectric - 1.0 / s->solvent_dielectric);
+    g.pre = -(s->alchemical_obc2 ? 138.935485 : MOL_ONE_4PI_EPS0) * (1.0 / s->solute_dielectric - 1.0 / s->solvent_dielectric);
     g.on = 1;
+    g.engulf = s->alchemical_obc2 ? 1 : 0;
     g.prop_bytes = (int)(sizeof(double) * (4 * (size_t)n * n + 3 * (size_t)n));
     const int rc = mol_check_shared(h, *m, &g, "rx_set_implicit_solvent: the term and solvent tables");
     if (rc) return rc;

@@ -24,6 +24,8 @@ struct StateDev {
     // the second alchemical region's lambda_sterics<suffix> and its two soft-core factors (rx_set_states_region2);
     // read only by the two-region kernels
     double lambda2, la2, ob2;
+    // lambda_electrostatics (rx_state_params); read only by the alchemical molecule kernels
+    double lambda_e;
 };
 
 // ---- owned memory ---------------------------------------------------------------------------------------------------

@@ -221,7 +221,7 @@ __global__ void __launch_bounds__(256) k_mc_move(EnParams p, const double4 *__re
 
 // A molecule: one warp per replica, lane q moves atom sub[q] (a subset has at most 32 atoms); the centre of a rotation is the
 // plain mean of the subset (no periodic images).  pos: double[kloc][n][3].
-template <bool GB>
+template <bool GB, bool ALCH>
 __global__ void __launch_bounds__(32) k_mc_move_mol(MolDev m, const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                    const rx_mc_move *__restrict__ moves, const int32_t *__restrict__ atoms,
                                                    double *__restrict__ pos, int k0, int slot, uint2 key, uint32_t iteration,
@@ -242,7 +242,8 @@ __global__ void __launch_bounds__(32) k_mc_move_mol(MolDev m, const StateDev *__
     const MolGBArrays gs((double *)(tb + mol_gb_at(m, false)), n);
     if (a < n) for (int c = 0; c < 3; c++) X[a][c] = XN[a][c] = pos[((size_t)r * n + a) * 3 + c];
     __syncthreads();
-    const double U0 = __shfl_sync(0xffffffffu, mol_energy<GB>(m, g, tb, X, S, gs), 0);
+    const StateDev st = states[l];
+    const double U0 = __shfl_sync(0xffffffffu, mol_energy<GB, ALCH>(m, g, tb, X, S, gs, &st), 0);
     double T[9];
     mc_proposal(mv, philox4x32_10(make_uint4((uint32_t)slot, 0xE0000000u, (uint32_t)k, iteration), key), T);
     const int ns = mv.subset_len;
@@ -260,7 +261,7 @@ __global__ void __launch_bounds__(32) k_mc_move_mol(MolDev m, const StateDev *__
         }
     }
     __syncthreads();
-    const double U1 = __shfl_sync(0xffffffffu, mol_energy<GB>(m, g, tb, XN, S, gs), 0);
+    const double U1 = __shfl_sync(0xffffffffu, mol_energy<GB, ALCH>(m, g, tb, XN, S, gs, &st), 0);
     int yes = 0;
     if (a == 0) du[r * RX_MAX_MC_MOVES + slot] = U1 - U0;
     if (a == 0) yes = mc_accept(true, U1 - U0, states[l].beta, slot, k, iteration, key, n_acc + l * RX_MAX_MC_MOVES + slot,
@@ -276,7 +277,7 @@ int rxi_mc_moves(rx_engine *h, uint64_t seed, uint64_t iteration, int *launches)
     if (h->cfg.system_kind == RX_SYSTEM_MOLECULE) {
         const MolDev *md = &h->mol->dev;
         const MolGB *gb = mol_gb_of(h);
-        auto kern = gb ? k_mc_move_mol<true> : k_mc_move_mol<false>;
+        auto kern = with_flag(gb != nullptr, [&](auto g) { return with_flag(mol_alch(h), [&](auto al) { return k_mc_move_mol<g, al>; }); });
         const int dyn = mol_dyn_bytes(*md, gb, false);
         const int rco = smem_opt_in(h, (const void *)kern, dyn);
         if (rco) return rco;

@@ -34,8 +34,13 @@ template <typename T> struct TBond { short i, j, si, sj; T K, r0; };
 template <typename T> struct TAngle { short i, j, k, si, sj, sk; T K, t0; };
 template <typename T> struct TTors { short i, j, k, l, si, sj, sk, sl; T n, phase, kk; };
 template <typename T> struct TPair { short i, j, si, sj; T qq, sig, eps; };   // qq = 138.935456 q_i q_j (exceptions: their own values)
+// An alchemical pair (rx_set_molecule with an alchemical mask; alchemy.py:1380-1450, NoCutoff): a pair or 1-4 exception with
+// an alchemical atom whose soft-core sterics follow the state's lambda_sterics (ls = 1; ls = 0: lambda 1, an alchemical/
+// alchemical pair without annihilate_sterics) and whose Coulomb term is scaled by lambda_electrostatics (le = 1; le = 0: by 1).
+//   U = le_factor qq / r + la 4 eps x (x - 1),  x = (ob + (r/sig)^c)^(-6/c),  la = lambda^a, ob = alpha (1 - lambda)^b
+template <typename T> struct TAPair { short i, j, si, sj, ls, le, pad[2]; T qq, sig, eps; };
 struct MolTerms {      // one contiguous blob: header, then the arrays (offsets in bytes from the blob's start)
-    int o_bond, o_angle, o_tors, o_pair, o_goff, pad[3];   // goff (at o_goff): atom a's slots are [goff[a], goff[a + 1])
+    int o_bond, o_angle, o_tors, o_pair, o_goff, o_apair, pad[2];   // goff (at o_goff): atom a's slots are [goff[a], goff[a + 1])
 };
 
 struct MolDev {
@@ -46,6 +51,11 @@ struct MolDev {
     const MolCons *cons;
     const MolTerms *terms32, *terms64;   // the term list in f32 and in f64 (bytes32, bytes64: multiples of 16)
     int bytes32, bytes64, n_tb, n_ta, n_tt, n_tp, n_slots;
+    // alchemical molecules only (the ALCH instantiations read them): the alchemical pairs, the region as a bit mask of atoms,
+    // the soft-core exponent c (c6: c == 6)
+    int n_tap, c6;
+    unsigned alch;
+    double sc_c;
 };
 
 // OBC generalized Born implicit solvent (rx_set_implicit_solvent), passed to the kernels as a trailing argument so that the
@@ -61,7 +71,12 @@ struct MolGB {
     double alpha, beta, gamma, pre;
     int on;               // (0: vacuum; the GB = true kernels are only launched with 1)
     int prop_bytes;       // the arrays of MolGBArrays, behind the slots (mol_gb_at)
+    int engulf;           // the alchemical OBC2 expression's engulfment term C (alchemy.py:2188-2193; ALCH kernels only)
 };
+
+// The weight of atom i's charge and descreening in an alchemical state: w_i = lambda_e alch_i + (1 - alch_i)
+// (alchemy.py:2188-2203 and the rewriting rules of :2223-2300).
+__device__ __forceinline__ double mol_w(const MolDev &m, int i, double le) { return ((m.alch >> i) & 1u) ? le : 1.0; }
 
 // Dynamic shared memory of the molecule kernels: the staged term table (f32: k_propagate_mol, f64: k_energy_mol and
 // k_minimize_mol), then one double[3] per slot (k_propagate_mol: the float[3] forces of its steps, then the energy slots of
@@ -70,7 +85,8 @@ __host__ __device__ inline int mol_slots_at(const MolDev &m, bool f32) { return 
 __host__ __device__ inline int mol_gb_at(const MolDev &m, bool f32) { return mol_slots_at(m, f32) + 24 * m.n_slots; }
 
 // I_ij at distance r of atom i (offset radius rt) descreened by j (scaled radius sr); *dIdr its derivative.
-__device__ __forceinline__ double gb_descreen(double r, double rt, double sr, double *dIdr) {
+// engulf: with the engulfment term 1/2 C, C = 2 (1/rt - 1/L) step(sr - r - rt) (the alchemical OBC2 expression).
+__device__ __forceinline__ double gb_descreen(double r, double rt, double sr, double *dIdr, bool engulf = false) {
     if (!(r + sr > rt)) { *dIdr = 0.0; return 0.0; }
     const double U = r + sr, d = r - sr, ad = fabs(d);
     const bool far = ad > rt;
@@ -78,7 +94,9 @@ __device__ __forceinline__ double gb_descreen(double r, double rt, double sr, do
     const double iL = 1.0 / L, iU = 1.0 / U, ir = 1.0 / r, iL2 = iL * iL, iU2 = iU * iU, q = sr * sr * ir, lg = log(L * iU);
     *dIdr = 0.5 * (-dL * iL2 + iU2 + 0.25 * (1.0 + q * ir) * (iU2 - iL2) + 0.5 * (r - q) * (dL * iL2 * iL - iU2 * iU) +
                    0.5 * ((dL * iL - iU) - lg * ir) * ir);
-    return 0.5 * (iL - iU + 0.25 * (r - q) * (iU2 - iL2) + 0.5 * lg * ir);
+    const double I = 0.5 * (iL - iU + 0.25 * (r - q) * (iU2 - iL2) + 0.5 * lg * ir);
+    if (engulf && sr - r > rt) { *dIdr += dL * iL2; return I + (1.0 / rt - iL); }
+    return I;
 }
 
 // Born radius from the descreening sum; *dBdI its derivative.
@@ -114,6 +132,11 @@ __device__ __forceinline__ void mol_cross(const double *a, const double *b, doub
 }
 __device__ __forceinline__ double mol_dot(const double *a, const double *b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
+__device__ __forceinline__ double mol_warp_sum(double v) {   // fixed tree: bit-reproducible
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
 // The f32 and f64 forms of the math of mol_terms (the f32 ones are those the dynamics has always used).
 __device__ __forceinline__ float mol_sqrt(float x) { return sqrtf(x); }
 __device__ __forceinline__ double mol_sqrt(double x) { return sqrt(x); }
@@ -137,8 +160,24 @@ __device__ __forceinline__ void mol_stage(unsigned char *dst, const MolTerms *sr
 // term's force on that atom.  ENERGY (T = double): the term's energy goes to the slot of its owner -- the smaller atom index
 // of a bond or pair, role 0 of an angle or torsion -- as the two factors x, y of its last product, so that the owner's sum
 // e = fma(x, y, e) over its slots in slot order (mol_energy) rounds as one fused multiply-add per term; its other slots get 0.
-template <typename T, bool ENERGY>
-__device__ __forceinline__ void mol_terms(const MolDev &m, const unsigned char *tb, const double (*X)[3], T (*S)[3]) {
+// One alchemical pair at state st: *e its energy, *c = -dU/dr / r.
+template <typename T>
+__device__ __forceinline__ void mol_apair(const MolDev &m, const TAPair<T> &p, const double (*X)[3], const StateDev &st, T *e, T *c) {
+    const T d[3] = {(T)(X[p.i][0] - X[p.j][0]), (T)(X[p.i][1] - X[p.j][1]), (T)(X[p.i][2] - X[p.j][2])};
+    const T r2 = d[0] * d[0] + d[1] * d[1] + d[2] * d[2], ir2 = T(1) / r2, ir = mol_sqrt(ir2);
+    const T la = p.ls ? (T)st.la : T(1), ob = p.ls ? (T)st.ob : T(0), le = p.le ? (T)st.lambda_e : T(1);
+    const T u2 = r2 / (p.sig * p.sig);                                      // (r/sig)^2
+    const T s = m.c6 ? u2 * u2 * u2 : (T)pow((double)u2, 0.5 * m.sc_c);   // (r/sig)^c
+    const T x = m.c6 ? T(1) / (ob + s) : (T)pow((double)(ob + s), -6.0 / m.sc_c);
+    const T qe = le * p.qq * ir, lj = la * T(4) * p.eps;
+    *e = qe + lj * x * (x - T(1));
+    *c = (qe + T(6) * lj * (T(2) * x - T(1)) * x * s / (ob + s)) * ir2;
+}
+
+// ALCH: the alchemical pairs too, at the state st (forces; ENERGY: their slots get 0, mol_alch_energy has their energy).
+template <typename T, bool ENERGY, bool ALCH = false>
+__device__ __forceinline__ void mol_terms(const MolDev &m, const unsigned char *tb, const double (*X)[3], T (*S)[3],
+                                          const StateDev *st = nullptr) {
     const MolTerms *h = (const MolTerms *)tb;
     const int lane = threadIdx.x, nth = blockDim.x;   // (k_propagate_mol: all warps of the block; the other kernels: one warp)
     auto energy = [&](int s, bool own, T x, T y) { S[s][0] = own ? x : T(0); S[s][1] = own ? y : T(0); };
@@ -215,6 +254,30 @@ __device__ __forceinline__ void mol_terms(const MolDev &m, const unsigned char *
             for (int q = 0; q < 3; q++) { S[p.si][q] = c * d[q]; S[p.sj][q] = -c * d[q]; }
         }
     }
+    if (!ALCH) return;
+    const TAPair<T> *AP = (const TAPair<T> *)(tb + h->o_apair);
+    for (int t = lane; t < m.n_tap; t += nth) {
+        const TAPair<T> p = AP[t];
+        if (ENERGY) { energy(p.si, false, 0, 0); energy(p.sj, false, 0, 0); continue; }
+        T e, c;
+        mol_apair<T>(m, p, X, *st, &e, &c);
+        const T d[3] = {(T)(X[p.i][0] - X[p.j][0]), (T)(X[p.i][1] - X[p.j][1]), (T)(X[p.i][2] - X[p.j][2])};
+        for (int q = 0; q < 3; q++) { S[p.si][q] = c * d[q]; S[p.sj][q] = -c * d[q]; }
+    }
+}
+
+// The alchemical pairs' energy at state st, summed by each warp over its lanes in a fixed order (every warp gets the same
+// bits, whatever the block size).
+__device__ __forceinline__ double mol_alch_energy(const MolDev &m, const unsigned char *t64, const double (*X)[3],
+                                                  const StateDev &st) {
+    const TAPair<double> *AP = (const TAPair<double> *)(t64 + ((const MolTerms *)t64)->o_apair);
+    double e = 0.0;
+    for (int t = threadIdx.x & 31; t < m.n_tap; t += 32) {
+        double et, c;
+        mol_apair<double>(m, AP[t], X, st, &et, &c);
+        e += et;
+    }
+    return mol_warp_sum(e);
 }
 
 // Constraints are solved per cluster (connected component of the constraint graph) by ONE lane.  Clusters of up to
@@ -566,11 +629,6 @@ __device__ __forceinline__ void mol_star_shake(const MolDev &m, MolStar &k, doub
     mol_star_invert(k);
 }
 
-__device__ __forceinline__ double mol_warp_sum(double v) {   // fixed tree: bit-reproducible
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // The GB terms, pair-parallel over the block, in the arrays of MolGB::prop_bytes: n x n matrices I_ij, dI_ij/dr, the pair's
 // dE/dr / r (symmetric; ENERGY: the pair's energy for j > i) and dE_pair/dB_i, then B_i, dB_i/dI_i and C_i = dE/dB_i dB_i/dI_i.
 // Every entry is written by one thread and every atom adds up its row in index order: no atomics, the same bits whatever the
@@ -580,13 +638,16 @@ struct MolGBArrays {
     __device__ MolGBArrays(double *s, int n) : I(s), D(s + n * n), P(s + 2 * n * n), EB(s + 3 * n * n), B(s + 4 * n * n), dB(B + n), C(dB + n) {}
 };
 
-// phase 1 (before the barrier that ends the term evaluation): the descreening integrals of the ordered pairs
-template <bool ENERGY>
-__device__ __forceinline__ void mol_gb_integrals(const MolGB &g, const double (*X)[3], int n, const MolGBArrays &s) {
+// phase 1 (before the barrier that ends the term evaluation): the descreening integrals of the ordered pairs.  ALCH: at
+// lambda_electrostatics le of the alchemical molecule m, j's descreening of i weighted by w_j (I and dI/dr alike).
+template <bool ENERGY, bool ALCH = false>
+__device__ __forceinline__ void mol_gb_integrals(const MolGB &g, const double (*X)[3], int n, const MolGBArrays &s,
+                                                 const MolDev *m = nullptr, double le = 1.0) {
     for (int t = threadIdx.x; t < n * n; t += blockDim.x) {
         const int i = t / n, j = t - i * n;
         double d[3], dI = 0.0, I = 0.0;
-        if (i != j) I = gb_descreen(gb_dist(X, i, j, d), g.atom[4 * i], g.atom[4 * j + 1], &dI);
+        if (i != j) I = gb_descreen(gb_dist(X, i, j, d), g.atom[4 * i], g.atom[4 * j + 1], &dI, ALCH && g.engulf);
+        if (ALCH) { const double w = mol_w(*m, j, le); I *= w; dI *= w; }
         s.I[t] = I;
         if (!ENERGY) s.D[t] = dI;
     }
@@ -594,8 +655,10 @@ __device__ __forceinline__ void mol_gb_integrals(const MolGB &g, const double (*
 
 // phases 2 and 3 (after it; every thread of the block): Born radii, the pair terms, then the chain-rule factors C_i or, ENERGY,
 // the GB energy atom a < n owns (returned): its self and ACE terms, then its pairs with larger partners in index order.
-template <bool ENERGY>
-__device__ __forceinline__ double mol_gb_radii_pairs(const MolGB &g, const double (*X)[3], const double *q, int n, const MolGBArrays &s) {
+// ALCH: the pair term with charges w_i q_i, w_j q_j, the self and ACE terms of atom a scaled by w_a.
+template <bool ENERGY, bool ALCH = false>
+__device__ __forceinline__ double mol_gb_radii_pairs(const MolGB &g, const double (*X)[3], const double *q, int n, const MolGBArrays &s,
+                                                     const MolDev *m = nullptr, double le = 1.0) {
     const int a = threadIdx.x;
     if (a < n) {
         double I = 0.0, dB;
@@ -609,7 +672,8 @@ __device__ __forceinline__ double mol_gb_radii_pairs(const MolGB &g, const doubl
         if (j <= i) continue;
         double d[3], dr, dbi, dbj;
         const double r = gb_dist(X, i, j, d);
-        const double e = gb_pair(r * r, s.B[i], s.B[j], g.pre * q[i] * q[j], &dr, &dbi, &dbj);
+        const double pqq = ALCH ? g.pre * (mol_w(*m, i, le) * q[i]) * (mol_w(*m, j, le) * q[j]) : g.pre * q[i] * q[j];
+        const double e = gb_pair(r * r, s.B[i], s.B[j], pqq, &dr, &dbi, &dbj);
         if (ENERGY) s.P[t] = e;
         else { s.P[t] = s.P[j * n + i] = dr; s.EB[t] = dbi; s.EB[j * n + i] = dbj; }
     }
@@ -618,6 +682,7 @@ __device__ __forceinline__ double mol_gb_radii_pairs(const MolGB &g, const doubl
     if (a < n) {
         double dEdB;
         e = gb_self(g, q[a], s.B[a], g.atom[4 * a + 2], g.atom[4 * a + 3], &dEdB);
+        if (ALCH) { const double w = mol_w(*m, a, le); e *= w; dEdB *= w; }
         if (ENERGY) {
             for (int j = a + 1; j < n; j++) e += s.P[a * n + j];
         } else {
@@ -640,12 +705,39 @@ __device__ __forceinline__ void mol_gb_force(const double (*X)[3], int a, int n,
     }
 }
 
+// The lambda-independent part of an alchemical molecule's U: every term of the table but the alchemical pairs.  Every thread
+// of the block, after a block barrier; the result is warp 0's.
+__device__ __forceinline__ double mol_energy_fixed(const MolDev &m, const unsigned char *t64, const double (*X)[3], double (*S)[3]) {
+    mol_terms<double, true, true>(m, t64, X, S);
+    __syncthreads();
+    const int a = threadIdx.x, *goff = (const int *)(t64 + ((const MolTerms *)t64)->o_goff);
+    double e = 0.0;
+    if (a < m.n)
+        for (int q = goff[a]; q < goff[a + 1]; q++) e = fma(S[q][0], S[q][1], e);
+    return mol_warp_sum(a < m.n ? e : 0.0);
+}
+
+// The alchemical OBC energy at lambda_electrostatics le (every thread of the block; warp 0's result).
+__device__ __forceinline__ double mol_energy_gb(const MolDev &m, const MolGB &g, const double (*X)[3], const MolGBArrays &gs, double le) {
+    __syncthreads();   // (the arrays may still be read by the previous evaluation)
+    mol_gb_integrals<true, true>(g, X, m.n, gs, &m, le);
+    __syncthreads();
+    const double e = mol_gb_radii_pairs<true, true>(g, X, m.charge, m.n, gs, &m, le);
+    return mol_warp_sum(threadIdx.x < m.n ? e : 0.0);
+}
+
 // U of the molecule at X from the f64 term table t64, in k_energy_mol and at the end of k_propagate_mol (the same function:
 // the same bits).  Every thread of the block calls it after a block barrier; S: double[n_slots][3] with, GB, the arrays of gs
 // behind them.  The result is warp 0's.
-template <bool GB>
+// ALCH: U at the state st, mol_energy_fixed + (mol_energy_gb + mol_alch_energy) -- k_energy_mol evaluates the same functions
+// and adds them in the same order, re-evaluating only the lambda-dependent ones per state.
+template <bool GB, bool ALCH = false>
 __device__ __forceinline__ double mol_energy(const MolDev &m, const MolGB &g, const unsigned char *t64, const double (*X)[3],
-                                             double (*S)[3], const MolGBArrays &gs) {
+                                             double (*S)[3], const MolGBArrays &gs, const StateDev *st = nullptr) {
+    if (ALCH) {
+        const double u0 = mol_energy_fixed(m, t64, X, S);
+        return u0 + ((GB ? mol_energy_gb(m, g, X, gs, st->lambda_e) : 0.0) + mol_alch_energy(m, t64, X, *st));
+    }
     mol_terms<double, true>(m, t64, X, S);
     if (GB) mol_gb_integrals<true>(g, X, m.n, gs);
     __syncthreads();
@@ -668,7 +760,8 @@ __device__ __forceinline__ double mol_energy(const MolDev &m, const MolGB &g, co
 // (a block barrier) Born radii, (barrier) pair terms, (barrier) chain-rule factors, then each atom's sum.
 // mv: the move, __grid_constant__ so that the program is indexed in the parameter bank (a plain by-value struct of this
 // size is copied to local memory).  `reassign` stays an argument: read from mv, it costs this kernel 40-250 instructions.
-template <bool STAR, bool GB>
+// ALCH: an alchemical molecule (MolDev::n_tap, alch) at the lambdas of the replica's state.
+template <bool STAR, bool GB, bool ALCH>
 __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, const __grid_constant__ MoveDev mv, const StateDev *__restrict__ states,
                                                       const int *__restrict__ perm, double *__restrict__ pos,
                                                       double *__restrict__ vel, int k0, uint2 key, uint32_t iteration,
@@ -723,10 +816,10 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
             if (op == 'V') {
                 if (!f_valid) {
                     __syncthreads();   // warp 0's positions are in shared memory
-                    mol_terms<float, false>(m, tb, X, FS);
-                    if (GB) mol_gb_integrals<false>(g, X, n, gs);
+                    mol_terms<float, false, ALCH>(m, tb, X, FS, &st);
+                    if (GB) mol_gb_integrals<false, ALCH>(g, X, n, gs, &m, st.lambda_e);
                     __syncthreads();   // every term's contributions are in their slots
-                    if (GB) mol_gb_radii_pairs<false>(g, X, m.charge, n, gs);
+                    if (GB) mol_gb_radii_pairs<false, ALCH>(g, X, m.charge, n, gs, &m, st.lambda_e);
                     if (active) {   // this atom's slots, in slot order
                         float fx = 0.f, fy = 0.f, fz = 0.f;
                         for (int q = g_off[a]; q < g_off[a + 1]; q++) { fx += FS[q][0]; fy += FS[q][1]; fz += FS[q][2]; }
@@ -768,7 +861,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
         }
     }
     __syncthreads();   // warp 0's final positions; the force slots are free for the energy's
-    const double U = mol_energy<GB>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs);
+    const double U = mol_energy<GB, ALCH>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs, &st);
     const double KE = mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
     const bool bad = active && !(isfinite(X[a][0]) && isfinite(X[a][1]) && isfinite(X[a][2]) && isfinite(V[a][0]) &&
                                  isfinite(V[a][1]) && isfinite(V[a][2]));
@@ -787,7 +880,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol(MolDev m, cons
 // the same function as the energy rows), KE a fixed-tree warp sum in f64, the forces those of k_propagate_mol (f32 terms).
 // No CM-motion removal: the reference removes it before the velocity draw, where it has no effect.  stats[r] += (accepted,
 // trials) of a launch that ends finite; energy[r] = (Eold, Enew) of the last trial.
-template <bool STAR, bool GB>
+template <bool STAR, bool GB, bool ALCH>
 __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol_hmc(MolDev m, const __grid_constant__ MoveDev mv,
                                                           const StateDev *__restrict__ states, const int *__restrict__ perm,
                                                           double *__restrict__ pos, double *__restrict__ vel, int k0, uint2 key,
@@ -825,10 +918,10 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol_hmc(MolDev m, 
     double f[3] = {0, 0, 0};
     auto forces = [&]() {   // every thread of the block (as in k_propagate_mol)
         __syncthreads();
-        mol_terms<float, false>(m, tb, X, FS);
-        if (GB) mol_gb_integrals<false>(g, X, n, gs);
+        mol_terms<float, false, ALCH>(m, tb, X, FS, &st);
+        if (GB) mol_gb_integrals<false, ALCH>(g, X, n, gs, &m, st.lambda_e);
         __syncthreads();
-        if (GB) mol_gb_radii_pairs<false>(g, X, m.charge, n, gs);
+        if (GB) mol_gb_radii_pairs<false, ALCH>(g, X, m.charge, n, gs, &m, st.lambda_e);
         if (active) {
             float fx = 0.f, fy = 0.f, fz = 0.f;
             for (int q = g_off[a]; q < g_off[a + 1]; q++) { fx += FS[q][0]; fy += FS[q][1]; fz += FS[q][2]; }
@@ -839,7 +932,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol_hmc(MolDev m, 
     };
     auto total = [&]() {   // KE + U (warp 0's; every thread of the block calls it)
         __syncthreads();
-        const double U = mol_energy<GB>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs);
+        const double U = mol_energy<GB, ALCH>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs, &st);
         return U + mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
     };
     const double dt = mv.dt_d, hdt = 0.5 * dt, inv_dt = 1.0 / dt;
@@ -885,7 +978,7 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol_hmc(MolDev m, 
         }
     }
     __syncthreads();
-    const double U = mol_energy<GB>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs);
+    const double U = mol_energy<GB, ALCH>(m, g, (const unsigned char *)m.terms64, X, (double (*)[3])FS, gs, &st);
     const double KE = mol_warp_sum(active ? 0.5 * mass * (V[a][0] * V[a][0] + V[a][1] * V[a][1] + V[a][2] * V[a][2]) : 0.0);
     const bool bad = active && !(isfinite(X[a][0]) && isfinite(X[a][1]) && isfinite(X[a][2]) && isfinite(V[a][0]) &&
                                  isfinite(V[a][1]) && isfinite(V[a][2]));
@@ -906,13 +999,17 @@ __global__ void __launch_bounds__(32 * MOL_WARPS) k_propagate_mol_hmc(MolDev m, 
 // velocity is kept tangent.  Converged when the RMS of the projected force
 // falls below tol_rms (kJ/mol/nm); f64 throughout.  (OpenMM's L-BFGS is not reproduced, as for the other systems.)
 // GB: the OBC force of g added to each atom's (mol_gb_radii_pairs, mol_gb_force).
-template <bool GB>
+// ALCH: at the lambdas of the replica's state (states[perm[k]]).
+template <bool GB, bool ALCH>
 __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restrict__ pos, int k0, double tol_rms, int max_iter,
-                                                     double *__restrict__ rms_out, int *__restrict__ iters_out, MolGB g) {
+                                                     double *__restrict__ rms_out, int *__restrict__ iters_out, MolGB g,
+                                                     const StateDev *__restrict__ states, const int *__restrict__ perm) {
     __shared__ double X[MOL_MAX_ATOMS][3], XO[MOL_MAX_ATOMS][3], V[MOL_MAX_ATOMS][3], F[MOL_MAX_ATOMS][3];
     extern __shared__ unsigned long long mol_tab[];
     const int r = blockIdx.x, k = k0 + r, a = threadIdx.x, n = m.n;
     const bool active = a < n;
+    StateDev st;
+    if (ALCH) st = states[perm[k]];
     unsigned char *tb = (unsigned char *)mol_tab;
     mol_stage(tb, m.terms64, m.bytes64);
     double (*FS)[3] = (double (*)[3])(tb + mol_slots_at(m, false));
@@ -944,10 +1041,10 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
     int n_pos = 0, it = 0;
     for (;; it++) {
         double f[3] = {0, 0, 0};
-        mol_terms<double, false>(m, tb, X, FS);
-        if (GB) mol_gb_integrals<false>(g, X, n, gs);
+        mol_terms<double, false, ALCH>(m, tb, X, FS, &st);
+        if (GB) mol_gb_integrals<false, ALCH>(g, X, n, gs, &m, st.lambda_e);
         __syncwarp();   // every term's contributions are in their slots
-        if (GB) mol_gb_radii_pairs<false>(g, X, m.charge, n, gs);
+        if (GB) mol_gb_radii_pairs<false, ALCH>(g, X, m.charge, n, gs, &m, st.lambda_e);
         if (active) {   // this atom's slots, in slot order
             for (int q = goff[a]; q < goff[a + 1]; q++) for (int c = 0; c < 3; c++) f[c] += FS[q][c];
             if (GB) mol_gb_force(X, a, n, gs, f);
@@ -992,7 +1089,10 @@ __global__ void __launch_bounds__(32) k_minimize_mol(MolDev m, double *__restric
 // u[k][l] = beta_l (U(x_k) + offset_l): the states of a molecule differ in temperature only (parallel tempering,
 // paralleltempering.py:175-237: one potential evaluation per replica, scaled by beta_l).
 // GB: with the OBC energy of g.
-template <bool GB>
+// ALCH: u[k][l] = beta_l (U_l(x_k) + offset_l) of an alchemical molecule: the lambda-independent part once per replica, the
+// OBC energy again only where lambda_electrostatics differs from the previous state's, the alchemical pairs only where
+// (lambda_sterics, lambda_electrostatics) does -- the functions and the order of additions of mol_energy<GB, true>.
+template <bool GB, bool ALCH>
 __global__ void __launch_bounds__(32) k_energy_mol(MolDev m, const StateDev *__restrict__ states, int n_states,
                                                    const double *__restrict__ pos, int k0, double *__restrict__ u_out, MolGB g) {
     __shared__ double X[MOL_MAX_ATOMS][3];
@@ -1002,9 +1102,22 @@ __global__ void __launch_bounds__(32) k_energy_mol(MolDev m, const StateDev *__r
     mol_stage(tb, m.terms64, m.bytes64);
     if (a < n) for (int c = 0; c < 3; c++) X[a][c] = pos[((size_t)r * n + a) * 3 + c];
     __syncthreads();
-    const double U = mol_energy<GB>(m, g, tb, X, (double (*)[3])(tb + mol_slots_at(m, false)),
-                                    MolGBArrays((double *)(tb + mol_gb_at(m, false)), n));
-    for (int l = a; l < n_states; l += 32) u_out[(size_t)k * n_states + l] = states[l].beta * (U + states[l].offset);
+    double (*S)[3] = (double (*)[3])(tb + mol_slots_at(m, false));
+    const MolGBArrays gs((double *)(tb + mol_gb_at(m, false)), n);
+    if (!ALCH) {
+        const double U = mol_energy<GB>(m, g, tb, X, S, gs);
+        for (int l = a; l < n_states; l += 32) u_out[(size_t)k * n_states + l] = states[l].beta * (U + states[l].offset);
+        return;
+    }
+    const double u0 = mol_energy_fixed(m, tb, X, S);
+    double e_gb = 0.0, e_ap = 0.0;
+    for (int l = 0; l < n_states; l++) {
+        const StateDev st = states[l];
+        const bool new_e = l == 0 || st.lambda_e != states[l - 1].lambda_e;
+        if (GB && new_e) e_gb = mol_energy_gb(m, g, X, gs, st.lambda_e);
+        if (new_e || st.la != states[l - 1].la || st.ob != states[l - 1].ob) e_ap = mol_alch_energy(m, tb, X, st);
+        if (a == 0) u_out[(size_t)k * n_states + l] = st.beta * ((u0 + (e_gb + e_ap)) + st.offset);
+    }
 }
 
 __global__ void k_randomize_velocities_mol(MolDev m, const StateDev *__restrict__ states, const int *__restrict__ perm,

@@ -251,7 +251,7 @@ class ThermodynamicState:
     def _engine_parameters(self):
         s = self._standard_system
         p = dict(temperature=self._temperature, lambda_sterics=s.global_parameters.get('lambda_sterics', 1.0),
-                 ho_K=s.ho_K, ho_x0=s.ho_x0, ho_U0=s.ho_U0, pressure=self._pressure_md)
+                 lambda_electrostatics=s.global_parameters.get('lambda_electrostatics', 1.0), ho_K=s.ho_K, ho_x0=s.ho_x0, ho_U0=s.ho_U0, pressure=self._pressure_md)
         if getattr(s, 'alchemical_regions', None) is not None:   # each region's lambda_sterics<suffix>
             for n in s.lambda_sterics_names():
                 p[n] = s.global_parameters.get(n, 1.0)
@@ -748,7 +748,7 @@ class CompoundThermodynamicState(ThermodynamicState):
         p = super()._engine_parameters()
         for s in self._composable_states:
             for n, v in getattr(s, '_parameters', {}).items():
-                if v is not None and n.startswith('lambda_sterics'):   # (with a region's suffix, if any)
+                if v is not None and (n.startswith('lambda_sterics') or n == 'lambda_electrostatics'):   # (with a region's suffix, if any)
                     p[n] = v
         return p
 

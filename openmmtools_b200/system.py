@@ -141,6 +141,8 @@ class System:
         # -- alchemical modification (AbsoluteAlchemicalFactory)
         self.alchemical_atoms = None          # sorted tuple of atom indices, None = not alchemically modified
         self.annihilate_sterics = False
+        self.annihilate_electrostatics = True   # (molecules; the LJ fluid has no charges)
+        self.alchemical_obc2 = False            # (molecules in OBC2: the alchemical expression's own constants)
         self.softcore_alpha = 0.5
         self.softcore_a = 1.0
         self.softcore_b = 1.0
@@ -268,6 +270,9 @@ class System:
                 for a in (self.gb_radius, self.gb_scale):
                     h.update(np.asarray(a, dtype=np.float64).tobytes())
                 h.update(repr(tuple(float(v) for v in self.gb_parameters)).encode())
+            if self.is_alchemical:   # (other molecules keep their hash)
+                h.update(repr((self.alchemical_atoms, self.annihilate_sterics, self.annihilate_electrostatics,
+                               self.softcore_alpha, self.softcore_a, self.softcore_b, self.softcore_c)).encode())
         for f in getattr(self, 'forces', ()):   # a barostat's kind and scaled axes, not its pressure (systems without keep their hash)
             h.update(f._hash_key())
         return h.hexdigest()
@@ -279,3 +284,5 @@ class System:
         self.__dict__.update(d)
         self.__dict__.setdefault('alchemical_regions', None)
         self.__dict__.setdefault('forces', [])
+        self.__dict__.setdefault('annihilate_electrostatics', True)
+        self.__dict__.setdefault('alchemical_obc2', False)

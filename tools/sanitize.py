@@ -55,4 +55,18 @@ MBAR.from_history(e, np.arange(3, 40), np.r_[40, np.arange(40), 41], N_k).close(
 u = rng.normal(size=(5, 3 * 8192 + 5)) + np.array([-900.0, 0.0, 400.0, 800.0, 1700.0])[:, None] - 1.0e5
 MBAR(u, [0, 8192, 8192, 8197, 0]).close()
 e.close()
+# alchemical molecules (ALCH instantiations): OBC2 with a partial region, vacuum with the whole molecule -- Langevin,
+# HMC, Monte Carlo moves, FIRE, energy rows at sampled and unsampled states
+for cls, atoms in ((testsystems.TolueneImplicitOBC2, [0, 3, 9, 10]), (testsystems.TolueneVacuum, range(15))):
+    tol = cls()
+    amol = alchemy.AbsoluteAlchemicalFactory().create_alchemical_system(tol.system, alchemy.AlchemicalRegion(alchemical_atoms=atoms))
+    ats = states.create_thermodynamic_state_protocol(amol, {'lambda_electrostatics': [1.0, 0.5, 0.0, 0.0], 'lambda_sterics': [1.0, 1.0, 0.5, 0.0]},
+                                                     constants={'temperature': 300 * unit.kelvin},
+                                                     composable_states=alchemy.AlchemicalState.from_system(amol))
+    for mv in (mcmc.LangevinSplittingDynamicsMove(n_steps=10), mcmc.HMCMove(n_steps=3),
+               mcmc.SequenceMove([mcmc.MCDisplacementMove(displacement_sigma=0.01 * unit.nanometer, atom_subset=list(range(15))),
+                                  mcmc.MCRotationMove(atom_subset=list(range(15)))])):
+        ms = multistate.ReplicaExchangeSampler(mcmc_moves=mv, number_of_iterations=2, seed=3)
+        ms.create(ats, [states.SamplerState(tol.positions)], unsampled_thermodynamic_states=[ats[0], ats[-1]])
+        ms.minimize(max_iterations=20); ms.run()
 print('sanitize workload done')
