@@ -115,6 +115,83 @@ def test_oracle_forces_are_the_gradient_of_its_energy(name, annihilate):
             assert abs(F[a, c] - fd) <= 1e-5 * max(1.0, np.abs(F).max()), (a, c, F[a, c], fd)
 
 
+def _engulfed():
+    from alchemical_cases import make
+    from oracle.alchemical_molecule import AlchemicalMolecule
+    from oracle import implicit
+    s, x, asys = make('engulfed-methane-obc2')
+    x = x + np.random.default_rng(9).normal(0, 0.003, x.shape)
+    B, engulfed = implicit.Molecule(s).born_radii(x)
+    assert engulfed == 4 and np.all(B > 0)        # every (H, C) pair: sr_C - r > rt_H
+    return s, x, asys, AlchemicalMolecule(asys)
+
+
+@pytest.mark.parametrize('le', [0.0, 0.5, 1.0])
+def test_oracle_forces_are_the_gradient_of_its_energy_at_engulfed_pairs(le):
+    """The alchemical OBC2 expression's engulfment term C = 2 (1/rt_i - 1/L) step(sr_j - r - rt_i) and its force."""
+    _, x, _, m = _engulfed()
+    _, F = m.energy(x, 0.7, le, forces=True)
+    h = 1e-6
+    for a in range(x.shape[0]):
+        for c in range(3):
+            xp, xm = x.copy(), x.copy()
+            xp[a, c] += h; xm[a, c] -= h
+            fd = -(m.energy(xp, 0.7, le) - m.energy(xm, 0.7, le)) / (2 * h)
+            assert abs(F[a, c] - fd) <= 1e-6 * max(1.0, np.abs(F).max()), (a, c, F[a, c], fd)
+
+
+def test_engulfment_term_is_continuous_at_its_boundary_and_vanishes_without_engulfed_pairs():
+    """Moving one hydrogen along its bond through r = sr_C - rt_H, where C = 0 (L = rt_H): no jump in energy, forces the
+    gradient on both sides.  Stretched so that no pair is engulfed, the molecule at lambda 1 is the unmodified OBC2 model; at
+    its own geometry it is not (the term is on)."""
+    from oracle import implicit
+    s, x, asys, m = _engulfed()
+    rt, sr = s.gb_radius[1] - s.gb_parameters[3], s.gb_scale[0] * (s.gb_radius[0] - s.gb_parameters[3])
+    edge = sr - rt
+    u = (x[1] - x[0]) / np.linalg.norm(x[1] - x[0])
+    at = lambda r: np.concatenate([x[:1], [x[0] + r * u], x[2:]])
+    for le in (0.0, 0.5, 1.0):
+        Fmax = np.abs(m.energy(at(edge), 0.7, le, forces=True)[1]).max()
+        d = 1e-7
+        assert abs(m.energy(at(edge + d), 0.7, le) - m.energy(at(edge - d), 0.7, le)) <= 2 * d * Fmax * 1.01
+        for r in (edge - 2e-3, edge + 2e-3):
+            _, F = m.energy(at(r), 0.7, le, forces=True)
+            h = 1e-6
+            fd = -(m.energy(at(r + h), 0.7, le) - m.energy(at(r - h), 0.7, le)) / (2 * h)
+            assert abs(F[1] @ u - fd) <= 1e-6 * max(1.0, Fmax), (le, r, F[1] @ u, fd)
+    ref = _with_obc2_literals(s)
+    xs = x[0] + 1.8 * (x - x[0])           # hydrogens 0.196 nm out: past the boundary
+    assert implicit.Molecule(ref).born_radii(xs)[1] == 0
+    e0, e1 = implicit.Molecule(ref).energy(xs), m.energy(xs, 1.0, 1.0)
+    assert abs(e1 - e0) <= 1e-12 * abs(e0), (e1, e0)
+    assert abs(m.energy(x, 1.0, 1.0) - implicit.Molecule(ref).energy(x)) > 1.0
+
+
+def test_alchemical_cases_of_the_device_tests_build_and_reach_what_they_are_for():
+    """tests/alchemical_cases.py: each case has the region, the pair table and the flags its device tests rely on."""
+    import alchemical_cases as A
+    from oracle.alchemical_molecule import AlchemicalMolecule
+    got = {}
+    for name, swapped in A.variants():
+        s, x, asys = A.make(name, swapped)
+        got[name, swapped] = (asys, AlchemicalMolecule(asys))
+    a, m = got['decane-obc2-top', False]
+    assert a.n_particles == 32 and 31 in a.alchemical_atoms and a.alchemical_obc2
+    a, m = got['decane-all-annihilated', False]
+    n = a.n_particles
+    n_plain = n * (n - 1) // 2 - len(a.exclusions) - len(a.exceptions)
+    assert len(m.pairs) == n_plain + len(a.exceptions) and all(p[5] and p[6] for p in m.pairs)   # no plain pair
+    assert len(got['methane-obc1-carbon', False][1].pairs) == 0
+    assert got['ion-obc1', False][0].n_particles == 1
+    for c in ('torsion-probe-sc-c4', 'torsion-probe-sc-c12'):
+        a = got[c, False][0]
+        assert a.softcore_c != 6 and a.softcore_a == 2 and a.softcore_b == 2 and a.softcore_alpha == 0.3
+        assert len(got[c, False][1].pairs) == 2
+    # the swapped flags change which lambdas the alchemical/alchemical pairs follow
+    for c in A.SWAPPED:
+        assert [p[5:] for p in got[c, False][1].pairs] != [p[5:] for p in got[c, True][1].pairs], c
+
+
 def test_factory_records_the_region_and_the_lambdas():
     t, asys = _make('toluene-obc2-partial', annihilate_sterics=True, annihilate_electrostatics=False)
     assert asys.alchemical_atoms == (0, 3, 9, 10)
